@@ -2,6 +2,7 @@
 """bench.py -- EOT-samples/sec of the DorPatch hot loop (BASELINE.json metric).
 
     python bench.py [--gpus N --steps K --warmup W] [--impl native|reference] [--precision tf32|bf16|fp32]
+                    [--dump-outputs DIR]
 
 A "step" is one iteration of attack.py:184-342 of the reference over one batch: sample occlusion masks on the host,
 paste + expand (K1), ResNetV2-50x1-BiT forward + backward-to-input (K2), CW loss (K4), masked EOT gradient reduce
@@ -16,16 +17,21 @@ all-reduce of the patch gradient per step).
 
 Prints ONE JSON line (rank 0).  `value` = device-resident throughput, `e2e` = the same step through host buffers
 (H2D of x/mask/pattern + D2H of mask/pattern/losses every step, dp_attack_step_host), `roofline` = the hand-written K1
-kernel, timed on the variant and launch shape the step itself uses (one launch per step), against the measured HBM copy
-bandwidth: `frac` counts the algorithmic bytes (3 channels), `frac_physical` the bytes really moved (the fp32 / tf32 network
-input carries a zero pad channel for the library stem), `traffic` the DRAM bytes of that launch from the last ncu capture
-(profiles/k1_traffic.json); `kernels` = per-category device time / achieved byte and flop rates of one profiled step,
+kernel, timed on the variant and launch shape the step itself uses (one launch per step), against the HBM bandwidth:
+`frac` counts the algorithmic bytes (3 channels), `frac_physical` the bytes really moved (the fp32 / tf32 network
+input carries a zero pad channel for the library stem); `kernels` = per-category device time / achieved byte and flop rates of one profiled step,
 `host_ms_per_step` = host time the GPU waits for, `graph_replays` = CUDA-graph replays of dp_attack_grad so far,
 `cpu_baseline` = the oracle port of the reference's step on this box's host cores.  Extra legs (N=1 only; `legs`): the same step at bf16, configs[1] ("c2",
 32 x 16) at both precisions, the reference's default shape (1 image x 128 EOT), the stage-0 step of configs[4]
 ("c5": targeted, 10 % budget, density + group-lasso regularisers live), PatchCleanser evaluation throughput, and the
 scan-amortised throughput (the reference re-scans the whole mask universe every 100 steps, attack.py:187-190); the c3 / c2
 legs carry the K1 roofline of their own launch shape (`k1_roofline`).  `--config c5s0 --gpus 4` = configs[4] on 4 GPUs.
+
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step handed back to its caller as DIR/<name>.npy
+(float32): the per-sample losses and predictions, the per-image loss terms, the updated mask, and the patch gradient and
+updated pattern (a fixed, seeded sample of 2^22 elements where an array is larger).  The inputs are seeded and the library
+algorithms are picked by heuristic rather than by timing, so a run is reproducible and two builds run with the same arguments
+can be compared output for output.
 """
 import argparse
 import json
@@ -68,7 +74,7 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sus=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sus=1400.0, src="fallback (B200_PROFILING.md)")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sus=989.0, src="H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense bf16 at 700 W)")
 
 
 class ClockSampler(threading.Thread):
@@ -260,7 +266,7 @@ class Workload:
         t0 = time.perf_counter()
         idx, rects = self._samples(i)
         self.host_s += time.perf_counter() - t0               # host time the GPU waits for (sampling that was not ready, rectangle gather)
-        r = self.eng.attack_grad(self.x, self.mask, self.pattern, rects, self.y, self.crit, 0.1, 4.0, self.stage, self.G, S_total=self.S)
+        r = self.last = self.eng.attack_grad(self.x, self.mask, self.pattern, rects, self.y, self.crit, 0.1, 4.0, self.stage, self.G, S_total=self.S)
         t0 = time.perf_counter()
         lr, st_used, cg_used = self.finish(i, idx, r, self.G)
         self.host_s += time.perf_counter() - t0               # exchange + bookkeeping (the all-reduce runs under it)
@@ -286,6 +292,19 @@ class Workload:
             self.eng.attack_update(self.dx, self.dm, self.dp_, self.G, lr, st_used, cg_used, 1e-3, self.stage)
             self.hm.copy_(self.dm, non_blocking=True); self.hp.copy_(self.dp_, non_blocking=True)
             torch.cuda.synchronize()
+
+    def dump(self, out_dir, max_elems=1 << 22):
+        """The last step's results as float32 .npy files; arrays above max_elems keep a fixed, seeded sample of their elements."""
+        import torch
+        torch.cuda.synchronize()
+        os.makedirs(out_dir, exist_ok=True)
+        arrays = {k: self.last[k] for k in ("loss_adv", "preds", "loss_struc", "loss_density", "group_lasso", "l2")}
+        arrays.update(mask=self.mask, grad_adv=self.G, pattern=self.pattern)
+        for name, a in arrays.items():
+            a = (a.detach().float().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)).astype(np.float32).ravel()
+            if a.size > max_elems:
+                a = a[np.sort(np.random.RandomState(0).choice(a.size, max_elems, replace=False))]
+            np.save(os.path.join(out_dir, name + ".npy"), a)
 
     def io_bytes(self):
         B, S = self.B, self.S_loc
@@ -322,8 +341,11 @@ def run_native(args):
             for e in engines.values():                  # one engine's workspace at a time
                 e.close()
             engines.clear()
+            # autotune=False: cuDNN / cublasLt algorithms come from the libraries' heuristics, not from timing trials, so two
+            # runs with the same arguments compute the same outputs (timed selection flips between near-equal algorithms
+            # from run to run, and the sign steps turn their different roundings into different patches)
             e = Engine(img=IMG, precision=precision, chunk=args.chunk, max_images=max(shape_for(args.config, world)["B"], 64),
-                       device=local, autotune=True)
+                       device=local, autotune=False)
             e.load_state_dict(sd)
             engines[precision] = e
         return engines[precision]
@@ -350,7 +372,7 @@ def run_native(args):
 
     W, K = max(args.warmup, 3), args.steps
 
-    def measure(precision, config, K, e2e=True, sampler=None):
+    def measure(precision, config, K, e2e=True, sampler=None, dump=None):
         eng = engine(precision)
         wl = Workload(eng, config, world, rank, dev, dist if world > 1 else None)
         for i in range(W):
@@ -361,6 +383,8 @@ def run_native(args):
         wl.host_s = 0.0
         ms, launches = timed(eng, wl.step, K, W)
         clocks = sampler.stop() if sampler is not None else None
+        if dump and rank == 0:
+            wl.dump(dump)
         res = dict(value=wl.samples_per_step * K / (ms / 1e3), ms_per_step=ms / K, launches=int(launches), clocks=clocks, wl=wl, eng=eng,
                    host_ms=wl.host_s / K * 1e3, graph_replays=eng.graph_replays)
         if e2e:
@@ -383,7 +407,7 @@ def run_native(args):
         torch.cuda.profiler.stop()
         return
 
-    head = measure(args.precision, args.config, K, e2e=True, sampler=ClockSampler(local))
+    head = measure(args.precision, args.config, K, e2e=True, sampler=ClockSampler(local), dump=args.dump_outputs)
     wl, eng = head["wl"], head["eng"]
     h2d, d2h = wl.io_bytes()
     out = {
@@ -396,6 +420,7 @@ def run_native(args):
                 "d2h_bytes_per_step": d2h,
                 "path": "dp_attack_step_host (C ABI, host buffers)" if world == 1 else "pinned host -> H2D -> grad/allreduce/update -> D2H"},
         "engine": {"chunk": args.chunk, "c_pad": eng.c_pad, "device_bytes": eng.device_bytes,
+                   "algorithm_selection": "cuDNN / cublasLt heuristics (autotune off, so outputs are reproducible)",
                    "gn": os.environ.get("DORPATCH_GN", "v2"), "fused_gemm": os.environ.get("DORPATCH_FUSED_GEMM", "0")},
         "precision_note": "tf32 = fp32 storage + TF32 tensor-core convolutions, the reference's own GPU arithmetic (torch cudnn.allow_tf32 "
                           "default); bf16 legs are reported under `legs` and are backed by tests/test_gpu_attack_success.py",
@@ -505,18 +530,12 @@ def run_native(args):
         k1_ms_single = e0.elapsed_time(e1)
         img_in_launch = max(1, n_chunk // S_loc)
         alg_bytes = n_chunk * IMG * IMG * 3 * es + img_in_launch * 7 * IMG * IMG * 4
-        traffic, tnote = None, None
-        tpath = os.path.join(ROOT, "profiles", "k1_traffic.json")     # dram bytes of this launch from the last ncu --set full capture
-        if os.path.exists(tpath):
-            for tj in json.load(open(tpath)).get("entries", []):
-                if tj.get("samples") == n_chunk and tj.get("dtype") == args.precision:
-                    traffic, tnote = tj.get("dram_bytes"), tj.get("note")
         phys_bytes = n_chunk * IMG * IMG * eng.c_pad * es + img_in_launch * 7 * IMG * IMG * 4
         out["roofline"] = {"kernel": "expand_kernel<FUSED=1> (K1: paste + L2-scale + normalise + occlude, TMA bulk tiles), the in-step variant and launch shape (%d samples per launch)" % n_chunk,
                            "physical_bytes_per_launch": phys_bytes, "frac_physical": phys_bytes / k1_ms / 1e6 / pk["hbm"],
                            "physical_note": "bytes the launch really moves: the network input is [N,H,W,%d] (channel pad %d -> %d for the library stem)" % (eng.c_pad, 3, eng.c_pad) if eng.c_pad != 3 else "tight C=3 layout: physical == algorithmic",
                            "bound": "hbm", "achieved": alg_bytes / k1_ms / 1e6, "peak": pk["hbm"], "unit": "GB/s",
-                           "frac": alg_bytes / k1_ms / 1e6 / pk["hbm"], "traffic": traffic, "traffic_note": tnote,
+                           "frac": alg_bytes / k1_ms / 1e6 / pk["hbm"],
                            "ms": k1_ms, "ms_single_launch_event_pair": k1_ms_single, "samples_per_launch": n_chunk,
                            "timing": "CUDA events around 10 back-to-back launches rotating over %d output buffers (> L2 in total), median of 7" % n_rot,
                            "unoccluded_gbs": alg_bytes / k1_ms_clean / 1e6,
@@ -526,7 +545,7 @@ def run_native(args):
         del bufs
         out["roofline_step"] = {"bound": "tensor", "achieved": GFLOP_PER_SAMPLE * head["value"] / world / 1e3, "peak": pk["tf_sus"],
                                 "unit": "TFLOP/s", "frac": GFLOP_PER_SAMPLE * head["value"] / world / 1e3 / pk["tf_sus"],
-                                "note": "16.36 GFLOP (fwd+dgrad) per EOT sample x per-GPU samples/s vs sustained bf16 cuBLAS peak (TF32 peak is half of it)"}
+                                "note": "16.36 GFLOP (fwd+dgrad) per EOT sample x per-GPU samples/s vs the dense bf16 peak (TF32 peak is half of it)"}
         out["kernels"] = kern
         out["kernels_total_ms"] = ktot
         out["kernels_note"] = "one step profiled with CUDA events around every launch, chunks serialised on ONE lane; the timed steps overlap two lanes (two streams), so ms_per_step < kernels_total_ms"
@@ -631,6 +650,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-legs", action="store_true", help="skip the extra legs (bf16 / c2 / B=1 / stage 0)")
     ap.add_argument("--ncu", action="store_true", help="run W warm-up steps, then ONE step inside cudaProfilerStart/Stop, and exit")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's outputs as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,6 +1,6 @@
-"""DorPatch patch generation on the native B200 engine -- host control flow.
+"""DorPatch patch generation on the native H100 engine -- host control flow.
 
-Drop-in for /root/reference/attack.py: ``DorPatch().generate(...)`` keeps the reference's
+Drop-in for reference attack.py: ``DorPatch().generate(...)`` keeps the reference's
 signature (attack.py:51-53), side effects (prints, stage-0 artefacts in the parent directory,
 RNG consumption) and return value.  Everything numeric in the hot loop (attack.py:184-247,
 332-342) runs in libdorpatch.so through ``dorpatch_b200.engine.Engine``; what stays here is
@@ -271,7 +271,7 @@ class DorPatch(object):
             raise NotImplementedError("dropout=%r (the reference's dropout=0 path is degenerate)" % (dropout,))
         net = unwrap_native(model)
         if not x.is_cuda:
-            raise RuntimeError("DorPatch.generate needs CUDA tensors: the hot loop exists only as native sm_100a kernels")
+            raise RuntimeError("DorPatch.generate needs CUDA tensors: the hot loop exists only as native sm_90a kernels")
         x = x.contiguous().float()
         B, _, H, W = x.shape
         eng = net.engine(W, max_images=B)

@@ -1,4 +1,4 @@
-"""Build libdorpatch.so in-tree with nvcc for sm_100a (B200).
+"""Build libdorpatch.so in-tree with nvcc for sm_90a (H100).
 
     python -m dorpatch_b200.build [--force]
 
@@ -16,7 +16,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libdorpatch.so")
 SOURCES = ["kernels_net.cu", "kernels_patch.cu", "kernels_stem.cu", "kernels_gemm.cu", "engine.cu"]
 HEADERS = ["common.cuh", "kernels.h", os.path.join("..", "..", "include", "dorpatch.h")]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _site_nvidia():

@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the DorPatch sm_100a kernels.
+// common.cuh -- shared device helpers for the DorPatch sm_90a kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

@@ -91,7 +91,7 @@ struct Block {
   // saved tensors / stats for backward (device, per chunk)
   void* h1 = nullptr; void* h2 = nullptr; void* out = nullptr;
   float* st1 = nullptr; float* st2 = nullptr; float* st3 = nullptr;
-  void* c1p = nullptr; void* c3p = nullptr;   // conv1 / conv3 weights as tcgen05 operand tiles (DORPATCH_FUSED_GEMM=1)
+  void* c1p = nullptr; void* c3p = nullptr;   // conv1 / conv3 weights as wgmma operand tiles (DORPATCH_FUSED_GEMM=1)
 };
 
 struct CudnnPlan {
@@ -116,10 +116,10 @@ struct dp_engine {
   int Cp = 4;               // channels per pixel of the network INPUT (3 = tight, own stem kernel)
   int Cpd = 4;              // channels per pixel of d(input) produced by the library dgrad (4 fp32 / 8 bf16)
   bool own_stem = false;    // bf16: hand-written tensor-core stem forward on the tight C=3 layout
-  bool fused_gemm = false;  // opt-in (DORPATCH_FUSED_GEMM=1, bf16): GN+ReLU applied inside the tcgen05 1x1-conv GEMM of kernels_gemm.cu
+  bool fused_gemm = false;  // opt-in (DORPATCH_FUSED_GEMM=1, bf16): GN+ReLU applied inside the wgmma 1x1-conv GEMM of kernels_gemm.cu
   void* stem_w_kn = nullptr;
   int H = 224, K = 1000, chunk = 64;
-  int num_sms = 148;
+  int num_sms = 132;
   cudnnHandle_t cudnn = nullptr;
   cublasLtHandle_t lt = nullptr;
   cudnnDataType_t cudnn_dt = CUDNN_DATA_FLOAT;
@@ -271,8 +271,8 @@ struct dp_engine {
     CUDA_OK(cudaMallocHost((void**)&pin, pin_bytes));
   }
   // K1 for the WHOLE step in one launch (all B*S samples into one buffer, the chunks then read their slices): the launch
-  // shape of one classifier chunk (16 images x 28 row tiles) is too small to fill 148 SMs for more than one ragged wave
-  // (in-step 0.49-0.55 of HBM peak against 0.69 for a 512-sample launch, profiles/README.md).  Bounded by
+  // shape of one classifier chunk (16 images x 28 row tiles) is too small to fill 132 SMs for more than one ragged wave
+  // (a 512-sample launch reaches a larger share of the HBM peak).  Bounded by
   // DORPATCH_K1_WHOLE_MB (default 4096; 0 = one launch per chunk as in round 1).
   void* net_in_all = nullptr;
   size_t net_in_all_cap = 0, k1_whole_max = (size_t)4096 << 20;
@@ -669,7 +669,7 @@ struct dp_engine {
     int lid = 1;
     for (auto& b : blocks) {
       const int pin_ = b.hin * b.hin, pout = b.hout * b.hout;
-      // opt-in: statistics pass + tcgen05 GEMM that normalises its A operand on the way into shared memory
+      // opt-in: statistics pass + wgmma GEMM that normalises its A operand on the way into shared memory
       // (the relu(gn(.)) tensors of norm1 / norm3 are never written); blocks with a downsample branch keep norm1.
       const bool fuse1 = fused_gemm && !b.has_ds && dp::gn_gemm_supported(pin_, b.cin, b.mid);
       const bool fuse3 = fused_gemm && dp::gn_gemm_supported(pout, b.mid, b.cout);
@@ -848,7 +848,7 @@ int32_t dp_engine_create(const dp_config* cfg, dp_engine** out) {
   CUDA_OK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CUDA_OK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major < 10) fail("device %d is sm_%d%d; this engine is built for sm_100a (B200) only", cfg->device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) fail("device %d is sm_%d%d; this engine is built for sm_90a (H100) only", cfg->device, prop.major, prop.minor);
   dp_engine* e = new dp_engine();
   try {
     e->cfg = *cfg;
@@ -864,7 +864,7 @@ int32_t dp_engine_create(const dp_config* cfg, dp_engine** out) {
     const char* sb_env = getenv("DORPATCH_STEM_BWD");
     e->fused_stem_bwd = e->own_stem && !(sb_env && strcmp(sb_env, "cudnn") == 0);
     const char* fg_env = getenv("DORPATCH_FUSED_GEMM");
-    e->fused_gemm = e->bf16 && fg_env && atoi(fg_env) != 0;   // validated on hardware (tests/test_gpu_ops.py, test_gpu_fused_gemm.py) but 2x slower than cublasLt + GroupNorm: off unless asked for
+    e->fused_gemm = e->bf16 && fg_env && atoi(fg_env) != 0;   // validated (tests/test_gpu_ops.py, test_gpu_fused_gemm.py) but slower than cublasLt + GroupNorm: off unless asked for
     if (const char* g_env = getenv("DORPATCH_GRAPH")) e->graphs_on = atoi(g_env) != 0;
     if (const char* k_env = getenv("DORPATCH_K1_WHOLE_MB")) e->k1_whole_max = (size_t)std::max(0, atoi(k_env)) << 20;
     const char* pb_env = getenv("DORPATCH_POOL_BWD");
@@ -1447,7 +1447,7 @@ int32_t dp_debug_gn_gemm(dp_engine* e, const void* x, const void* w_nk, const fl
   if (!e) fail("null engine");
   CUDA_OK(cudaSetDevice(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  if (!dp::gn_gemm_supported(P, K, Nout)) fail("dp_debug_gn_gemm: shape P=%d K=%d Nout=%d not supported by the tcgen05 kernel", P, K, Nout);
+  if (!dp::gn_gemm_supported(P, K, Nout)) fail("dp_debug_gn_gemm: shape P=%d K=%d Nout=%d not supported by the wgmma kernel", P, K, Nout);
   void* packed = nullptr;
   CUDA_OK(cudaMalloc(&packed, (size_t)Nout * K * 2));
   dp::launch_gn_gemm_pack(w_nk, packed, Nout, K, st);
@@ -1467,7 +1467,7 @@ int32_t dp_debug_gn(dp_engine* e, const void* x, const void* dy, const void* add
   CUDA_OK(cudaSetDevice(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   if (N > e->chunk) fail("dp_debug_gn: N=%d exceeds chunk=%d (statistics scratch)", N, e->chunk);
-  if (y == nullptr) {   // statistics only: the pass in front of the tcgen05 GEMM / the classifier head
+  if (y == nullptr) {   // statistics only: the pass in front of the wgmma GEMM / the classifier head
     dp::launch_gn_stats(x, e->gn_partial, stats, N, P, C, e->bf16, st); KERNEL_OK();
     e->launches += 2;
     return 0;

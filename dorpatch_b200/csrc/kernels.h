@@ -1,4 +1,4 @@
-// kernels.h -- host-side launchers of the hand-written sm_100a kernels.
+// kernels.h -- host-side launchers of the hand-written sm_90a kernels.
 // Activation tensors are NHWC ("[N, P=H*W, C]"), element type fp32 or bf16 (`bf16` flag).
 #pragma once
 #include <cuda_runtime.h>
@@ -59,7 +59,7 @@ void launch_stem_bwd_reduce(const void* dY, const void* w_krsc, int cin_pad, con
 void launch_stem_bwd_pool_reduce(const void* dpool, const int8_t* amax, const void* w_krsc, int cin_pad, const int16_t* rects,
                                  float* G, int B, int S, int n0, int n, int H, int W, cudaStream_t st);
 
-// ---- opt-in: GroupNorm+ReLU applied in the prologue of a tcgen05 1x1-convolution GEMM (kernels_gemm.cu, bf16)
+// ---- opt-in: GroupNorm+ReLU applied in the prologue of a wgmma 1x1-convolution GEMM (kernels_gemm.cu, bf16)
 // out[m,n] = sum_k relu(gn(x))[m,k] * W[n,k] (+ shortcut[m,n]); `stats` from launch_gn_stats on x.
 bool gn_gemm_supported(int P, int K, int Nout);
 void launch_gn_gemm_pack(const void* w_nk, void* w_packed, int Nout, int K, cudaStream_t st);

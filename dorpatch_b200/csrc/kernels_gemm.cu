@@ -1,5 +1,5 @@
 // kernels_gemm.cu -- 1x1 convolution with the GroupNorm(32)+ReLU of its INPUT applied on the way into shared
-// memory, on the 5th-generation tensor cores (tcgen05.mma, fp32 accumulators in TMEM).
+// memory, on the Hopper warpgroup tensor cores (wgmma.mma_async, fp32 accumulators in registers).
 //
 //   D[m, n] = sum_k relu(sa[s(m), k] * X[m, k] + sb[s(m), k]) * W[n, k]   (+ R[m, n])
 //
@@ -9,25 +9,20 @@
 //   The normalised activation tensor y = relu(gn(x)) is never written to HBM (SURVEY 8d: "tensor-core bound
 //   only if GN/ReLU are fused"); reference: timm PreActBottleneck norm1->conv1 / norm3->conv3 (SURVEY App. B).
 //
-// STATUS (end of round 2): opt-in (DORPATCH_FUSED_GEMM=1).  Validated on B200 -- every fused layer shape within one bf16 ulp of an
-// fp32 restatement on the same rounded operands (tests/test_gpu_ops.py::test_tcgen05_gn_gemm_vs_fp32), the whole network as
-// accurate against the fp32 engine as the default bf16 path (tests/test_gpu_fused_gemm.py).  It
-// is NOT the default: 9.6 ms per 512-sample step against 3.25 ms for cublasLt on the same layers (profiles/r02_gemmbench.txt;
-// cublasLt runs these HBM-bound GEMMs at 0.8 of the copy peak), so the fusion (at best 5.7 % of the step) does not pay yet.
-// The measured gap is the A-operand path below: register-staged loads are issued one k block ahead of their use.
-// The two descriptor encodings below were compared bit for bit with cute::UMMA::SmemDescriptor / InstrDescriptor
-// filled field by field (host program against the vendored CUTLASS headers).
+// STATUS: opt-in (DORPATCH_FUSED_GEMM=1).  Checked per fused layer shape against an fp32 restatement on the same
+// rounded operands (tests/test_gpu_ops.py::test_tcgen05_gn_gemm_vs_fp32, named after the
+// kernel's first, tcgen05 version) and, as a whole network, against the fp32
+// engine (tests/test_gpu_fused_gemm.py).  It is not the default path.
 //
-// Structure (one 128 x BN output tile per CTA, 192 threads):
-//   warps 0-3  A producers: 16-byte global loads of the raw x tile (8 in flight per thread), scale / shift /
-//              ReLU in registers, st.shared into the canonical K-major no-swizzle core-matrix layout
-//              (8 rows x 16 B, conflict-free: the 8 lanes of a store phase write 8 consecutive rows), then
-//              fence.proxy.async + mbarrier arrive; afterwards the same warps run the epilogue
-//              (tcgen05.ld 32x32b: warp w owns TMEM lanes 32w..32w+31 = tile rows), + shortcut, bf16 stores.
-//   warp 4     allocates TMEM, one lane issues 4 x tcgen05.mma (K = 16 each) per 64-wide k block and
-//              tcgen05.commit's the stage back to the producers / the accumulator to the epilogue.
-//   warp 5     one lane streams the pre-packed weight tiles (already in the canonical layout) with
-//              cp.async.bulk, completing on the same per-stage "full" mbarrier.
+// Structure (one 128 x BN output tile per CTA, 256 threads = two warpgroups, two shared-memory stages):
+//   every thread  16-byte global loads of the raw x tile and of the pre-packed weight tile for k block kb + 1 are
+//                 issued while the wgmma of k block kb runs; scale / shift / ReLU in registers, st.shared into the
+//                 canonical K-major no-swizzle core-matrix layout (8 rows x 16 B; chunk q of a tile lands at byte
+//                 16 q, so the 8 lanes of a store phase write 8 consecutive rows, conflict-free), then
+//                 fence.proxy.async + __syncthreads.
+//   warpgroup g   4 x wgmma.m64nBNk16 per 64-wide k block on tile rows 64g..64g+63, one commit group per k block;
+//                 wait_group 1 keeps one k block in flight, so stage kb % 2 is free again at k block kb + 2.
+//   epilogue      accumulator fragments (+ shortcut) -> bf16 stores straight from registers.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -37,79 +32,63 @@
 namespace dp {
 namespace tc {
 
-constexpr int BM = 128, BK = 64, STAGES = 3;
-constexpr int THREADS = 192, PRODUCERS = 128;
+constexpr int BM = 128, BK = 64, STAGES = 2;
+constexpr int THREADS = 256;
 constexpr int A_STAGE = BM * BK * 2;                 // 16 KB
-constexpr int HDR = 1024, TAB = 2 * 4 * BK * 8;      // barriers | 2 x [4 samples][64 ch] float2
+constexpr int TAB = 2 * 4 * BK * 8;                  // 2 x [4 samples][64 ch] float2
 constexpr int MAX_TILE_SAMPLES = 4;
 
 __host__ __device__ constexpr int b_stage(int bn) { return bn * BK * 2; }
-__host__ __device__ constexpr size_t smem_bytes(int bn) { return HDR + TAB + (size_t)STAGES * (A_STAGE + b_stage(bn)); }
+__host__ __device__ constexpr size_t smem_bytes(int bn) { return TAB + (size_t)STAGES * (A_STAGE + b_stage(bn)); }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  }
-}
-__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src),
-               "r"(bytes), "r"(bar)
-               : "memory");
-}
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// Shared-memory matrix descriptor, K-major, no swizzle (cute::UMMA::SmemDescriptor): 8-row x 16-byte core
-// matrices; LBO = byte distance between the two core matrices of one K = 16 step, SBO = between 8-row groups.
+// wgmma shared-memory matrix descriptor, K-major, no swizzle: 8-row x 16-byte core matrices; LBO = byte distance
+// between the two core matrices of one K = 16 step, SBO = between 8-row groups.
 __device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((addr >> 4) & 0x3fffu);            // start address        bits [ 0,14)
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16; // leading byte offset  bits [16,30)
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32; // stride byte offset   bits [32,46)
-  d |= (uint64_t)1 << 46;                            // descriptor version 1 (sm_100)
-  return d;                                          // base offset 0, layout type 0 = SWIZZLE_NONE
+  return d;                                          // base offset 0, layout type 0 = no swizzle
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D fp32, A and B bf16, both K-major, M = 128, N = bn.
-__host__ __device__ constexpr uint32_t instr_desc(int bn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(bn >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-__device__ __forceinline__ void mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D (+)= A * B^T, A 64 x 16 and B BN x 16, both K-major bf16 in shared memory; d[] the m64nBN fp32 fragment
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
+      "%30,%31}, %32, %33, 1, 1, 1, 0, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),
+        "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]),
+        "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc));
 }
-__device__ __forceinline__ void mma_commit(uint32_t bar) {   // arrives on `bar` when every MMA issued so far has completed
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
+__device__ __forceinline__ void wgmma_n128(float* d, uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
+      "%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,"
+      "%58,%59,%60,%61,%62,%63}, %64, %65, 1, 1, 1, 0, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),
+        "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]),
+        "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+        "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]),
+        "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]),
+        "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),
+        "+f"(d[63])
+      : "l"(adesc), "l"(bdesc));
+}
+template <int BN> __device__ __forceinline__ void wgmma_bn(float* d, uint64_t adesc, uint64_t bdesc) {
+  if constexpr (BN == 64) wgmma_n64(d, adesc, bdesc);
+  else wgmma_n128(d, adesc, bdesc);
 }
 
 __device__ __forceinline__ uint32_t pack2(float a, float b) {
@@ -131,192 +110,117 @@ struct GemmParams {
 };
 
 template <int BN>
-__global__ void __launch_bounds__(THREADS, 2) gn_gemm_fwd_kernel(GemmParams p) {
+__global__ void __launch_bounds__(THREADS, 1) gn_gemm_fwd_kernel(GemmParams p) {
+  constexpr int A_CHUNKS = A_STAGE / 16 / THREADS;        // 4 16-byte chunks per thread
+  constexpr int B_CHUNKS = b_stage(BN) / 16 / THREADS;    // 2 (BN = 64) or 4 (BN = 128)
   extern __shared__ __align__(1024) unsigned char smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int t = threadIdx.x, wg = t >> 7, warp = t >> 5, lane = t & 31;
   const int n_tiles = p.Nout / BN;
   const int nt = blockIdx.x % n_tiles, mt = blockIdx.x / n_tiles;   // CTAs sharing an x tile are adjacent
   const int m0 = mt * BM, n0 = nt * BN, KB = p.K / BK;
 
-  const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar_full = sbase, bar_empty = sbase + 8 * STAGES, bar_acc = sbase + 16 * STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + 16 * STAGES + 8);
-  float2* tab = reinterpret_cast<float2*>(smem + HDR);
-  const uint32_t a_base = sbase + HDR + TAB, b_base = a_base + STAGES * A_STAGE;
+  float2* tab = reinterpret_cast<float2*>(smem);
+  const uint32_t a_base = smem_u32(smem + TAB), b_base = a_base + STAGES * A_STAGE;
+  uint4* a_st = reinterpret_cast<uint4*>(smem + TAB);
+  uint4* b_st = reinterpret_cast<uint4*>(smem + TAB + STAGES * A_STAGE);
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, PRODUCERS + 1); mbar_init(bar_empty + 8 * s, 1); }
-    mbar_init(bar_acc, 1);
-    fence_mbar_init();
-    fence_proxy_async();
-  }
-  if (warp == 4) {   // TMEM: BN fp32 columns x 128 lanes
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(BN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
+  const int n_first = m0 / p.P;
+  const int b1 = (n_first + 1) * p.P - m0, b2 = b1 + p.P, b3 = b2 + p.P;   // tile rows where the sample changes
+  const int cpg = p.K / GN_GROUPS;
+  // scale / shift table entry of this thread: sample n_first + ts, channel tc of the k block
+  const int ts = t >> 6, tcol = t & 63;
+  const int tn = min(n_first + ts, p.N - 1);
+  const __nv_bfloat16* wt = p.Wp + (size_t)nt * KB * BN * BK;
 
-  if (warp < 4) {
-    // ===================== A producers =====================
-    const int n_first = m0 / p.P;
-    const int b1 = (n_first + 1) * p.P - m0, b2 = b1 + p.P, b3 = b2 + p.P;   // tile rows where the sample changes
-    const int cpg = p.K / GN_GROUPS;
-    const int rin = lane & 7, kc0 = (lane >> 3) * 2;                          // row in the 8-row group, first 16-byte chunk
-    const int t = threadIdx.x;
-    for (int kb = 0; kb < KB; ++kb) {
-      const int stage = kb % STAGES;
-      const uint32_t phase = (uint32_t)(kb / STAGES) & 1u;
-      const int k0 = kb * BK;
-      // global loads first (independent of the stage being free): 4 row groups x 2 chunks per thread
-      uint4 v[8];
+  uint4 va[A_CHUNKS], vb[B_CHUNKS];
+  float mean_r, rstd_r, gam_r, bet_r;
+  auto load = [&](int kb) {
+    const int k0 = kb * BK;
+#pragma unroll
+    for (int i = 0; i < A_CHUNKS; ++i) {
+      const int q = i * THREADS + t, row = m0 + (q >> 6) * 8 + (q & 7), kc = (q >> 3) & 7;
+      va[i] = row < p.M ? __ldg(reinterpret_cast<const uint4*>(p.X + (size_t)row * p.K + k0 + kc * 8)) : make_uint4(0u, 0u, 0u, 0u);
+    }
+    const uint4* wsrc = reinterpret_cast<const uint4*>(wt + (size_t)kb * BN * BK);
+#pragma unroll
+    for (int i = 0; i < B_CHUNKS; ++i) vb[i] = __ldg(wsrc + i * THREADS + t);
+    const int g = (k0 + tcol) / cpg;
+    mean_r = __ldg(p.stats + ((size_t)tn * GN_GROUPS + g) * 2);
+    rstd_r = __ldg(p.stats + ((size_t)tn * GN_GROUPS + g) * 2 + 1);
+    gam_r = __ldg(p.gamma + k0 + tcol);
+    bet_r = __ldg(p.beta + k0 + tcol);
+  };
+
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+
+  load(0);
+  for (int kb = 0; kb < KB; ++kb) {
+    const int stage = kb % STAGES;
+    {
+      const float sa = rstd_r * gam_r;
+      tab[(stage * MAX_TILE_SAMPLES + ts) * BK + tcol] = make_float2(sa, bet_r - mean_r * sa);
+    }
+    // the table is visible, and both warpgroups have retired the wgmma of k block kb - 2 (wait_group 1 below)
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < A_CHUNKS; ++i) {
+      const int q = i * THREADS + t, r = (q >> 6) * 8 + (q & 7), kc = (q >> 3) & 7;
+      const int s = (r >= b1) + (r >= b2) + (r >= b3);
+      const float4* tp = reinterpret_cast<const float4*>(tab + (stage * MAX_TILE_SAMPLES + s) * BK + kc * 8);
+      const uint32_t w[4] = {va[i].x, va[i].y, va[i].z, va[i].w};
+      const bool live = m0 + r < p.M;
+      uint32_t o[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const int row = m0 + (warp * 4 + j) * 8 + rin;
-        const __nv_bfloat16* src = p.X + (size_t)row * p.K + k0 + kc0 * 8;
-#pragma unroll
-        for (int c = 0; c < 2; ++c)
-          v[j * 2 + c] = row < p.M ? __ldg(reinterpret_cast<const uint4*>(src) + c) : make_uint4(0u, 0u, 0u, 0u);
+        const float4 ss = tp[j];                                            // (sa, sb) of channels 2j, 2j + 1
+        const float2 f = unpack2(w[j]);
+        o[j] = live ? pack2(fmaxf(fmaf(ss.x, f.x, ss.y), 0.f), fmaxf(fmaf(ss.z, f.y, ss.w), 0.f)) : 0u;
       }
-      // scale / shift of this k block for the <= 4 samples the tile touches
-      {
-        const int s = t >> 5, c = (t & 31) * 2;
-        int n = n_first + s;
-        n = n < p.N ? n : p.N - 1;
-        const int g = (k0 + c) / cpg;                                         // cpg >= 2: both channels in one group
-        const float mean = __ldg(p.stats + ((size_t)n * GN_GROUPS + g) * 2), rstd = __ldg(p.stats + ((size_t)n * GN_GROUPS + g) * 2 + 1);
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const float sa = rstd * __ldg(p.gamma + k0 + c + i);
-          tab[((kb & 1) * MAX_TILE_SAMPLES + s) * BK + c + i] = make_float2(sa, __ldg(p.beta + k0 + c + i) - mean * sa);
-        }
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");                          // table visible to the 128 producers
-      mbar_wait(bar_empty + 8 * stage, phase ^ 1u);                           // the MMAs that read this stage are done
-      int cur = -1;
-      float sa[16], sb[16];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int r = (warp * 4 + j) * 8 + rin;
-        const int s = (r >= b1) + (r >= b2) + (r >= b3);
-        if (s != cur) {
-          const float4* tp = reinterpret_cast<const float4*>(tab + ((kb & 1) * MAX_TILE_SAMPLES + s) * BK + kc0 * 8);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { const float4 q = tp[i]; sa[2 * i] = q.x; sb[2 * i] = q.y; sa[2 * i + 1] = q.z; sb[2 * i + 1] = q.w; }
-          cur = s;
-        }
-        const bool live = m0 + r < p.M;
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const uint4 in = v[j * 2 + c];
-          const uint32_t w[4] = {in.x, in.y, in.z, in.w};
-          uint32_t o[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float2 f = unpack2(w[i]);
-            const float y0 = fmaxf(fmaf(sa[c * 8 + 2 * i], f.x, sb[c * 8 + 2 * i]), 0.f);
-            const float y1 = fmaxf(fmaf(sa[c * 8 + 2 * i + 1], f.y, sb[c * 8 + 2 * i + 1]), 0.f);
-            o[i] = live ? pack2(y0, y1) : 0u;
-          }
-          const uint32_t dst = a_base + stage * A_STAGE + (warp * 4 + j) * 1024 + (kc0 + c) * 128 + rin * 16;
-          asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(dst), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
-        }
-      }
-      fence_proxy_async();                                                    // generic-proxy stores -> visible to the tensor core
-      mbar_arrive(bar_full + 8 * stage);
+      a_st[stage * (A_STAGE / 16) + q] = make_uint4(o[0], o[1], o[2], o[3]);
     }
-    // ===================== epilogue =====================
-    // warp w owns TMEM lanes 32w..32w+31 = tile rows; a thread handles one output row, 64 columns per trip: the 8
-    // shortcut loads of a trip are issued together (and the first trip's before the accumulator wait), so the row's
-    // latency is paid once per 64 columns instead of once per 16
-    const int m = m0 + warp * 32 + lane;
-    const bool live = m < p.M;
-    __nv_bfloat16* drow = p.D + (size_t)m * p.Nout + n0;
-    const __nv_bfloat16* rrow = (p.R && live) ? p.R + (size_t)m * p.Nout + n0 : nullptr;
-    uint4 rq[8];
-    if (rrow != nullptr) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) rq[i] = *(reinterpret_cast<const uint4*>(rrow) + i);   // plain loads: R may be D (in-place shortcut)
+    for (int i = 0; i < B_CHUNKS; ++i) b_st[stage * (b_stage(BN) / 16) + i * THREADS + t] = vb[i];
+    fence_proxy_async();                                                    // generic-proxy stores -> visible to wgmma
+    __syncthreads();
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < BK / 16; ++ks) {
+      const uint64_t ad = smem_desc(a_base + stage * A_STAGE + wg * (A_STAGE / 2) + ks * 256, 128, 1024);
+      const uint64_t bd = smem_desc(b_base + stage * b_stage(BN) + ks * 256, 128, 1024);
+      wgmma_bn<BN>(acc, ad, bd);
     }
-    mbar_wait(bar_acc, 0u);
-    tc_fence_after();
-#pragma unroll 1
-    for (int h0 = 0; h0 < BN; h0 += 64) {
-      if (h0 > 0 && rrow != nullptr) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) rq[i] = *(reinterpret_cast<const uint4*>(rrow + h0) + i);
-      }
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        uint32_t acc[16];
-        tmem_ld16(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)(h0 + q * 16), acc);
-        if (live) {
-          float f[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(acc[i]);
-          if (rrow != nullptr) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const uint4 qv = rq[q * 2 + h];
-              const uint32_t w[4] = {qv.x, qv.y, qv.z, qv.w};
-#pragma unroll
-              for (int i = 0; i < 4; ++i) { const float2 e = unpack2(w[i]); f[h * 8 + 2 * i] += e.x; f[h * 8 + 2 * i + 1] += e.y; }
-            }
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint4 o;
-            o.x = pack2(f[h * 8 + 0], f[h * 8 + 1]); o.y = pack2(f[h * 8 + 2], f[h * 8 + 3]);
-            o.z = pack2(f[h * 8 + 4], f[h * 8 + 5]); o.w = pack2(f[h * 8 + 6], f[h * 8 + 7]);
-            *(reinterpret_cast<uint4*>(drow + h0 + q * 16) + h) = o;
-          }
-        }
-      }
-    }
-  } else if (warp == 4) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t IDESC = instr_desc(BN);
-    for (int kb = 0; kb < KB; ++kb) {
-      const int stage = kb % STAGES;
-      const uint32_t phase = (uint32_t)(kb / STAGES) & 1u;
-      mbar_wait(bar_full + 8 * stage, phase);
-      tc_fence_after();
-      if (lane == 0) {
-#pragma unroll
-        for (int ks = 0; ks < BK / 16; ++ks) {
-          const uint64_t ad = smem_desc(a_base + stage * A_STAGE + ks * 256, 128, 1024);
-          const uint64_t bd = smem_desc(b_base + stage * b_stage(BN) + ks * 256, 128, 1024);
-          mma_bf16(tmem, ad, bd, IDESC, (uint32_t)((kb | ks) != 0));
-        }
-        mma_commit(bar_empty + 8 * stage);          // stage reusable once these MMAs have read it
-        if (kb == KB - 1) mma_commit(bar_acc);       // accumulator complete
-      }
-      __syncwarp();
-    }
-  } else if (lane == 0) {
-    // ===================== weight-tile loader =====================
-    const __nv_bfloat16* wt = p.Wp + (size_t)nt * KB * BN * BK;
-    for (int kb = 0; kb < KB; ++kb) {
-      const int stage = kb % STAGES;
-      const uint32_t phase = (uint32_t)(kb / STAGES) & 1u;
-      mbar_wait(bar_empty + 8 * stage, phase ^ 1u);
-      mbar_expect_tx(bar_full + 8 * stage, (uint32_t)b_stage(BN));
-      bulk_load(b_base + stage * b_stage(BN), wt + (size_t)kb * BN * BK, (uint32_t)b_stage(BN), bar_full + 8 * stage);
-    }
+    wgmma_commit();
+    if (kb + 1 < KB) load(kb + 1);                                          // in flight under this k block's wgmma
+    wgmma_wait<1>();
   }
+  wgmma_wait<0>();
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(BN) : "memory");
+  // ===================== epilogue =====================
+  // m64nBN fragment: acc[4 j + e] is row 16 w + lane / 4 + 8 (e / 2), column 8 j + 2 (lane % 4) + e % 2
+  const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int c0 = n0 + 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = r0 + 8 * h;
+    if (m >= p.M) continue;
+    __nv_bfloat16* drow = p.D + (size_t)m * p.Nout + c0;
+    const __nv_bfloat16* rrow = p.R ? p.R + (size_t)m * p.Nout + c0 : nullptr;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+      if (rrow != nullptr) {                                                // plain load: R may be D (in-place shortcut)
+        const float2 e = unpack2(*reinterpret_cast<const uint32_t*>(rrow + 8 * j));
+        x0 += e.x; x1 += e.y;
+      }
+      *reinterpret_cast<uint32_t*>(drow + 8 * j) = pack2(x0, x1);
+    }
   }
 }
 
 // W [Nout][K] bf16 row-major -> tiles [Nout/BN][K/64] of BN x 64 in the canonical K-major core-matrix layout
-// (element (r, kk) at (r/8)*512 + (kk/8)*64 + (r%8)*8 + kk%8), so that one cp.async.bulk lands a ready B operand.
+// (element (r, kk) at (r/8)*512 + (kk/8)*64 + (r%8)*8 + kk%8), so that a k block's B operand is one contiguous, ready-laid-out tile.
 __global__ void pack_w_kernel(const __nv_bfloat16* __restrict__ w, __nv_bfloat16* __restrict__ out, int Nout, int K, int BN) {
   const size_t total = (size_t)Nout * K;
   const int KB = K / BK;
@@ -329,7 +233,7 @@ __global__ void pack_w_kernel(const __nv_bfloat16* __restrict__ w, __nv_bfloat16
 
 }  // namespace tc
 
-// BN <= 128: 101 KB of shared memory and 128 TMEM columns per CTA -> two CTAs per SM, one's epilogue under the other's main loop
+// BN <= 128: 68 KB of shared memory per CTA
 int gn_gemm_tile_n(int Nout) { return Nout >= 128 ? 128 : Nout; }
 
 bool gn_gemm_supported(int P, int K, int Nout) {

@@ -1,9 +1,9 @@
-// kernels_net.cu -- hand-written sm_100a kernels around the classifier's tensor-core
+// kernels_net.cu -- hand-written sm_90a kernels around the classifier's tensor-core
 // convolutions: weight standardisation, GroupNorm(32)+ReLU forward / backward-to-input,
 // pad+maxpool, head (GN+ReLU+avgpool, fc), layout packers.  All activations NHWC.
 //
 // Restates the third-party classifier the reference uses (timm 0.6.7
-// resnetv2_50x1_bit_distilled, /root/reference/utils.py:51-58): StdConv2d eps=1e-8,
+// resnetv2_50x1_bit_distilled, reference utils.py:51-58): StdConv2d eps=1e-8,
 // GroupNormAct(32 groups, eps=1e-5, ReLU), stem 'fixed' (ConstantPad2d(1,0)+MaxPool 3x3/2).
 // These kernels are HBM-bound; every one is a coalesced 16-byte-vector pass.
 #include <cooperative_groups.h>
@@ -872,8 +872,8 @@ __global__ void __launch_bounds__(gnc::MAX_THREADS, 1) gn_bwd_cluster_smem_kerne
 
 struct GnPlan { int cl; int nbuf; size_t smem; uint32_t slab_stride; int ctas_per_sm; bool persistent; int threads; };
 // Tunables (environment, read once): DORPATCH_GN=twopass disables the cluster kernels;
-// DORPATCH_GN_PERSIST=1 -> persistent clusters with double-buffered slab prefetch (measured slower on
-// B200 than one cluster per sample: fewer resident CTAs); DORPATCH_GN_SOFT=<KB> per-CTA smem budget
+// DORPATCH_GN_PERSIST=1 -> persistent clusters with double-buffered slab prefetch (measured slower
+// than one cluster per sample: fewer resident CTAs); DORPATCH_GN_SOFT=<KB> per-CTA smem budget
 // used to pick the cluster size.
 static bool gn_plan(int P, int C, size_t es, GnPlan* out) {
   static int mode = -1, persist = 0, big_threads = gnc::MAX_THREADS, cl16 = 0;
@@ -1164,7 +1164,7 @@ void launch_subsample2_adjoint_add(const void* dy, void* dx, int N, int H, int W
 
 // ====================================================================================
 // GroupNorm v2 (round 2): the same cluster-per-sample scheme, rebuilt for instruction count.
-// ncu of v1 (profiles/r02_gn_v1_ncu.txt): DRAM traffic = algorithmic, but 330 warp-instructions per
+// ncu of v1: DRAM traffic = algorithmic, but 330 warp-instructions per
 // 16-byte (x, dy) vector pair at IPC 1.5 -- 64-bit address arithmetic, per-row bound / chunk checks and
 // per-element unpack + gate dominate; the kernels are issue-bound, not HBM-bound.  v2:
 //   * a CTA's slab is a LINEAR array of 16-byte vectors; thread t owns vectors t, t + T, t + 2T, ... (its channel
@@ -1277,7 +1277,7 @@ template <> struct Acc<__nv_bfloat16> {
 // Deterministic CTA reduction of per-thread per-channel accumulators (a[V], b[V]) to the 32 per-group sums, for the
 // linear thread -> column mapping (column = threadIdx.x % cols): fixed xor-shuffle tree inside each warp, one
 // shared-memory exchange, fixed-order sum over the warps.  ~300 cycles; the shared-memory loop of gnc::cta_group_reduce
-// it replaces took 3-9k cycles per slab (phase trace, profiles/r02_gn_v2_trace.txt).  red: >= (blockDim/32) * 64 floats.
+// it replaces took 3-9k cycles per slab (phase trace).  red: >= (blockDim/32) * 64 floats.
 template <int V>
 __device__ __forceinline__ void group_reduce(const float* a, const float* b, int C, float* red, float* part) {
   const int cols = C / V, cpg = C / GN_GROUPS;
@@ -1336,7 +1336,7 @@ __device__ __forceinline__ void group_reduce(const float* a, const float* b, int
   }
 }
 
-// ---- statistics only (the tcgen05 GEMM applies GroupNorm+ReLU in its prologue; the classifier head) -----------------
+// ---- statistics only (the wgmma GEMM applies GroupNorm+ReLU in its prologue; the classifier head) -----------------
 // Streaming: grid (tiles, N), a CTA reads one contiguous 64 KB tile of one sample with the linear thread -> vector
 // mapping (16 independent 16-byte loads per thread, two batches of 8 in flight), reduces to the 32 group sums and
 // writes partial[n][tile][group][2]; gn_finalize_kernel adds the tiles in order (deterministic).
@@ -1699,12 +1699,12 @@ struct Plan { int cl, threads; bool dys; size_t smem; uint32_t stride; };
 
 // ====================================================================================
 // GroupNorm v3: streaming two-phase kernel, second read from L2 (no clusters, no slab in shared memory).
-// Phase traces of v2 (tools/gnbench.cu, profiles/r02_gn_v2_trace.txt) show where a cluster-per-sample kernel loses:
+// Phase traces of v2 (tools/gnbench.cu) show where a cluster-per-sample kernel loses:
 // one 200 KB slab per SM serialises load -> statistics -> cluster barrier (2-3k cycles of skew) -> DSMEM finalize ->
-// apply, clusters of 8 strand 20 of 148 SMs (GPCs hold 16-20 SMs), and 16 warps per SM cannot hide any of it --
+// apply, clusters of 8 strand SMs of partly filled GPCs, and 16 warps per SM cannot hide any of it --
 // while a plain two-pass pair of kernels streams at 90 % of peak but moves 3 units instead of 2.  v3 keeps the
 // streaming structure AND the 2-unit traffic: a persistent grid pulls work items (sample, 32-64 KB tile, phase) from a
-// global counter, ordered so that a group of G samples (G x sample bytes ~ 24 MB, far inside the 126 MB L2) has all its
+// global counter, ordered so that a group of G samples (G x sample bytes ~ 24 MB, inside the H100's 50 MB L2) has all its
 // phase-1 items (read x, per-tile group sums -> global partials, count) ahead of its phase-2 items (wait for the
 // sample's statistics flag, re-read the tile -- an L2 hit --, normalise, write).  The last tile of a sample reduces the
 // partials in tile order (deterministic) and publishes mean / rstd.  Phase-1 items never wait, items are handed out in

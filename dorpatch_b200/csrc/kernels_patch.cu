@@ -1,4 +1,4 @@
-// kernels_patch.cu -- hand-written sm_100a kernels of the patch side of the DorPatch hot loop.
+// kernels_patch.cu -- hand-written sm_90a kernels of the patch side of the DorPatch hot loop.
 //
 //   paste    utils.py:105-110 (clip) + attack.py:185        per image, L2 norm via warp shuffles
 //   expand   K1: attack.py:204-220 + utils.py:77-78         paste + normalise + occlude, ONE HBM pass,
@@ -8,7 +8,7 @@
 //   struct   attack.py:33-45,227-228                        structural loss + its (one-sided) gradient
 //   maskreg  attack.py:72-80,235-245                        density + group-lasso values / statistics
 //   update   K3: attack.py:332-342                          chain rule through clip + sign step + clip
-// (file:line into /root/reference).  Images are NCHW fp32; network input is NHWC(Cp) T.
+// (file:line into the reference).  Images are NCHW fp32; network input is NHWC(Cp) T.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -300,13 +300,14 @@ __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(ExpandParams p) {
 }
 
 // Launch shape.  Work items = images x row tiles (R rows) x sample groups, walked grid-stride by the resident CTAs.
-// Measured over tile heights x sample groups x launch sizes (tools/k1_step_sweep.py, profiles/r02_k1_sweep.txt): tiles of
+// Measured over tile heights x sample groups x launch sizes (tools/k1_step_sweep.py, on the GPU this rule was first tuned on;
+// the sweep has not been repeated on the H100): tiles of
 // 4-8 rows are equivalent and best (a CTA's load + compose prologue stays short and 3-6 CTAs per SM overlap it with their
 // neighbours' stores), 14-16 rows lose 10-30 % (1-2 CTAs per SM, the prologue is exposed), 2 rows lose 15-20 % (per-item
 // overhead), and a launch wants >= 4 items per SM.  Rule: R = 8, or 4 when that leaves fewer than 4 items per SM; sample
 // groups (each re-loads and re-composes the tile) only when the images alone give fewer than 2 items per SM (B = 1).
-// Round 2's first rule maximised "wave efficiency" and picked R = 14 for 512- and 2048-sample launches: 0.29 / 0.65 of
-// peak against 0.72 / 0.79 with R = 8.  DORPATCH_K1_ROWS / _K1_SG (or dp_debug_k1_tuning) pin the choice.
+// A rule that maximised "wave efficiency" picked R = 14 for 512- and 2048-sample launches and was far slower than R = 8.
+// DORPATCH_K1_ROWS / _K1_SG (or dp_debug_k1_tuning) pin the choice.
 static int g_k1_rows = -2, g_k1_sg = -1, g_k1_mode = 0;   // launch-shape overrides (environment, or set_expand_tuning for sweeps)
 static int g_k1_last[4] = {0, 0, 0, 0};                    // tile rows, sample groups, grid, resident CTAs per SM of the last launch
 void get_expand_last(int* out4) { for (int i = 0; i < 4; ++i) out4[i] = g_k1_last[i]; }

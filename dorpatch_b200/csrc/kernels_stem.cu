@@ -1,7 +1,7 @@
 // kernels_stem.cu -- hand-written tensor-core stem convolution (bf16): 7x7 stride 2 pad 3, 3 -> 64.
 //
 // The classifier's first layer (timm ResNetV2 'fixed' stem, StdConv2d 7x7/2; reference call site
-// /root/reference/utils.py:78 -> timm) has only 3 input channels: library kernels want the channel
+// reference utils.py:78 -> timm) has only 3 input channels: library kernels want the channel
 // dimension padded to 8 (bf16), which (i) makes K1 write 8/3 of the algorithmic bytes and (ii) runs
 // at ~23 TFLOP/s in cuDNN.  This kernel reads the TIGHT NHWC C=3 layout K1 produces, builds the
 // im2col tile in shared memory and runs mma.sync.m16n8k16 (bf16 in, fp32 accumulate).

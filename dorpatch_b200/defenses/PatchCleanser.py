@@ -1,6 +1,6 @@
 """PatchCleanser defense (evaluation of the generated patch) on the native forward engine.
 
-Mirrors /root/reference/defenses/PatchCleanser.py: MaskWindow :6-59, PatchCleanser :62-118
+Mirrors reference defenses/PatchCleanser.py: MaskWindow :6-59, PatchCleanser :62-118
 (robust_predict :68-97, mask :99-100, robustness_certificate :102-112), PatchCleanserRecord
 :121-126, PatchCleanserResult :129-134.  Masks are rectangle tables (dorpatch_b200.masks);
 the bool mask tensors of the reference are materialised lazily, only if someone reads

@@ -37,7 +37,7 @@ class Engine:
     def __init__(self, img=224, n_classes=1000, precision="bf16", chunk=64, max_images=1, device=None,
                  autotune=True):
         if not torch.cuda.is_available():
-            raise RuntimeError("dorpatch_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise RuntimeError("dorpatch_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = _lib.load()
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.img, self.n_classes, self.precision = int(img), int(n_classes), precision

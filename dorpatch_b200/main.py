@@ -1,5 +1,5 @@
 """Experiment driver: same command line, artefacts and metrics line as the reference's main.py
-(/root/reference/main.py:8-41 flags, :44-187 main), running on the native engine.
+(reference main.py:8-41 flags, :44-187 main), running on the native engine.
 
 Flags added here (all excluded from the result-directory name so layouts stay compatible):
 --synthetic N, --random_init, --max_iterations, --sampling_size, --num_batches, --precision,

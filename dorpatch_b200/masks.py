@@ -1,7 +1,7 @@
 """Occlusion-mask geometry of the PatchCleanser mask window, as rectangle tables.
 
 Every mask the reference materialises as a [1,H,W] bool tensor
-(/root/reference/defenses/PatchCleanser.py:8-59, /root/reference/attack.py:25-31,83-85) is
+(reference defenses/PatchCleanser.py:8-59, reference attack.py:25-31,83-85) is
 "keep everything except <= 2 axis-aligned rectangles"; the native K1 kernel synthesises the
 occlusion from the rectangles (int16 r0,r1,c0,c1 -- rows [r0,r1) x cols [c0,c1) become 0.5),
 so the 126 MB bool universe is never built.

@@ -1,7 +1,7 @@
 """ResNetV2-50x1-BiT parameter container whose forward runs on the native engine.
 
 The reference obtains this classifier from timm (``timm.create_model(
-'resnetv2_50x1_bit_distilled')``, /root/reference/utils.py:51-58).  timm is not vendored
+'resnetv2_50x1_bit_distilled')``, reference utils.py:51-58).  timm is not vendored
 there; this module keeps timm's parameter names (``stem.conv.weight``,
 ``stages.S.blocks.B.{downsample.conv,norm1,conv1,norm2,conv2,norm3,conv3}``, ``norm``,
 ``head.fc``) so PatchCleanser checkpoints load with ``load_state_dict``, and executes on

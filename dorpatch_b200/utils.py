@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's utils.py (same names, arguments and error behaviour).
 
-Reference: /root/reference/utils.py -- set_device :12-13, set_random_seed :16-21,
+Reference: reference utils.py -- set_device :12-13, set_random_seed :16-21,
 generate_saving_path :24-44, get_model :47-63, get_normalize :66-68, NormModel :71-78,
 get_dataset :81-102, clip :105-110, convert_float_list_to_str :112.
 Compute (`clip`, the classifier) runs in libdorpatch.so; this file is glue.

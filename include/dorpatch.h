@@ -1,4 +1,4 @@
-/* dorpatch.h -- C ABI of libdorpatch.so, the B200-native DorPatch hot-path engine.
+/* dorpatch.h -- C ABI of libdorpatch.so, the H100-native (sm_90a) DorPatch hot-path engine.
  *
  * Plain C: opaque handle, raw pointers, sizes, int error codes.  No torch types.
  * "dev" pointers are CUDA device pointers on the engine's device, "host" pointers
@@ -10,7 +10,7 @@
  * Every entry point returns 0 on success, non-zero on failure; dp_last_error()
  * then holds a human-readable message (the Python host raises RuntimeError with it).
  *
- * Reference interfaces replaced (CGCL-codes/DorPatch @ 0751fd4, /root/reference):
+ * Reference interfaces replaced (CGCL-codes/DorPatch @ 0751fd4):
  *   dp_paste            utils.py:105-110 `clip` + attack.py:185 (adv_x = x + delta)
  *   dp_expand           attack.py:204-220 (mask gather + occlude [+dual]) and
  *                       utils.py:77-78 NormModel's (x-0.5)/0.5, fused       [K1]
@@ -211,11 +211,11 @@ int32_t dp_failed_set_read(dp_engine* e, int32_t b, int32_t* idx_host_out, int32
 /* Op-level hooks for the parity tests (tests/test_gpu_ops.py); not part of the reference-facing surface.
  * dp_debug_stem_bwd_reduce: the bf16 engine's fused stem-dgrad + masked EOT reduce (K1^T as the bench runs it) on a
  *   caller-supplied dY [B*S, H/2, H/2, 64] bf16 dev: G[B,3,H,W] = 2 * sum_s keep_s * conv7x7s2^T(dY_s, W_stem).
- * dp_debug_gn_gemm: the tcgen05 GroupNorm-prologue GEMM on caller-supplied operands: out[m,n] = sum_k
+ * dp_debug_gn_gemm: the wgmma GroupNorm-prologue GEMM on caller-supplied operands: out[m,n] = sum_k
  *   relu(gn(x))[m,k] * W[n,k] (+ shortcut); x [N*P,K] bf16, w_nk [Nout,K] bf16, stats [N,32,2] (mean, rstd), all dev.
  * dp_debug_gn: GroupNorm(32)+ReLU forward (and, with dy, backward-to-input) in the engine's activation dtype on
  *   caller-supplied [N,P,C] tensors; stats [N,32,2] dev out.  y == NULL: statistics pass only (the streaming
- *   kernel in front of the tcgen05 GEMM and the classifier head). */
+ *   kernel in front of the wgmma GEMM and the classifier head). */
 int32_t dp_debug_stem_bwd_reduce(dp_engine* e, const void* dY, const int16_t* rects_host, int32_t B, int32_t S, float* G,
                                  void* stream);
 /* K1 launch-shape sweep hook (tools/k1_step_sweep.py): tile rows / sample groups (0 = the wave-efficiency heuristic) and the

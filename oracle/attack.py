@@ -1,8 +1,8 @@
 """Oracle restatement of the DorPatch optimisation loop (torch-CPU, fp32).
 
-Follows /root/reference/attack.py (CW_loss :10-23, local_variance :33-39,
+Follows reference attack.py (CW_loss :10-23, local_variance :33-39,
 min_var_weighted_variance :41-45, DorPatch.generate :51-361, patch_selection
-:363-382, collect_failure :384-406) and /root/reference/utils.py:105-110 (clip).
+:363-382, collect_failure :384-406) and reference utils.py:105-110 (clip).
 
 Differences from the reference, all deliberate and documented in DESIGN.md:
   * B > 1 is defined as B independent single-image problems (the reference is

@@ -1,7 +1,7 @@
 """Oracle: PatchCleanser occlusion-mask geometry as rectangles.
 
-Restates /root/reference/defenses/PatchCleanser.py:8-59 (MaskWindow) and the
-attack's mask universe (/root/reference/attack.py:25-31,83-85).
+Restates reference defenses/PatchCleanser.py:8-59 (MaskWindow) and the
+attack's mask universe (reference attack.py:25-31,83-85).
 Every mask is "keep everything except <= 2 axis-aligned rectangles" (True=keep).
 A rectangle is (r0, r1, c0, c1), rows [r0,r1) x cols [c0,c1) occluded.
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).

@@ -1,6 +1,6 @@
 """Oracle restatement of the PatchCleanser defense used to score the attack.
 
-Follows /root/reference/defenses/PatchCleanser.py:62-112 (robust_predict,
+Follows reference defenses/PatchCleanser.py:62-112 (robust_predict,
 robustness_certificate).  ``model`` maps [N,3,H,W] in [0,1] -> logits on CPU.
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 """

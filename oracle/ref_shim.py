@@ -1,9 +1,8 @@
-"""Import the UNMODIFIED reference (/root/reference) on a CPU-only box.
+"""Import the UNMODIFIED reference (a checkout of the original DorPatch project at
+``$DORPATCH_REFERENCE_ROOT``) on a CPU-only machine.
 
-Used only in the build container (``/root/reference`` does not exist on the GPU
-box) by ``tests/golden/make_golden.py`` to generate golden vectors and by
-``tests/test_oracle_vs_reference.py`` (skipped when the reference is absent) to
-pin the oracle.  Nothing is copied: the reference modules are imported from
+Used only by ``tests/golden/make_golden.py`` to generate the golden vectors the
+tests compare with.  Nothing is copied: the reference modules are imported from
 where they lie.
 
 Shim (SURVEY.md section 8c):
@@ -14,7 +13,7 @@ Shim (SURVEY.md section 8c):
     ``Module.cuda`` is identity;
   * ``timm`` (not installed, third-party) is replaced by an empty stub module --
     ``utils.get_model`` is never called, the caller passes its own model;
-  * ``/root/reference`` is put on ``sys.path`` so ``attack``, ``utils`` and
+  * the reference root is put on ``sys.path`` so ``attack``, ``utils`` and
     ``defenses.PatchCleanser`` resolve to the reference's files.
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 """
@@ -25,12 +24,21 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = "/root/reference"
+REFERENCE_ROOT = os.environ.get("DORPATCH_REFERENCE_ROOT", "")
 _REF_MODULES = ("attack", "utils", "defenses", "defenses.PatchCleanser", "main")
+_REPO_ROOT = os.path.realpath(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
-def available():
-    return os.path.isfile(os.path.join(REFERENCE_ROOT, "attack.py"))
+def _root():
+    """The reference checkout, or a clear error: never the current directory, never this repository (whose root holds
+    same-named drop-in modules)."""
+    if not REFERENCE_ROOT or not os.path.isabs(REFERENCE_ROOT) or not os.path.isdir(REFERENCE_ROOT):
+        raise RuntimeError("DORPATCH_REFERENCE_ROOT must be the absolute path of a checkout of the original DorPatch project "
+                           "(got %r)" % REFERENCE_ROOT)
+    root = os.path.realpath(REFERENCE_ROOT)
+    if root == _REPO_ROOT:
+        raise RuntimeError("DORPATCH_REFERENCE_ROOT points at this repository, not at the original DorPatch project")
+    return root
 
 
 @contextlib.contextmanager
@@ -39,6 +47,7 @@ def reference_modules():
     ``utils`` and ``PatchCleanser`` modules; restores sys.modules/sys.path and
     the torch monkeypatches on exit so the product's same-named root modules
     are unaffected."""
+    ref_root = _root()
     import torch
     import torchvision  # noqa: F401  (the reference imports it)
     saved = {k: sys.modules.get(k) for k in _REF_MODULES + ("timm",)}
@@ -48,7 +57,7 @@ def reference_modules():
         for k in _REF_MODULES:
             sys.modules.pop(k, None)
         sys.modules["timm"] = types.ModuleType("timm")
-        sys.path.insert(0, REFERENCE_ROOT)
+        sys.path.insert(0, ref_root)
         torch.Tensor.cuda = lambda self, *a, **k: self.clone()
         torch.Tensor.cpu = lambda self, *a, **k: self.clone()
         torch.nn.Module.cuda = lambda self, *a, **k: self
@@ -56,11 +65,11 @@ def reference_modules():
         # Load by file path: the repo root holds same-named drop-in modules (attack, utils,
         # defenses/ -- a regular package, which would shadow the reference's namespace package).
         pkg = types.ModuleType("defenses")
-        pkg.__path__ = [os.path.join(REFERENCE_ROOT, "defenses")]
+        pkg.__path__ = [os.path.join(ref_root, "defenses")]
         sys.modules["defenses"] = pkg
 
         def load(name, rel):
-            spec = importlib.util.spec_from_file_location(name, os.path.join(REFERENCE_ROOT, rel))
+            spec = importlib.util.spec_from_file_location(name, os.path.join(ref_root, rel))
             mod = importlib.util.module_from_spec(spec)
             sys.modules[name] = mod
             spec.loader.exec_module(mod)
@@ -69,7 +78,7 @@ def reference_modules():
         ns.utils = load("utils", "utils.py")
         ns.PatchCleanser = load("defenses.PatchCleanser", "defenses/PatchCleanser.py")
         ns.attack = load("attack", "attack.py")
-        assert ns.attack.__file__.startswith(REFERENCE_ROOT), ns.attack.__file__
+        assert os.path.realpath(ns.attack.__file__).startswith(ref_root + os.sep), ns.attack.__file__
         assert ns.attack.MaskWindow is ns.PatchCleanser.MaskWindow and ns.attack.clip is ns.utils.clip
         yield ns
     finally:

@@ -1,8 +1,8 @@
 """Oracle restatement of the classifier the reference attacks.
 
 The reference builds ``timm.create_model('resnetv2_50x1_bit_distilled')``
-(/root/reference/utils.py:51-58) and wraps it in ``NormModel`` with
-mean=std=0.5 (/root/reference/utils.py:66-78).  timm 0.6.7 is a third-party
+(reference utils.py:51-58) and wraps it in ``NormModel`` with
+mean=std=0.5 (reference utils.py:66-78).  timm 0.6.7 is a third-party
 dependency that is not vendored in the reference and not installed here, so the
 architecture is restated from its published definition (timm 0.6.7
 ``models/resnetv2.py``: ResNetV2 with PreActBottleneck blocks, StdConv2d
@@ -135,7 +135,7 @@ def forward_normalized(params, z, taps=None):
 
 
 def forward(params, x01, taps=None):
-    """NormModel.forward (/root/reference/utils.py:77-78): (x-0.5)/0.5 -> net."""
+    """NormModel.forward (reference utils.py:77-78): (x-0.5)/0.5 -> net."""
     return forward_normalized(params, (x01 - 0.5) / 0.5, taps)
 
 

@@ -55,13 +55,14 @@ def main():
                     help="NOISE-FLOOR run: every image += perturb * N(0,1) (1e-7: below any arithmetic difference between fp32 "
                          "implementations) -- how far the END METRIC of the reference's own arithmetic moves under a last-bit change")
     ap.add_argument("--out", default="attack_success_golden.npz")
-    ap.add_argument("--save-adv", type=int, default=1, help="keep the final adversarial images (frozen-patch evaluation parity)")
+    ap.add_argument("--save-adv", type=int, default=1,
+                    help="keep the final pasted perturbations, adv = image + delta (frozen-patch evaluation parity)")
     a = ap.parse_args()
     K, iters, S, eps, perturb = a.K, a.iters, a.S, a.eps, a.perturb
     torch.set_num_threads(min(16, os.cpu_count() or 1))
     params = OR.random_init(seed=0, affine_jitter=0.1)
     net = OR.OracleNet(params, weights_require_grad=False).eval()
-    rec = dict(y=[], pred_adv=[], pc_pred=[], pc_cert=[], mask_frac=[], l2=[], steps=[], adv=[], margin=[])
+    rec = dict(y=[], pred_adv=[], pc_pred=[], pc_cert=[], mask_frac=[], l2=[], steps=[], delta=[], margin=[])
     t0 = time.time()
     for i in range(K):
         x = image(i)
@@ -87,7 +88,7 @@ def main():
         rec["mask_frac"].append(float(m.mean())); rec["l2"].append(float(delta.norm())); rec["steps"].append(len(trace))
         rec["margin"].append(float(top2[0] - top2[1]))
         if a.save_adv:
-            rec["adv"].append(adv[0].numpy().copy())
+            rec["delta"].append(delta[0].numpy().copy())
         print("img %2d  y %3d  adv %3d (top-2 margin %.2e)  PC %s cert %s  mask %.4f  l2 %.3f  steps %d  (%.0f s)" % (
             i, y, pa, rec["margin"][-1], preds, [int(c) for c in certs], rec["mask_frac"][-1], rec["l2"][-1], len(trace), time.time() - t0),
             flush=True)

@@ -1,13 +1,15 @@
-"""Generate golden vectors by running the UNMODIFIED reference (/root/reference) under the CPU
-shim of oracle/ref_shim.py.  Run in the build container only (the reference is absent on
-the GPU box); the resulting small .npz fixtures are committed next to this script.
+"""Generate golden vectors by running the UNMODIFIED reference (a checkout of the original DorPatch
+project, located by DORPATCH_REFERENCE_ROOT) under the CPU shim of oracle/ref_shim.py; the resulting
+.npz fixtures are committed next to this script, so the tests need no reference checkout.
 
-    python tests/golden/make_golden.py
+    DORPATCH_REFERENCE_ROOT=/path/to/DorPatch python tests/golden/make_golden.py
 
 Pins (SURVEY.md section 4): G1 mask geometry, G2 utils.clip, G3 losses + gradients,
 G4 patch_selection, G5/G6 generate trajectories (tiny stand-in classifier: targeted 10 steps,
 and untargeted 1100 steps crossing the i==500 targeted switch, the i>=1000 failed-set sampling
-and the lr-decay path), G7 PatchCleanser records, G9 a ResNetV2-50 trajectory at 112 px.
+and the lr-decay path), G7 PatchCleanser records, G8 a 25-step dual-dropout trajectory,
+G9 a ResNetV2-50 trajectory at 112 px.  The G2 vectors go to reference_golden_g2.npz, the rest to
+reference_golden.npz (each file stays below 1 MB).
 """
 import contextlib
 import io
@@ -69,7 +71,6 @@ def run_generate(ref, net, x, **kw):
 
 
 def main():
-    assert ref_shim.available(), "reference not present"
     torch.set_num_threads(8)
     out = {}
     with ref_shim.reference_modules() as ref:
@@ -156,6 +157,11 @@ def main():
             out["g6_%s_rng_t" % name] = rt
             print(name, "log lines", len(log), "mask mean", mo.mean())
         out["g6_x"] = xs.numpy()
+        # ---- G8 targeted 25-step run, dropout 2 (tests/test_oracle_vs_reference.py) -----------------------
+        x8 = torch.rand(1, 3, 56, 56, generator=torch.Generator().manual_seed(21))
+        mo, po, log, rn, rt = run_generate(ref, tiny, x8, patch_budget=0.12, n_classes=1000, targeted=True,
+                                           y=torch.tensor([7]), max_iterations=25, sampling_size=3, dropout=2)
+        out.update(g8_mask=mo, g8_pattern=po, g8_log=np.array(log), g8_rng_np=rn)
         # ---- G7 PatchCleanser records -------------------------------------------------------------------
         with contextlib.redirect_stdout(io.StringIO()):
             for r in (0.03, 0.12):
@@ -181,8 +187,20 @@ def main():
         out["g9_log"] = np.array(log)
         out["g9_rng_np"] = rn
         out["g9_target"] = ((yr + 17) % 1000).numpy()
-    np.savez_compressed(os.path.join(HERE, "reference_golden.npz"), **out)
-    print("wrote", os.path.join(HERE, "reference_golden.npz"), os.path.getsize(os.path.join(HERE, "reference_golden.npz")))
+    for name, keep in (("reference_golden.npz", lambda k: not k.startswith("g2_")),
+                       ("reference_golden_g2.npz", lambda k: k.startswith("g2_"))):
+        path = os.path.join(HERE, name)
+        np.savez_compressed(path, **{k: v for k, v in out.items() if keep(k)})
+        print("wrote", path, os.path.getsize(path))
+
+
+def load():
+    """Both fixture files as one {name: array} dict."""
+    G = {}
+    for name in ("reference_golden.npz", "reference_golden_g2.npz"):
+        with np.load(os.path.join(HERE, name), allow_pickle=False) as f:
+            G.update({k: f[k] for k in f.files})
+    return G
 
 
 if __name__ == "__main__":

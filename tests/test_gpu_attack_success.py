@@ -118,13 +118,14 @@ def _report(tag, precision, y, g, pred_adv, pc_pred, pc_cert):
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_evaluation_bits_on_frozen_adversarial_images(oracle_params, precision):
     g = _load(GOLD)
-    if "adv" not in g.files:
-        pytest.skip("attack_success_golden.npz holds no adversarial images: regenerate it (--save-adv 1)")
+    if "delta" not in g.files:
+        pytest.skip("attack_success_golden.npz holds no adversarial perturbations: regenerate it (--save-adv 1)")
     K, img = int(g["K"]), int(g["img"])
     y = g["y"].astype(np.int64)
+    adv = torch.cat([_image(i, img, g["img_seed0"]) for i in range(K)]) + torch.from_numpy(g["delta"])
     pipe = _Pipeline(oracle_params, precision, img, K, g["ratios"])
     try:
-        pred_adv, pc_pred, pc_cert = pipe.evaluate(torch.from_numpy(g["adv"]).to(DEV))
+        pred_adv, pc_pred, pc_cert = pipe.evaluate(adv.to(DEV))
     finally:
         pipe.close()
     _report("frozen", precision, y, g, pred_adv, pc_pred, pc_cert)
@@ -133,8 +134,7 @@ def test_evaluation_bits_on_frozen_adversarial_images(oracle_params, precision):
            or not np.array_equal(pc_cert[i], g["pc_cert"][i].astype(bool))]
     print("[frozen %s] images with any differing bit: %s (oracle top-2 margins %s)" % (
         precision, bad, [float("%.2e" % g["margin"][i]) for i in bad] if "margin" in g.files else "n/a"))
-    # Measured on hardware (profiles/r02_attack_success.txt): fp32 and tf32 reproduce ALL bits of all 16 images; bf16 differs on
-    # images 1, 8, 13 (oracle top-2 margins 0.007 / 0.019 / 0.016 -- bf16 resolves logits to ~5 % of their norm).  The library
+    # bf16 resolves logits to ~5 % of their norm, so it may flip images whose oracle top-2 margin is small.  The library
     # convolution algorithms are chosen by timing, so roundings may differ between runs: the bars leave room for the images whose
     # oracle decision hangs on a margin below 0.05 (6 of the 16): fp32 <= 1, tf32 <= 2, bf16 <= that count.
     small = int((g["margin"] < 0.05).sum()) if "margin" in g.files else K // 4
@@ -151,7 +151,7 @@ def test_attack_success_rates_within_the_reference_noise_floor(oracle_params, pr
     # sqrt(K q) images (one sigma).  q is estimated per metric from the flips between the two oracle runs, and the bar is
     # three sigma, never below one image:  bar_k = max(1, ceil(3 sqrt(flips_k))) / K.  (Every run of the engine is a fresh
     # draw from that distribution -- cuDNN / cublasLt algorithms are picked by timing -- so a two-sigma bar would fail one run
-    # in five over the six checks.  Measured deviations over two hardware runs x three precisions: 0 to 3 images.)
+    # in five over the six checks.)
     yn = nz["y"].astype(np.int64)
 
     def bits(yy, pred_adv, pc_pred, pc_cert):

@@ -1,6 +1,6 @@
 """Op-level GPU parity of the hand-written kernels that the network-level tests only see through the whole net:
 GroupNorm(32)+ReLU v2 forward / backward (fp32 and bf16, every ResNetV2-50 shape class), the bf16 engine's fused
-stem-dgrad + masked EOT reduce (K1^T as the bench runs it), and the tcgen05 GroupNorm-prologue GEMM -- each against
+stem-dgrad + masked EOT reduce (K1^T as the bench runs it), and the wgmma GroupNorm-prologue GEMM -- each against
 a PyTorch fp32/fp64 CPU restatement of the same operator on the same (bf16-rounded) operands, through the C ABI's
 dp_debug_* hooks.  Restated operators: timm GroupNormAct = F.group_norm(32, eps 1e-5) + ReLU and its autograd
 gradient (reference call site utils.py:77-78 -> timm resnetv2); the stem's StdConv2d 7x7/2 transposed; 1x1 StdConv2d."""
@@ -86,7 +86,7 @@ def test_groupnorm_relu_fwd_bwd_vs_fp64(engines, precision, P, Cc, neg_gamma):
     mean_ref = x.double().reshape(N, P, 32, Cc // 32).mean((1, 3))
     rstd_ref = 1.0 / torch.sqrt(x.double().reshape(N, P, 32, Cc // 32).var((1, 3), unbiased=False) + 1e-5)
     assert (stats[:, :, 0].cpu().double() - mean_ref).abs().max().item() <= 1e-4
-    # the statistics-only pass (streaming kernel in front of the tcgen05 GEMM / the classifier head): same (mean, rstd)
+    # the statistics-only pass (streaming kernel in front of the wgmma GEMM / the classifier head): same (mean, rstd)
     stats2 = torch.full((N, 32, 2), float("nan"), device=DEV)
     _lib.check(e.lib.dp_debug_gn(e.handle, _ptr(xd), None, None, _ptr(gd), _ptr(bd), 1, None, None, _ptr(stats2), N, P, Cc, e._stream()))
     torch.cuda.synchronize()
@@ -134,7 +134,7 @@ GEMM_SHAPES = [  # (N, P, K, Nout, shortcut): conv3 of every stage (with the res
 
 @pytest.mark.parametrize("N,P,K,Nout,shortcut", GEMM_SHAPES)
 def test_tcgen05_gn_gemm_vs_fp32(engines, N, P, K, Nout, shortcut):
-    """kernels_gemm.cu (tcgen05.mma, TMEM accumulators): out = relu(gn(x)) @ W^T (+ shortcut) with relu(gn(x)) rounded to
+    """kernels_gemm.cu (wgmma.mma_async, register accumulators): out = relu(gn(x)) @ W^T (+ shortcut) with relu(gn(x)) rounded to
     bf16 on its way into shared memory, against the same product in torch fp32 on the same bf16-rounded operands
     (timm PreActBottleneck norm1->conv1 / norm3->conv3 + residual).  fp32 accumulation on both sides, output rounded to
     bf16: |diff| <= 1/128 of the output's max (one bf16 ulp at the top of the range) and relative L2 <= 4e-3."""

@@ -1,5 +1,5 @@
-"""Print the figures of a bench.py JSON line that matter when reading a gpurun tail.
-usage: python tools/bench_digest.py gpurun_out/bench.json"""
+"""Print the figures of a bench.py JSON line that matter when reading a log tail.
+usage: python tools/bench_digest.py bench.json"""
 import json
 import sys
 

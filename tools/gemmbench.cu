@@ -1,8 +1,8 @@
-// gemmbench.cu -- per-layer time of the tcgen05 GroupNorm-prologue 1x1-convolution GEMM (kernels_gemm.cu) on every fused
+// gemmbench.cu -- per-layer time of the wgmma GroupNorm-prologue 1x1-convolution GEMM (kernels_gemm.cu) on every fused
 // ResNetV2-50 shape at 224 px: norm1 -> conv1 (blocks without a downsample branch) and norm3 -> conv3 (+ shortcut).
 // Prints ms, algorithmic GB/s (x read once + out written (+ shortcut read) + weights) and TFLOP/s per shape, plus the
 // statistics pass in front of it.  Buffers rotate over > 300 MB so that no launch finds its operands in L2.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o gemmbench tools/gemmbench.cu \
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o gemmbench tools/gemmbench.cu \
 //        -Ldorpatch_b200/lib -ldorpatch -Xlinker -rpath,$PWD/dorpatch_b200/lib
 //   ./gemmbench [N]
 #include <cuda_bf16.h>

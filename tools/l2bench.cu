@@ -1,9 +1,9 @@
-// l2bench.cu -- ceiling of an "L2-windowed two-kernel" GroupNorm on B200: the statistics pass and the apply pass run as two
-// plain streaming kernels over a WINDOW of samples small enough that the apply pass re-reads x from the 126 MB L2 instead of
+// l2bench.cu -- ceiling of an "L2-windowed two-kernel" GroupNorm: the statistics pass and the apply pass run as two
+// plain streaming kernels over a WINDOW of samples small enough that the apply pass re-reads x from L2 (50 MB on the H100) instead of
 // HBM.  HBM traffic is then the cluster kernels' (1 read + 1 write forward; x, dy read + dx written backward) but no CTA holds a
 // slab, no cluster barrier, every SM streams.  Prints effective GB/s = algorithmic bytes / time for window sizes 8..96 MB and
 // for the unwindowed two-pass baseline (window = whole buffer: the second read comes from HBM).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o gpurun_out/l2bench tools/l2bench.cu && gpurun_out/l2bench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o build/l2bench tools/l2bench.cu && build/l2bench
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

@@ -1,5 +1,5 @@
 """Aggregate an `ncu --metrics gpu__time_duration.sum --csv` launch list by kernel name.
-usage: python tools/launch_summary.py gpurun_out/launches.csv "<title>" > profiles/rNN_launches.txt"""
+usage: python tools/launch_summary.py launches.csv "<title>" > launches.txt"""
 import collections
 import csv
 import re

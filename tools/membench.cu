@@ -1,7 +1,7 @@
-// membench.cu -- what does a B200 SM-side access pattern cost?  Diagnostic for the GroupNorm kernels, which sit
-// at ~3.1 TB/s whatever the CTA shape while the driver's copy peak is 6.5 TB/s and K1's bulk stores reach 5.2.
+// membench.cu -- what does an SM-side access pattern cost?  Diagnostic for the GroupNorm kernels, which sit
+// at a fraction of the copy peak whatever the CTA shape, while K1's bulk stores come much closer to it.
 // Each pattern moves the same buffers; prints GB/s (bytes read + written).  Standalone:
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o gpurun_out/membench tools/membench.cu && gpurun_out/membench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o build/membench tools/membench.cu && build/membench
 #include <cooperative_groups.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
-"""Summarise an .ncu-rep (ncu --set full) into a small text table for profiles/.
-usage: python tools/ncu_summary.py gpurun_out/prof.ncu-rep "<title>" > profiles/rNN_xxx.txt"""
+"""Summarise an .ncu-rep (ncu --set full) into a small text table.
+usage: python tools/ncu_summary.py prof.ncu-rep "<title>" > prof.txt"""
 import csv
 import subprocess
 import sys
