@@ -5,6 +5,10 @@ Mirrors reference defenses/PatchCleanser.py: MaskWindow :6-59, PatchCleanser :62
 :121-126, PatchCleanserResult :129-134.  Masks are rectangle tables (dorpatch_b200.masks);
 the bool mask tensors of the reference are materialised lazily, only if someone reads
 ``mask_set`` / ``double_mask_set``.
+
+``MaskWindow(img, r, n_patch=2)`` is the two-patch window (reference :31-37): 630 first-round pairs and
+22 680 certificate masks of 3 rectangles each.  Its second round puts 4 rectangles on a sample, which is
+K1's per-sample limit, so the same code and kernels serve both windows.
 """
 import math
 
@@ -17,14 +21,15 @@ from ..utils import unwrap_native
 
 class MaskWindow(object):
     def __init__(self, img_size, patch_ratio=0.03, n_patch=1):
-        if n_patch != 1:
-            raise NotImplementedError("n_patch=%r (the reference's n_patch=2 path is unused by DorPatch)" % n_patch)
+        if n_patch not in (1, 2):
+            raise NotImplementedError("n_patch=%r: PatchCleanser masks exist for 1 or 2 patches" % (n_patch,))
         g = _masks.WindowGeometry(img_size, patch_ratio, n_patch)
         self.img_size, self.n_patch = img_size, n_patch
         self.mask_size, self.stride, self.window_size = g.mask_size, g.stride, g.window_size
         self.num_mask_per_axis = _masks.MASKS_PER_AXIS
-        self.mask_rects = _masks.mask_set(img_size, patch_ratio, 1)           # [36,2,4]
-        self.double_mask_rects = _masks.mask_set(img_size, patch_ratio, 2)    # [630,2,4]
+        # n_patch 1: [36,2,4] / [630,2,4];  n_patch 2: [630,2,4] / [22680,3,4]
+        self.mask_rects = _masks.mask_set(img_size, patch_ratio, 1, n_patch)
+        self.double_mask_rects = _masks.mask_set(img_size, patch_ratio, 2, n_patch)
         self._bool = {}
         print("mask size: %d, window size: %d, stride: %d" % (self.mask_size, self.window_size, self.stride))
 
@@ -65,7 +70,7 @@ class PatchCleanser(object):
 
     def robust_predict(self, img, certify=False):
         mw = self.mask_window
-        single = _masks.gather(mw.mask_rects, np.arange(len(mw.mask_rects)))          # [36,4,4]
+        single = _masks.gather(mw.mask_rects, np.arange(len(mw.mask_rects)))          # [36 or 630,4,4]
         preds_1 = self._predict(img, single)                                          # :70-72
         labels, counts = torch.from_numpy(preds_1.astype(np.int64)).unique(sorted=False, return_counts=True)
         label_majority = labels[counts.argmax()].item()                               # :74-75
@@ -78,7 +83,8 @@ class PatchCleanser(object):
                 if label == label_majority:
                     continue
                 for k in np.nonzero(preds_1 == label)[0]:
-                    # second-round masking of the already one-masked image = double mask (k, j)
+                    # second-round masking of the already-masked image: mask j plus mask k's rectangles
+                    # (one for n_patch 1, a pair for n_patch 2) in slots 2-3
                     second = single.copy()
                     second[:, 2:4, :] = single[k, 0:2, :]
                     if (self._predict(img, second) == label).all():
@@ -92,7 +98,7 @@ class PatchCleanser(object):
         return img * msk + 0.5 * ~msk
 
     def robustness_certificate(self, img, label, batch_size=64):
-        """All 630 double-mask predictions must equal `label` (:102-112).  `batch_size` is kept
+        """All double-mask predictions (630, or 22 680 for n_patch 2) must equal `label` (:102-112).  `batch_size` is kept
         for signature compatibility; batching is the engine's `chunk`."""
         mw = self.mask_window
         preds = self._predict(img, _masks.gather(mw.double_mask_rects, np.arange(len(mw.double_mask_rects))))

@@ -3,7 +3,11 @@
 
 Flags added here (all excluded from the result-directory name so layouts stay compatible):
 --synthetic N, --random_init, --max_iterations, --sampling_size, --num_batches, --precision,
---chunk, --img_size, --seed.
+--chunk, --img_size, --seed, --pc_n_patch.
+
+--pc_n_patch 2 evaluates against the two-patch PatchCleanser (MaskWindow(img, r, 2), reference
+defenses/PatchCleanser.py:34-37).  It does not change the generated patches, so a run on an existing
+result directory reuses them; its records go to adv_PC2_<i>.pt, apart from the one-patch adv_PC_<i>.pt.
 """
 import argparse
 import os
@@ -51,6 +55,8 @@ parser.add_argument('--precision', default=None, choices=['fp32', 'tf32', 'bf16'
 parser.add_argument('--chunk', default=None, type=int, help='samples per classifier pass')
 parser.add_argument('--img_size', default=224, type=int, help='synthetic image size (multiple of 56)')
 parser.add_argument('--seed', default=0, type=int, help='seed of the random-init weights')
+parser.add_argument('--pc_n_patch', default=1, type=int, choices=[1, 2],
+                    help='patches the PatchCleanser evaluation is provisioned for (2: records in adv_PC2_<i>.pt)')
 
 
 def _init_distributed():
@@ -96,7 +102,8 @@ def main(args):
                              synthetic=args.synthetic, img_size=args.img_size)
     attack = DorPatch()
     img = args.img_size if args.synthetic else 224
-    defense = [PatchCleanser(MaskWindow(img, r, 1), model) for r in [0.015, 0.03, 0.06, 0.12]]
+    defense = [PatchCleanser(MaskWindow(img, r, args.pc_n_patch), model) for r in [0.015, 0.03, 0.06, 0.12]]
+    pc_name = "adv_PC_%d.pt" if args.pc_n_patch == 1 else "adv_PC2_%d.pt"
 
     target_list, preds_list, y_list, preds_adv_list, records = [], [], [], [], []
     with torch.no_grad():
@@ -142,7 +149,7 @@ def main(args):
 
             adv_x, _, _ = eng.paste(x, adv_mask, adv_pattern, args.epsilon)
 
-            pc_path = os.path.join(result_dir, "adv_PC_%d.pt" % i)
+            pc_path = os.path.join(result_dir, pc_name % i)
             if os.path.exists(pc_path):
                 with open(pc_path, 'rb') as f:
                     records_batch = pickle.load(f)

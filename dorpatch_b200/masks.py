@@ -2,9 +2,11 @@
 
 Every mask the reference materialises as a [1,H,W] bool tensor
 (reference defenses/PatchCleanser.py:8-59, reference attack.py:25-31,83-85) is
-"keep everything except <= 2 axis-aligned rectangles"; the native K1 kernel synthesises the
-occlusion from the rectangles (int16 r0,r1,c0,c1 -- rows [r0,r1) x cols [c0,c1) become 0.5),
-so the 126 MB bool universe is never built.
+"keep everything except <= 3 axis-aligned rectangles" (<= 2 for the one-patch window and the
+attack's universe, 3 for the two-patch window's double masks); the native K1 kernel synthesises
+the occlusion from up to 4 rectangles per sample (int16 r0,r1,c0,c1 -- rows [r0,r1) x cols
+[c0,c1) become 0.5), so the 126 MB bool universe (1.1 GB for the two-patch double masks at
+224 px) is never built.
 """
 import math
 
@@ -40,8 +42,15 @@ def pair_index():
     return a, b
 
 
-def mask_set(img_size, patch_ratio, dropout):
-    """int16 [n,2,4] rectangle pairs of `mask_set` (dropout 1) / `double_mask_set` (dropout 2)."""
+def mask_set(img_size, patch_ratio, dropout, n_patch=1):
+    """Rectangle table of `mask_set` (dropout 1) / `double_mask_set` (dropout 2) of the window for n_patch patches
+    (PatchCleanser.py:19-39).  n_patch 1: int16 [36,2,4] single rectangles (slot 1 empty) / [630,2,4] pairs.
+    n_patch 2 (36 basic rectangles of the two-patch geometry): [630,2,4] pairs / [22680,3,4], mask i*630+j = pair j
+    plus basic rectangle i (PatchCleanser.py:36-37; entries with i in pair j are kept, as there)."""
+    if n_patch == 2:
+        return _two_patch_set(img_size, patch_ratio, dropout)
+    if n_patch != 1:
+        raise NotImplementedError("n_patch=%r: PatchCleanser masks exist for 1 or 2 patches" % (n_patch,))
     s = WindowGeometry(img_size, patch_ratio).single_rects()
     if dropout == 1:
         out = np.zeros((len(s), 2, 4), np.int16)
@@ -53,17 +62,35 @@ def mask_set(img_size, patch_ratio, dropout):
     raise ValueError("dropout must be 1 or 2, got %r" % (dropout,))
 
 
+def _two_patch_set(img_size, patch_ratio, dropout):
+    s = WindowGeometry(img_size, patch_ratio, 2).single_rects()
+    a, b = pair_index()
+    pairs = np.stack([s[a], s[b]], axis=1)                     # [630,2,4]
+    if dropout == 1:
+        return pairs
+    if dropout == 2:
+        out = np.empty((len(s), len(pairs), 3, 4), np.int16)   # [basic i, pair j]
+        out[:, :, 0:2] = pairs[None]
+        out[:, :, 2] = s[:, None]
+        return out.reshape(-1, 3, 4)
+    raise ValueError("dropout must be 1 or 2, got %r" % (dropout,))
+
+
 def universe(img_size, dropout, sizes=DROPOUT_SIZES):
     """The attack's mask universe (attack.py:83-85): [n_mask,2,4] int16."""
     return np.concatenate([mask_set(img_size, r, dropout) for r in sizes], axis=0)
 
 
 def gather(table, idx, idx_dual=None):
-    """Rectangles of the sampled masks: table [n,2,4], idx [...] -> [...,4,4] int16
-    (second pair from idx_dual, or empty)."""
+    """Rectangles of the sampled masks: table [n,k,4] (k <= 4), idx [...] -> [...,4,4] int16 with the table's k
+    rectangles in slots 0..k-1; slots 2-3 come from idx_dual (k = 2 tables only), else the rest is empty."""
     idx = np.asarray(idx)
+    k = table.shape[1]
+    if k > 4 or (idx_dual is not None and k > 2):
+        raise ValueError("gather: %d-rectangle table%s exceeds the 4 rectangle slots of a sample"
+                         % (k, " with idx_dual" if idx_dual is not None else ""))
     out = np.zeros(idx.shape + (4, 4), np.int16)
-    out[..., 0:2, :] = table[idx]
+    out[..., 0:k, :] = table[idx]
     if idx_dual is not None:
         out[..., 2:4, :] = table[np.asarray(idx_dual)]
     return out
