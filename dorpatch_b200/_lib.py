@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libdorpatch.so")
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 c_i32, c_i64, c_f32, c_vp = C.c_int32, C.c_int64, C.c_float, C.c_void_p
 
@@ -63,6 +63,7 @@ SIGNATURES = {
     "dp_attack_update": (c_i32, [c_vp, C.POINTER(DpUpdateArgs), c_vp]),
     "dp_attack_step_host": (c_i32, [c_vp, C.POINTER(DpAttackArgs), C.POINTER(DpUpdateArgs), c_vp]),
     "dp_net_forward_backward": (c_i32, [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    "dp_failed_set_reset": (c_i32, [c_vp, c_i32, c_vp]),
     "dp_failed_set_write": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_vp]),
     "dp_failed_set_update": (c_i32, [c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_f32, c_vp, c_vp]),
     "dp_failed_set_read": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_vp, c_vp]),

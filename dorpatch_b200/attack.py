@@ -16,7 +16,10 @@ Semantics beyond the reference (see DESIGN.md):
     a TypeError in the reference) pass the label.
   * EOT sharding: with torch.distributed initialised, each rank evaluates S/world samples and
     the ranks all-reduce the patch gradient once per step; the periodic universe scan
-    (collect_failure) is split over the ranks by mask index and its fail bits all-gathered.
+    (collect_failure) is split over the ranks by distinct occlusion and its fail bits all-gathered.
+  * ``pc_n_patch=2`` draws the universe from the two-patch PatchCleanser window (the reference
+    always uses the one-patch window, attack.py:25-31); the universe scans forward each distinct
+    occlusion once.
 """
 import os
 
@@ -225,12 +228,15 @@ def exchange_shards(dist, G, loss_adv, preds, defer=False):
     return loss_all, preds_all
 
 
-def scan_failures(predict, all_rects, y, targeted, dist=None, device="cpu"):
+def scan_failures(predict, all_rects, y, targeted, dist=None, device="cpu", inv=None):
     """collect_failure for one image (attack.py:384-406): indices of the universe masks under
     which the attack fails.  `predict(rects[k,4,4]) -> labels[k]`.  With torch.distributed the
     universe is split into contiguous shards, one per rank (SURVEY section 8e: the scan is
     embarrassingly parallel over the mask index), and the fail bits are all-gathered, so every
-    rank returns the identical list and takes the identical bookkeeping decisions."""
+    rank returns the identical list and takes the identical bookkeeping decisions.
+    With `inv`, all_rects holds the universe's distinct occlusions (masks.distinct_occlusions) and
+    universe mask k is all_rects[inv[k]]: each occlusion is forwarded once (on one rank) and its
+    result spread to every index sharing it, so the list is the one the full scan returns."""
     n = all_rects.shape[0]
     if dist is None:
         f = np.asarray(predict(all_rects)) == y
@@ -245,6 +251,8 @@ def scan_failures(predict, all_rects, y, targeted, dist=None, device="cpu"):
         outs = [torch.empty_like(bits) for _ in range(world)]
         dist.all_gather(outs, bits)
         f = torch.cat(outs).cpu().numpy()[:n].astype(bool)
+    if inv is not None:
+        f = f[inv]
     if targeted:
         f = ~f
     return np.nonzero(f)[0].tolist()
@@ -258,17 +266,25 @@ class DorPatch(object):
     def generate(self, model, x, patch_budget, n_classes, save_dir, batch_id, y=None, targeted=False,
                  lr=1e-2, confidence=1e-1, clip_min=0, clip_max=1, max_iterations=5000, basic_unit=7,
                  selection='topk', dropout=2, sampling_size=128, density=1e-3, structured=1e-3, eps=4., dual=False,
-                 eot_affine=0.0, eot_colour=0.0, eot_seed=0, **kwargs):
+                 eot_affine=0.0, eot_colour=0.0, eot_seed=0, pc_n_patch=1, **kwargs):
         """Reference signature (attack.py:51-53) plus three opt-in keywords for the affine / colour
         EOT extension (default 0 = off = the reference's behaviour).  `image_seeds=[s_0..s_{B-1}]` (keyword)
         makes row b of a B > 1 call replay the B == 1 run seeded with s_b (SURVEY section 0: parity of the
-        batched configs is defined per image against a B == 1 reference run)."""
+        batched configs is defined per image against a B == 1 reference run).
+        `pc_n_patch=2` trains against the two-patch PatchCleanser: the EOT occlusions and the universe scans come from
+        MaskWindow(W, r, 2) (dropout 1: its 630 pairs per ratio; dropout 2: its 22 680 three-rectangle masks per ratio)
+        instead of the reference's one-patch window (1, the default)."""
         if basic_unit != 7:
             raise NotImplementedError("the native kernels are built for basic_unit=7")
         if selection != 'topk':
             raise NotImplementedError("selection=%r" % (selection,))
         if dropout not in (1, 2):
             raise NotImplementedError("dropout=%r (the reference's dropout=0 path is degenerate)" % (dropout,))
+        if pc_n_patch not in (1, 2):
+            raise NotImplementedError("pc_n_patch=%r: PatchCleanser masks exist for 1 or 2 patches" % (pc_n_patch,))
+        if dual and pc_n_patch == 2 and dropout == 2:
+            raise NotImplementedError("dual=True with pc_n_patch=2, dropout=2 needs 6 rectangles per sample; "
+                                      "the native kernels take 4")
         net = unwrap_native(model)
         if not x.is_cuda:
             raise RuntimeError("DorPatch.generate needs CUDA tensors: the hot loop exists only as native sm_90a kernels")
@@ -306,13 +322,14 @@ class DorPatch(object):
         torch.nn.Conv2d(1, 1, basic_unit, stride=basic_unit, bias=False)
         torch.nn.Conv2d(1, 1, W // 8, stride=W // 8, bias=False)
 
-        table = _masks.universe(W, dropout)                      # attack.py:83-85 as rectangles
+        table = _masks.universe(W, dropout, pc_n_patch)          # attack.py:83-85 as rectangles
         n_mask = table.shape[0]
         S = min(sampling_size, n_mask)
         if S % world != 0:
             raise ValueError("sampling_size=%d must be divisible by the world size %d" % (S, world))
         S_loc = S // world
-        all_rects = _masks.gather(table, np.arange(n_mask))      # [n_mask,4,4] for the scans
+        distinct, inv = _masks.distinct_occlusions(table, len(_masks.DROPOUT_SIZES))   # scans forward each once
+        scan_rects = _masks.gather(distinct, np.arange(len(distinct)))
 
         if image_seeds is not None:
             rngs = [np.random.RandomState(int(s)) for s in image_seeds]
@@ -321,8 +338,9 @@ class DorPatch(object):
         else:
             rngs = [np.random.RandomState(int(np.random.randint(0, 2 ** 31 - 1))) for _ in range(B)]
         st = [_ImageState(lr, structured, y[b], targeted, rngs[b]) for b in range(B)]
-        device_sets = os.environ.get("DORPATCH_FAILED", "device") != "host" and n_mask <= 4096
+        device_sets = os.environ.get("DORPATCH_FAILED", "device") != "host"
         if device_sets:                                          # failed-mask sets as device bitmaps (SURVEY 8f N2)
+            eng.failed_reset(n_mask)
             for b, s in enumerate(st):
                 s.dev = (eng, b)
                 s.set_failed([])
@@ -337,17 +355,15 @@ class DorPatch(object):
         have_stale = False
         last_preds = None
         steps = 0
+        scans = [0, 0]                                           # universe scans, dp_predict forwards they issued here
 
         def scan(b, adv_x):                                      # collect_failure, attack.py:384-406
-            if dist is None:
-                preds = eng.predict(adv_x[b:b + 1], n_mask, all_rects)
-                f = preds == st[b].y
-                if st[b].targeted:
-                    f = ~f
-                failed = np.nonzero(f)[0].tolist()
-            else:                                                # universe split over the ranks by mask index
-                failed = scan_failures(lambda r: eng.predict(adv_x[b:b + 1], r.shape[0], r), all_rects, st[b].y,
-                                       st[b].targeted, dist, dev)
+            def predict(r):
+                scans[1] += r.shape[0]
+                return eng.predict(adv_x[b:b + 1], r.shape[0], r)
+            # distinct occlusions split over the ranks (if any), the result expanded to every universe index
+            failed = scan_failures(predict, scan_rects, st[b].y, st[b].targeted, dist, dev, inv=inv)
+            scans[0] += 1
             print(">> %d failures collected!" % len(failed))
             return failed
 
@@ -507,7 +523,8 @@ class DorPatch(object):
                         s.y, sw = _pick_target(last_preds[b], s.y)
                         s.crit_targeted = s.crit_targeted or sw
         sampler.shutdown(wait=True)
-        self.last_stats = dict(steps=steps, samples_per_step=B * S, final_labels=[s.y for s in st])
+        self.last_stats = dict(steps=steps, samples_per_step=B * S, final_labels=[s.y for s in st],
+                               scans=scans[0], scan_forwards=scans[1])
         return mask_best, pattern_best
 
     # ------------------------------------------------------------------------------------

@@ -182,8 +182,10 @@ struct dp_engine {
   float* adv_x = nullptr; float* dLs = nullptr; float* scale = nullptr; float* l2 = nullptr;
   float* loss_struc = nullptr; float* loss_density = nullptr; float* group_lasso = nullptr;
   float* win_dev = nullptr; float* grp_ss = nullptr;
-  // failed-mask sets (N2): one bitmap of FAILED_WORDS words per image, its popcounts, staging for one step's indices
-  static constexpr int FAILED_WORDS = 128;        // up to 4096 masks (the reference's universe has 2520)
+  // failed-mask sets (N2): one bitmap of failed_words words per image over failed_masks indices, its popcounts, staging
+  // for one step's indices.  4096 masks until dp_failed_set_reset sizes the sets by the universe (the reference's
+  // one-patch universe has 2520; the two-patch dropout-2 universe 90 720, 2835 words per image)
+  int failed_masks = 4096, failed_words = 128, failed_words_alloc = 128;
   uint32_t* failed_bits = nullptr; int32_t* failed_count = nullptr; int32_t* failed_idx = nullptr; int32_t* failed_nff = nullptr;
   uint8_t* failed_active = nullptr; float* failed_loss = nullptr; int failed_cap = 0;
   float* helper_scale = nullptr; float* helper_l2 = nullptr; float* helper_ws = nullptr;   // scratch of dp_paste(out) / dp_window_sum
@@ -419,8 +421,8 @@ struct dp_engine {
     for (float** p : {&scale, &l2, &loss_struc, &loss_density, &group_lasso, &lr_d, &structured_d, &coeff_d, &helper_scale, &helper_l2})
       *p = (float*)dmalloc(B * 4);
     helper_ws = (float*)dmalloc(B * HW * 4);
-    failed_bits = (uint32_t*)dmalloc(B * FAILED_WORDS * 4);
-    CUDA_OK(cudaMemset(failed_bits, 0, B * FAILED_WORDS * 4));
+    failed_bits = (uint32_t*)dmalloc(B * failed_words_alloc * 4);
+    CUDA_OK(cudaMemset(failed_bits, 0, B * failed_words_alloc * 4));
     failed_count = (int32_t*)dmalloc(B * 4); failed_nff = (int32_t*)dmalloc(B * 4); failed_active = (uint8_t*)dmalloc(B);
     win_dev = (float*)dmalloc(B * 64 * 4);
     grp_ss = (float*)dmalloc(B * (H / UNIT) * (H / UNIT) * 4);
@@ -1348,18 +1350,38 @@ int32_t dp_net_forward_backward(dp_engine* e, const float* z, int32_t N, float* 
 }
 
 /* ---- failed-mask sets on the device (attack.py:96,187-190,259-267) ------------------------------------- */
+int32_t dp_failed_set_reset(dp_engine* e, int32_t n_mask, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  if (n_mask < 1) fail("dp_failed_set_reset: n_mask %d < 1", n_mask);
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int words = (int)(((int64_t)n_mask + 31) / 32);
+  const size_t B = (size_t)e->cfg.max_images;
+  if (words > e->failed_words_alloc) {                 // the old bitmaps stay in `allocs` until destroy
+    CUDA_OK(cudaStreamSynchronize(st));
+    e->failed_bits = (uint32_t*)e->dmalloc(B * words * 4);
+    e->failed_words_alloc = words;
+  }
+  e->failed_masks = n_mask;
+  e->failed_words = words;
+  CUDA_OK(cudaMemsetAsync(e->failed_bits, 0, B * words * 4, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  DP_CATCH
+}
+
 int32_t dp_failed_set_write(dp_engine* e, int32_t b, const int32_t* idx_host, int32_t n, void* stream) {
   DP_TRY
   if (!e) fail("null engine");
   if (b < 0 || b >= e->cfg.max_images) fail("image %d outside [0, max_images=%d)", b, e->cfg.max_images);
   CUDA_OK(cudaSetDevice(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  std::vector<uint32_t> w(dp_engine::FAILED_WORDS, 0u);
+  std::vector<uint32_t> w(e->failed_words, 0u);
   for (int i = 0; i < n; ++i) {
-    if (idx_host[i] < 0 || idx_host[i] >= dp_engine::FAILED_WORDS * 32) fail("mask index %d outside [0, %d)", idx_host[i], dp_engine::FAILED_WORDS * 32);
+    if (idx_host[i] < 0 || idx_host[i] >= e->failed_masks) fail("mask index %d outside [0, %d)", idx_host[i], e->failed_masks);
     w[idx_host[i] >> 5] |= 1u << (idx_host[i] & 31);
   }
-  CUDA_OK(cudaMemcpyAsync(e->failed_bits + (size_t)b * dp_engine::FAILED_WORDS, w.data(), w.size() * 4, cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(e->failed_bits + (size_t)b * e->failed_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaStreamSynchronize(st));
   DP_CATCH
 }
@@ -1379,7 +1401,7 @@ int32_t dp_failed_set_update(dp_engine* e, int32_t B, int32_t S, const int32_t* 
     e->failed_loss = (float*)e->dmalloc((size_t)e->failed_cap * 4);
   }
   for (int i = 0; i < N; ++i)
-    if (idx_host[i] < 0 || idx_host[i] >= dp_engine::FAILED_WORDS * 32) fail("mask index %d outside [0, %d)", idx_host[i], dp_engine::FAILED_WORDS * 32);
+    if (idx_host[i] < 0 || idx_host[i] >= e->failed_masks) fail("mask index %d outside [0, %d)", idx_host[i], e->failed_masks);
   CUDA_OK(cudaMemcpyAsync(e->failed_idx, idx_host, (size_t)N * 4, cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaMemcpyAsync(e->failed_nff, nff_host, (size_t)B * 4, cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaMemcpyAsync(e->failed_active, active_host, (size_t)B, cudaMemcpyHostToDevice, st));
@@ -1388,7 +1410,7 @@ int32_t dp_failed_set_update(dp_engine* e, int32_t B, int32_t S, const int32_t* 
     CUDA_OK(cudaMemcpyAsync(e->failed_loss, loss_host, (size_t)N * 4, cudaMemcpyHostToDevice, st));
     loss = e->failed_loss;
   } else if (N > e->cap_samples) fail("dp_failed_set_update: no device losses for %d samples", N);
-  dp::launch_failed_update(e->failed_bits, dp_engine::FAILED_WORDS, e->failed_idx, loss, e->failed_nff, e->failed_active, B, S, thresh,
+  dp::launch_failed_update(e->failed_bits, e->failed_words, e->failed_idx, loss, e->failed_nff, e->failed_active, B, S, thresh,
                            e->failed_count, st);
   KERNEL_OK(); ++e->launches;
   CUDA_OK(cudaMemcpyAsync(count_host, e->failed_count, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
@@ -1402,12 +1424,16 @@ int32_t dp_failed_set_read(dp_engine* e, int32_t b, int32_t* idx_host_out, int32
   if (b < 0 || b >= e->cfg.max_images) fail("image %d outside [0, max_images=%d)", b, e->cfg.max_images);
   CUDA_OK(cudaSetDevice(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  std::vector<uint32_t> w(dp_engine::FAILED_WORDS);
-  CUDA_OK(cudaMemcpyAsync(w.data(), e->failed_bits + (size_t)b * dp_engine::FAILED_WORDS, w.size() * 4, cudaMemcpyDeviceToHost, st));
+  std::vector<uint32_t> w(e->failed_words);
+  CUDA_OK(cudaMemcpyAsync(w.data(), e->failed_bits + (size_t)b * e->failed_words, w.size() * 4, cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
   int n = 0;
-  for (int i = 0; i < dp_engine::FAILED_WORDS * 32; ++i)
-    if (w[i >> 5] & (1u << (i & 31))) { if (n < cap && idx_host_out) idx_host_out[n] = i; ++n; }
+  for (int j = 0; j < e->failed_words; ++j)            // set bits only: the 90 720-mask universe is 2835 words
+    for (uint32_t v = w[j]; v; v &= v - 1) {
+      const int i = j * 32 + __builtin_ctz(v);
+      if (n < cap && idx_host_out) idx_host_out[n] = i;
+      ++n;
+    }
   if (n_out) *n_out = n;
   if (n > cap && idx_host_out) fail("dp_failed_set_read: %d indices, buffer holds %d", n, cap);
   DP_CATCH

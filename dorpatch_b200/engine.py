@@ -50,6 +50,7 @@ class Engine:
         cp, eb = C.c_int32(), C.c_int32()
         _lib.check(self.lib.dp_input_layout(self.handle, C.byref(cp), C.byref(eb)))
         self.c_pad, self.elem_bytes = cp.value, eb.value
+        self.failed_masks = 4096                 # capacity of the failed-mask sets until failed_reset
 
     def close(self):
         if getattr(self, "handle", None):
@@ -245,6 +246,11 @@ class Engine:
 
     # ------------------------------------------------------------------------------
     # failed-mask sets on the device (attack.py:96,187-190,259-267)
+    def failed_reset(self, n_mask):
+        """Size every image's failed set for a universe of n_mask masks and clear it (default capacity: 4096)."""
+        _lib.check(self.lib.dp_failed_set_reset(self.handle, int(n_mask), self._stream()))
+        self.failed_masks = int(n_mask)
+
     def failed_write(self, b, indices):
         a, p = _host(np.asarray(indices, dtype=np.int32).reshape(-1), np.int32)
         _lib.check(self.lib.dp_failed_set_write(self.handle, int(b), p, int(a.size), self._stream()))
@@ -262,10 +268,11 @@ class Engine:
         _lib.check(self.lib.dp_failed_set_update(self.handle, B, S, ip, np_, ap, lp, float(thresh), C.c_void_p(cnt.ctypes.data), self._stream()))
         return cnt
 
-    def failed_read(self, b, cap=4096):
-        out = np.empty(cap, np.int32)
+    def failed_read(self, b):
+        out = np.empty(self.failed_masks, np.int32)
         n = C.c_int32()
-        _lib.check(self.lib.dp_failed_set_read(self.handle, int(b), C.c_void_p(out.ctypes.data), cap, C.cast(C.byref(n), C.c_void_p), self._stream()))
+        _lib.check(self.lib.dp_failed_set_read(self.handle, int(b), C.c_void_p(out.ctypes.data), out.size,
+                                               C.cast(C.byref(n), C.c_void_p), self._stream()))
         return out[:n.value].tolist()
 
     # ------------------------------------------------------------------------------

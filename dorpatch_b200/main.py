@@ -3,11 +3,15 @@
 
 Flags added here (all excluded from the result-directory name so layouts stay compatible):
 --synthetic N, --random_init, --max_iterations, --sampling_size, --num_batches, --precision,
---chunk, --img_size, --seed, --pc_n_patch.
+--chunk, --img_size, --seed, --pc_n_patch, --attack_pc_n_patch.
 
 --pc_n_patch 2 evaluates against the two-patch PatchCleanser (MaskWindow(img, r, 2), reference
 defenses/PatchCleanser.py:34-37).  It does not change the generated patches, so a run on an existing
 result directory reuses them; its records go to adv_PC2_<i>.pt, apart from the one-patch adv_PC_<i>.pt.
+
+--attack_pc_n_patch 2 generates the patches against that window (DorPatch.generate(pc_n_patch=2)).  It changes the
+artefacts, so it is the exception to the rule above: the first path component gets `__attack_pc_n_patch=2`, and a
+two-patch run never resumes from, or overwrites, one-patch patches.  The usual run sets both flags to 2.
 """
 import argparse
 import os
@@ -57,6 +61,8 @@ parser.add_argument('--img_size', default=224, type=int, help='synthetic image s
 parser.add_argument('--seed', default=0, type=int, help='seed of the random-init weights')
 parser.add_argument('--pc_n_patch', default=1, type=int, choices=[1, 2],
                     help='patches the PatchCleanser evaluation is provisioned for (2: records in adv_PC2_<i>.pt)')
+parser.add_argument('--attack_pc_n_patch', default=1, type=int, choices=[1, 2],
+                    help='patches of the PatchCleanser window the EOT occlusions are drawn from (2: result path suffix)')
 
 
 def _init_distributed():
@@ -141,7 +147,8 @@ def main(args):
                     model, x, args.patch_budget, NUM_CLASSES_DICT[args.dataset], targeted=args.targeted,
                     y=target if args.targeted else None, lr=args.lr, num_patch=args.num_patch, dropout=args.dropout,
                     density=args.density, structured=args.structured, save_dir=result_dir, batch_id=i,
-                    eps=args.epsilon, max_iterations=args.max_iterations, sampling_size=args.sampling_size)
+                    eps=args.epsilon, max_iterations=args.max_iterations, sampling_size=args.sampling_size,
+                    pc_n_patch=args.attack_pc_n_patch)
                 if rank == 0:                     # every rank holds the identical result; one writer
                     torch.save(adv_mask, os.path.join(result_dir, "adv_mask_%d.pt" % i))
                     torch.save(adv_pattern, os.path.join(result_dir, "adv_pattern_%d.pt" % i))

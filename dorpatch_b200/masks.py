@@ -76,9 +76,35 @@ def _two_patch_set(img_size, patch_ratio, dropout):
     raise ValueError("dropout must be 1 or 2, got %r" % (dropout,))
 
 
-def universe(img_size, dropout, sizes=DROPOUT_SIZES):
-    """The attack's mask universe (attack.py:83-85): [n_mask,2,4] int16."""
-    return np.concatenate([mask_set(img_size, r, dropout) for r in sizes], axis=0)
+def universe(img_size, dropout, n_patch=1, sizes=DROPOUT_SIZES):
+    """The attack's mask universe (attack.py:83-85) drawn from the window for n_patch patches: the concatenation over
+    the four ratios of mask_set(img_size, r, dropout, n_patch).  n_patch 1: [144,2,4] / [2520,2,4]; n_patch 2:
+    [2520,2,4] / [90720,3,4], mask r*22680 + i*630 + j as in the reference's double_mask_set."""
+    return np.concatenate([mask_set(img_size, r, dropout, n_patch) for r in sizes], axis=0)
+
+
+def distinct_occlusions(table, n_sets=1):
+    """The distinct occlusions of a rectangle table [n,k,4] and the map back: (distinct [m,k,4], inv [n]) with
+    table[k] and distinct[inv[k]] occluding the same pixels.  The table is the concatenation of n_sets equally long
+    mask sets (the universe: one per ratio); two masks are the same occlusion when they lie in the same set and list
+    the same basic rectangles (order and repeats ignored).  distinct[j] is the first such mask of the table, and
+    distinct keeps the table's order, so a table without repeats maps to itself (inv = arange(n)).  The two-patch
+    dropout-2 universe holds each triple {i,a,b} of basic rectangles 3 times and each pair 2 times (mask
+    i*630 + pair(a,b) with i in {a,b}): 7 770 distinct occlusions per ratio out of 22 680."""
+    t = np.asarray(table).astype(np.int64)
+    n = t.shape[0]
+    if n % n_sets:
+        raise ValueError("a table of %d masks is not %d equally long sets" % (n, n_sets))
+    key = (t[..., 0] << 48) | (t[..., 1] << 32) | (t[..., 2] << 16) | t[..., 3]   # one int64 per rectangle; empty = 0
+    key = np.sort(key, axis=1)
+    key[:, 1:][key[:, 1:] == key[:, :-1]] = 0                                       # a repeated rectangle adds nothing
+    key = np.sort(key, axis=1)
+    key = np.concatenate([(np.arange(n) // (n // n_sets))[:, None], key], axis=1)  # never merge across sets
+    _, first, inv = np.unique(key, axis=0, return_index=True, return_inverse=True)
+    order = np.argsort(first)
+    rank = np.empty_like(order)
+    rank[order] = np.arange(len(order))
+    return np.ascontiguousarray(table[first[order]]), rank[inv.reshape(-1)]
 
 
 def gather(table, idx, idx_dual=None):

@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define DP_ABI_VERSION 6
+#define DP_ABI_VERSION 7
 
 enum dp_precision {
   DP_PREC_FP32 = 0, /* fp32 storage, fp32 FMA math (no tensor cores): parity checks   */
@@ -201,7 +201,10 @@ int32_t dp_net_forward_backward(dp_engine* e, const float* z, int32_t N, float* 
  * result of a universe scan); dp_failed_set_update applies one step -- idx_host [B*S] sampled mask indices, the first
  * nff_host[b] of image b drawn from its failed set, loss < thresh = success; loss_host NULL = use the CW losses the last
  * dp_attack_grad left on the device -- and returns the set sizes count_host[B] (all the bookkeeping of attack.py:269-308
- * needs); dp_failed_set_read returns the sorted indices (needed only when the sampler draws from the set, i >= 1000). */
+ * needs); dp_failed_set_read returns the sorted indices (needed only when the sampler draws from the set, i >= 1000).
+ * dp_failed_set_reset sizes every image's set for a universe of n_mask masks (ceil(n_mask/32) words each) and clears
+ * them; the three calls above then reject indices outside [0, n_mask).  An engine that never calls it holds 4096. */
+int32_t dp_failed_set_reset(dp_engine* e, int32_t n_mask, void* stream);
 int32_t dp_failed_set_write(dp_engine* e, int32_t b, const int32_t* idx_host, int32_t n, void* stream);
 int32_t dp_failed_set_update(dp_engine* e, int32_t B, int32_t S, const int32_t* idx_host, const int32_t* nff_host,
                              const uint8_t* active_host, const float* loss_host, float thresh, int32_t* count_host,
