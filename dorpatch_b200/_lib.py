@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libdorpatch.so")
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 c_i32, c_i64, c_f32, c_vp = C.c_int32, C.c_int64, C.c_float, C.c_void_p
 
@@ -25,7 +25,7 @@ class DpAttackArgs(C.Structure):
                 ("confidence", c_f32), ("eps", c_f32),
                 ("grad_adv", c_vp), ("loss_adv_host", c_vp), ("preds_host", c_vp),
                 ("loss_struc_host", c_vp), ("loss_density_host", c_vp), ("group_lasso_host", c_vp),
-                ("l2_host", c_vp), ("xform_host", c_vp)]
+                ("l2_host", c_vp), ("xform_host", c_vp), ("basic_unit", c_i32)]
 
 
 class DpUpdateArgs(C.Structure):

@@ -274,8 +274,12 @@ class DorPatch(object):
         `pc_n_patch=2` trains against the two-patch PatchCleanser: the EOT occlusions and the universe scans come from
         MaskWindow(W, r, 2) (dropout 1: its 630 pairs per ratio; dropout 2: its 22 680 three-rectangle masks per ratio)
         instead of the reference's one-patch window (1, the default)."""
-        if basic_unit != 7:
-            raise NotImplementedError("the native kernels are built for basic_unit=7")
+        W = x.shape[-1]
+        if isinstance(basic_unit, bool) or not isinstance(basic_unit, (int, np.integer)) or basic_unit < 1 \
+                or W % basic_unit != 0:
+            # the reference fails later on such a unit, at stage 1's clip broadcast
+            raise ValueError("basic_unit=%r must be a positive integer dividing the image size %d" % (basic_unit, W))
+        basic_unit = int(basic_unit)
         if selection != 'topk':
             raise NotImplementedError("selection=%r" % (selection,))
         if dropout not in (1, 2):
@@ -448,7 +452,8 @@ class DorPatch(object):
                     from . import eot as _eot
                     xf = _eot.sample(eot_rng, B, S, eot_affine, eot_colour)[:, rank * S_loc:(rank + 1) * S_loc]
                 r = eng.attack_grad(x, adv_mask, adv_pattern, rects, [s.y for s in st],
-                                    [s.crit_targeted for s in st], confidence, eps, stage, G, S_total=S, xforms=xf)
+                                    [s.crit_targeted for s in st], confidence, eps, stage, G, S_total=S, xforms=xf,
+                                    basic_unit=basic_unit)
                 loss_adv, preds = r["loss_adv"], r["preds"]
                 reduce_work = None
                 if dist:                                         # one all-reduce of the patch gradient per step, under the bookkeeping
@@ -529,14 +534,14 @@ class DorPatch(object):
 
     # ------------------------------------------------------------------------------------
     def patch_selection(self, mask, patch_budget, basic_unit=7, selection='topk'):
-        """attack.py:363-382: top-k 7x7 groups with positive importance -> binary mask.
-        Window sums on the device (native kernel); the k-of-1024 selection on the host."""
+        """attack.py:363-382: top-k basic_unit x basic_unit groups with positive importance -> binary mask.
+        Window sums on the device (native kernel); the k-of-(H/basic_unit)^2 selection on the host."""
         if selection != 'topk':
             raise NotImplementedError("selection=%r" % (selection,))
         from .runtime import shared_engine
         B, _, H, W = mask.shape
         eng = shared_engine(W, B)
-        imp = eng.window_sum(mask.contiguous().float(), basic_unit)                   # [B, (H/7)*(W/7)]
+        imp = eng.window_sum(mask.contiguous().float(), basic_unit)                   # [B, (H/u)*(W/u)]
         num_group = int(np.floor((H * W * patch_budget) / (basic_unit ** 2)))
         sel = np.zeros_like(imp)
         for b in range(B):

@@ -74,8 +74,6 @@ struct NvtxRange {
   NvtxRange& operator=(const NvtxRange&) = delete;
 };
 
-constexpr int UNIT = 7;   // basic_unit of the group lasso / patch selection (attack.py:52)
-
 struct ConvW {            // one convolution's weights (device, KRSC, activation dtype)
   int cin = 0, cin_pad = 0, cout = 0, k = 1, stride = 1, pad = 0;
   void* w = nullptr;
@@ -181,7 +179,8 @@ struct dp_engine {
   // per-image buffers (max_images)
   float* adv_x = nullptr; float* dLs = nullptr; float* scale = nullptr; float* l2 = nullptr;
   float* loss_struc = nullptr; float* loss_density = nullptr; float* group_lasso = nullptr;
-  float* win_dev = nullptr; float* grp_ss = nullptr;
+  float* win_dev = nullptr; float* grp_ss = nullptr;   // grp_ss: B*H*H floats, one per group at basic_unit 1
+  int unit = 7;   // basic_unit of the last dp_attack_grad (attack.py:52); dp_attack_update's group-lasso term uses it
   // failed-mask sets (N2): one bitmap of failed_words words per image over failed_masks indices, its popcounts, staging
   // for one step's indices.  4096 masks until dp_failed_set_reset sizes the sets by the universe (the reference's
   // one-patch universe has 2520; the two-patch dropout-2 universe 90 720, 2835 words per image)
@@ -241,7 +240,7 @@ struct dp_engine {
   // signature and replayed; the first call of a signature runs eagerly (it picks cuDNN / cublasLt algorithms, which
   // synchronises and cannot be captured).  DORPATCH_GRAPH=0 disables.
   struct GraphEnt { int calls = 0; bool failed = false; cudaGraphExec_t exec = nullptr; int64_t launches = 0; };
-  typedef std::tuple<int, int, int, int, const void*, const void*, const void*, const void*, float, float, int> GraphKey;
+  typedef std::tuple<int, int, int, int, const void*, const void*, const void*, const void*, float, float, int, int> GraphKey;
   std::map<GraphKey, GraphEnt> graphs;
   bool graphs_on = true;
   cudaStream_t cap_stream = nullptr;   // capture happens here when the caller's stream is the legacy / per-thread default stream (not capturable)
@@ -425,7 +424,7 @@ struct dp_engine {
     CUDA_OK(cudaMemset(failed_bits, 0, B * failed_words_alloc * 4));
     failed_count = (int32_t*)dmalloc(B * 4); failed_nff = (int32_t*)dmalloc(B * 4); failed_active = (uint8_t*)dmalloc(B);
     win_dev = (float*)dmalloc(B * 64 * 4);
-    grp_ss = (float*)dmalloc(B * (H / UNIT) * (H / UNIT) * 4);
+    grp_ss = (float*)dmalloc(B * HW * 4);
     ensure_samples(chunk);
     ensure_pin((size_t)4 << 20);
   }
@@ -1119,7 +1118,7 @@ static void attack_grad_enqueue(dp_engine* e, const dp_attack_args* a, const Gra
   PROF(e, "paste", 10.0 * img_bytes, 0, st, dp::launch_paste(a->x, a->mask, a->pattern, e->adv_x, e->l2, e->scale, B, H, H, a->eps, st)); KERNEL_OK(); ++e->launches;
   PROF(e, "struct", 9.0 * img_bytes, 0, st, dp::launch_struct(e->adv_x, a->x, e->loss_struc, e->dLs, B, H, H, st)); KERNEL_OK(); ++e->launches;
   if (a->stage == 0) {
-    PROF(e, "maskreg", img_bytes, 0, st, dp::launch_maskreg(a->mask, e->loss_density, e->group_lasso, e->win_dev, e->grp_ss, B, H, H, UNIT, st)); KERNEL_OK(); ++e->launches;
+    PROF(e, "maskreg", img_bytes, 0, st, dp::launch_maskreg(a->mask, e->loss_density, e->group_lasso, e->win_dev, e->grp_ss, B, H, H, e->unit, st)); KERNEL_OK(); ++e->launches;
   }
   const float inv_s = 1.0f / (float)a->S_total;
   // Two lanes: chunks alternate between two workspaces / internal streams (only when every chunk holds whole
@@ -1198,6 +1197,9 @@ static void attack_grad_impl(dp_engine* e, const dp_attack_args* a, cudaStream_t
   if (a->S < 1 || a->S_total < a->S) fail("bad S=%d / S_total=%d", a->S, a->S_total);
   if (!a->x || !a->mask || !a->pattern || !a->grad_adv || !a->y_host || !a->targeted_host) fail("null pointer in dp_attack_args");
   const int B = a->B, S = a->S, N = B * S;
+  const int unit = a->basic_unit == 0 ? 7 : a->basic_unit;
+  if (unit < 1 || e->H % unit != 0) fail("basic_unit=%d does not divide the image size %d", unit, e->H);
+  e->unit = unit;
   e->ensure_samples(N);
   if (!a->xform_host) e->ensure_net_in_all(N);
   // per-sample labels / criterion flags / rectangles -> pinned staging.  Layout:
@@ -1220,7 +1222,7 @@ static void attack_grad_impl(dp_engine* e, const dp_attack_args* a, cudaStream_t
 
   bool done = false;
   if (e->graphs_on && !e->prof_on && !L_.xf_bytes) {
-    dp_engine::GraphKey key{B, S, a->S_total, a->stage, a->x, a->mask, a->pattern, a->grad_adv, a->eps, a->confidence, L_.rect_bytes ? 1 : 0};
+    dp_engine::GraphKey key{B, S, a->S_total, a->stage, a->x, a->mask, a->pattern, a->grad_adv, a->eps, a->confidence, L_.rect_bytes ? 1 : 0, unit};
     dp_engine::GraphEnt& ent = e->graphs[key];
     ++ent.calls;
     if (ent.exec != nullptr) {
@@ -1286,7 +1288,7 @@ static void attack_update_impl(dp_engine* e, const dp_update_args* u, cudaStream
   CUDA_OK(cudaMemcpyAsync(e->coeff_d, h + 2 * B, (size_t)B * 4, cudaMemcpyHostToDevice, st));
   PROF(e, "update_k3", (double)B * e->H * e->H * 4 * (u->stage == 0 ? 15.0 : 13.0), 0, st,
        dp::launch_update(u->x, u->mask, u->pattern, u->grad_adv, e->dLs, e->scale, e->win_dev, e->grp_ss, e->lr_d, e->structured_d,
-                         e->coeff_d, u->density, u->clip_min, u->clip_max, u->stage, u->grad_pattern_out, u->grad_mask_out, u->grad_pattern_bias, B, e->H, e->H, UNIT, st));
+                         e->coeff_d, u->density, u->clip_min, u->clip_max, u->stage, u->grad_pattern_out, u->grad_mask_out, u->grad_pattern_bias, B, e->H, e->H, e->unit, st));
   KERNEL_OK(); ++e->launches;
   CUDA_OK(cudaStreamSynchronize(st));   // `pin` may be reused by the next call
 }

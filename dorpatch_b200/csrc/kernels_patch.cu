@@ -658,41 +658,62 @@ void launch_struct(const float* adv_x, const float* x, float* loss_struc, float*
 }
 
 // =====================================================================================
-// density + group lasso (attack.py:72-80,235-245).  One CTA per image.
+// density + group lasso (attack.py:72-80,235-245) for any basic_unit `unit` dividing H == W.  One CTA per image; no
+// shared memory scales with the group count (unit = 1 at 224 px is 50 176 groups), and every sum has a fixed order.
 //   grp_ss[b][g]  = sum of m^2 over the unit x unit group g          (for d GL / d m = unit*m/sqrt(ss))
 //   win_dev[b][w] = 2*(ws_w - mean)/(nw-1) for density window w      (d var / d m inside window w)
 // =====================================================================================
 __global__ void __launch_bounds__(1024) maskreg_kernel(const float* __restrict__ mask, float* __restrict__ loss_density,
                                                        float* __restrict__ group_lasso, float* __restrict__ win_dev,
                                                        float* __restrict__ grp_ss, int H, int W, int unit) {
-  extern __shared__ float sh[];
   __shared__ float red[32];
-  const int b = blockIdx.x, GH = H / unit, GW = W / unit, NG = GH * GW;
-  float* g_s = sh;            // [NG] plain sums
-  float* g_q = sh + NG;       // [NG] sums of squares
+  __shared__ float ws[64];
+  const int b = blockIdx.x, GW = W / unit, NG = (H / unit) * GW;
   const float* mb = mask + (size_t)b * H * W;
+  float gl = 0.f;
   for (int g = threadIdx.x; g < NG; g += blockDim.x) {
     const int gy = g / GW, gx = g % GW;
-    float s = 0.f, q = 0.f;
+    float q = 0.f;
     for (int dy = 0; dy < unit; ++dy)
-      for (int dx = 0; dx < unit; ++dx) { const float m = mb[(gy * unit + dy) * W + gx * unit + dx]; s += m; q = fmaf(m, m, q); }
-    g_s[g] = s; g_q[g] = q;
+      for (int dx = 0; dx < unit; ++dx) { const float m = mb[(gy * unit + dy) * W + gx * unit + dx]; q = fmaf(m, m, q); }
     grp_ss[(size_t)b * NG + g] = q;
+    gl += sqrtf(q);
   }
-  __syncthreads();
-  float gl = 0.f;
-  for (int g = threadIdx.x; g < NG; g += blockDim.x) gl += sqrtf(g_q[g]);
   gl = block_sum(gl, red);
   if (threadIdx.x == 0) group_lasso[b] = (float)unit * gl;
-  // density windows: (W/8) x (W/8) pixels = (W/8/unit)^2 groups each, 8 x 8 windows
-  const int win = W / 8, gpw = win / unit, NWX = W / win, NWY = H / win, NW = NWX * NWY;
-  __shared__ float ws[64];
-  if ((int)threadIdx.x < NW) {
-    const int wy = threadIdx.x / NWX, wx = threadIdx.x % NWX;
+  // density windows: 8 x 8 windows of (W/8) x (W/8) pixels
+  const int win = W / 8, NWX = W / win, NWY = H / win, NW = NWX * NWY;
+  if (unit > 1 && win % unit == 0) {
+    // one thread per window: its (win/unit)^2 group sums, each in row-major pixel order, added row-major -- the order
+    // in which the unit = 7 engine has always summed, kept so that the default path's bits do not move
+    if ((int)threadIdx.x < NW) {
+      const int wy = threadIdx.x / NWX, wx = threadIdx.x % NWX;
+      const float* wb = mb + (size_t)wy * win * W + wx * win;
+      const int gpw = win / unit;
+      float s = 0.f;
+      for (int a = 0; a < gpw; ++a)
+        for (int c = 0; c < gpw; ++c) {
+          float gs = 0.f;
+          for (int dy = 0; dy < unit; ++dy)
+            for (int dx = 0; dx < unit; ++dx) gs += wb[(a * unit + dy) * W + c * unit + dx];
+          s += gs;
+        }
+      ws[threadIdx.x] = s;
+    }
+  } else {
+    // groups of one pixel, or groups straddling / exceeding the window: its pixels, 16 threads per window (rows
+    // strided over them, a fixed shuffle tree across the 16)
+    const int w = threadIdx.x >> 4, part = threadIdx.x & 15;
     float s = 0.f;
-    for (int a = 0; a < gpw; ++a)
-      for (int c = 0; c < gpw; ++c) s += g_s[(wy * gpw + a) * GW + wx * gpw + c];
-    ws[threadIdx.x] = s;
+    if (w < NW) {
+      const float* wb = mb + (size_t)(w / NWX) * win * W + (w % NWX) * win;
+      for (int y = part; y < win; y += 16)
+#pragma unroll 7
+        for (int x = 0; x < win; ++x) s += wb[y * W + x];
+    }
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (w < NW && part == 0) ws[w] = s;
   }
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -707,8 +728,7 @@ __global__ void __launch_bounds__(1024) maskreg_kernel(const float* __restrict__
 }
 void launch_maskreg(const float* mask, float* loss_density, float* group_lasso, float* win_dev, float* grp_ss,
                     int B, int H, int W, int unit, cudaStream_t st) {
-  const int NG = (H / unit) * (W / unit);
-  maskreg_kernel<<<B, 1024, 2 * NG * sizeof(float), st>>>(mask, loss_density, group_lasso, win_dev, grp_ss, H, W, unit);
+  maskreg_kernel<<<B, 1024, 0, st>>>(mask, loss_density, group_lasso, win_dev, grp_ss, H, W, unit);
 }
 
 // =====================================================================================

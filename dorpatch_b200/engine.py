@@ -165,8 +165,9 @@ class Engine:
 
     # ------------------------------------------------------------------------------
     def attack_grad(self, x, mask, pattern, rects, y, crit_targeted, confidence, eps, stage, grad_adv,
-                    S_total=None, host=False, xforms=None):
-        """attack.py:184-247.  rects [B,S,4,4] int16; y [B]; crit_targeted [B] bool.
+                    S_total=None, host=False, xforms=None, basic_unit=7):
+        """attack.py:184-247.  rects [B,S,4,4] int16; y [B]; crit_targeted [B] bool; basic_unit: side of the
+        group-lasso groups (must divide H), which the following attack_update also uses.
         Fills grad_adv [B,3,H,W] and returns a dict of host numpy results."""
         B = x.shape[0]
         rects = np.ascontiguousarray(rects, dtype=np.int16)
@@ -179,6 +180,7 @@ class Engine:
                    group_lasso=np.zeros(B, np.float32), l2=np.empty(B, np.float32))
         a = _lib.DpAttackArgs()
         a.B, a.S, a.S_total, a.stage = B, S, int(S_total or S), int(stage)
+        a.basic_unit = int(basic_unit)
         if host:
             self._keep = [np.ascontiguousarray(t, np.float32) for t in (x, mask, pattern)]
             a.x, a.mask, a.pattern = [t.ctypes.data for t in self._keep]

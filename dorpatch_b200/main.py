@@ -3,7 +3,7 @@
 
 Flags added here (all excluded from the result-directory name so layouts stay compatible):
 --synthetic N, --random_init, --max_iterations, --sampling_size, --num_batches, --precision,
---chunk, --img_size, --seed, --pc_n_patch, --attack_pc_n_patch.
+--chunk, --img_size, --seed, --pc_n_patch, --attack_pc_n_patch, --basic_unit.
 
 --pc_n_patch 2 evaluates against the two-patch PatchCleanser (MaskWindow(img, r, 2), reference
 defenses/PatchCleanser.py:34-37).  It does not change the generated patches, so a run on an existing
@@ -12,6 +12,10 @@ result directory reuses them; its records go to adv_PC2_<i>.pt, apart from the o
 --attack_pc_n_patch 2 generates the patches against that window (DorPatch.generate(pc_n_patch=2)).  It changes the
 artefacts, so it is the exception to the rule above: the first path component gets `__attack_pc_n_patch=2`, and a
 two-patch run never resumes from, or overwrites, one-patch patches.  The usual run sets both flags to 2.
+
+--basic_unit N (default 7, the reference's) sets the side of the square cells the group lasso and patch_selection work
+on (DorPatch.generate(basic_unit=N)); it must divide the image size.  It changes the patches and the stage-0 mask, so a
+non-default unit is also appended to the first path component (`__basic_unit=N`).
 """
 import argparse
 import os
@@ -63,6 +67,8 @@ parser.add_argument('--pc_n_patch', default=1, type=int, choices=[1, 2],
                     help='patches the PatchCleanser evaluation is provisioned for (2: records in adv_PC2_<i>.pt)')
 parser.add_argument('--attack_pc_n_patch', default=1, type=int, choices=[1, 2],
                     help='patches of the PatchCleanser window the EOT occlusions are drawn from (2: result path suffix)')
+parser.add_argument('--basic_unit', default=7, type=int,
+                    help='side of the group-lasso / patch-selection cells, dividing the image size (non-7: path suffix)')
 
 
 def _init_distributed():
@@ -148,7 +154,7 @@ def main(args):
                     y=target if args.targeted else None, lr=args.lr, num_patch=args.num_patch, dropout=args.dropout,
                     density=args.density, structured=args.structured, save_dir=result_dir, batch_id=i,
                     eps=args.epsilon, max_iterations=args.max_iterations, sampling_size=args.sampling_size,
-                    pc_n_patch=args.attack_pc_n_patch)
+                    pc_n_patch=args.attack_pc_n_patch, basic_unit=args.basic_unit)
                 if rank == 0:                     # every rank holds the identical result; one writer
                     torch.save(adv_mask, os.path.join(result_dir, "adv_mask_%d.pt" % i))
                     torch.save(adv_pattern, os.path.join(result_dir, "adv_pattern_%d.pt" % i))

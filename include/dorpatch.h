@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define DP_ABI_VERSION 7
+#define DP_ABI_VERSION 8
 
 enum dp_precision {
   DP_PREC_FP32 = 0, /* fp32 storage, fp32 FMA math (no tensor cores): parity checks   */
@@ -154,6 +154,9 @@ typedef struct dp_attack_args {
    * behaviour): [B*S][8] = {t00,t01,t02,t10,t11,t12 (affine_grid theta, align_corners=False,
    * border padding), contrast, brightness}; applied to adv_x before the occlusion. */
   const float* xform_host;
+  /* side of the square groups of the group lasso (attack.py:52,72-74,243-245); 0 = 7, the
+   * reference's default.  Must divide H.  The density windows stay (H/8) x (H/8) pixels. */
+  int32_t basic_unit;
 } dp_attack_args;
 
 /* attack.py:184-247 up to (and including) backward; leaves per-image state
@@ -180,7 +183,7 @@ typedef struct dp_update_args {
 } dp_update_args;
 
 /* attack.py:332-342: theta -= lr * sign(grad theta); clip.  Must follow a
- * dp_attack_grad on the same (x, mask, pattern). */
+ * dp_attack_grad on the same (x, mask, pattern); its group-lasso term uses that call's basic_unit. */
 int32_t dp_attack_update(dp_engine* e, const dp_update_args* a, void* stream);
 
 /* Same step through HOST buffers (bench.py's e2e leg): copies x/mask/pattern in from
