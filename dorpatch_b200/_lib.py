@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libdorpatch.so")
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 c_i32, c_i64, c_f32, c_vp = C.c_int32, C.c_int64, C.c_float, C.c_void_p
 
@@ -59,6 +59,8 @@ SIGNATURES = {
     "dp_expand_step_dev": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
     "dp_input_layout": (c_i32, [c_vp, C.POINTER(c_i32), C.POINTER(c_i32)]),
     "dp_predict": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    "dp_eot_forward": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp]),
+    "dp_eot_backward": (c_i32, [c_vp, c_vp, c_vp, c_vp]),
     "dp_attack_grad": (c_i32, [c_vp, C.POINTER(DpAttackArgs), c_vp]),
     "dp_attack_update": (c_i32, [c_vp, C.POINTER(DpUpdateArgs), c_vp]),
     "dp_attack_step_host": (c_i32, [c_vp, C.POINTER(DpAttackArgs), C.POINTER(DpUpdateArgs), c_vp]),

@@ -198,6 +198,17 @@ struct dp_engine {
   // pinned staging
   unsigned char* pin = nullptr; size_t pin_bytes = 0;
 
+  // ---- dp_eot_forward / dp_eot_backward: what the backward needs of the last forward.  fwd_gen is bumped by every
+  // call that overwrites the lane arenas (dp_predict, dp_attack_grad, dp_net_forward_backward, dp_eot_forward, new
+  // weights); a backward whose forward recorded an older generation is refused.  eot_held[l] is the chunk whose saved
+  // activations (pre-norm outputs, GroupNorm statistics, max-pool argmax) lane l still holds, -1 none.
+  struct EotSig { int64_t gen = -1; const float* img = nullptr; int B = 0, S = 0; bool rects = false; };
+  int64_t fwd_gen = 0;
+  EotSig eot;
+  int eot_held[2] = {-1, -1};
+  int16_t* eot_rects_d = nullptr; int eot_rects_cap = 0;   // the forward's rectangles (rects_d is shared scratch)
+  void forward_clobbered() { ++fwd_gen; eot_held[0] = eot_held[1] = -1; }
+
   // ---- optional per-category profiler (CUDA events around every launch) --------------
   bool prof_on = false;
   struct ProfRec { int cat; cudaEvent_t a, b; double bytes, flops; };
@@ -494,6 +505,7 @@ struct dp_engine {
     }
     cudaFree(tmp);
     weights_loaded = true;
+    forward_clobbered();
   }
 
   // ---- cuDNN convolution -------------------------------------------------------------
@@ -1066,6 +1078,7 @@ int32_t dp_predict(dp_engine* e, const float* img, int32_t B, int32_t S, const i
   CUDA_OK(cudaSetDevice(e->cfg.device));
   const int N = B * S;
   if (N < 1) fail("dp_predict: empty batch");
+  e->forward_clobbered();
   e->h2d_samples(rects_host, N, st);
   // forward-only scan (collect_failure, PatchCleanser): chunks alternate between the two lanes like dp_attack_grad
   cudaStream_t const user_st = st;
@@ -1200,6 +1213,7 @@ static void attack_grad_impl(dp_engine* e, const dp_attack_args* a, cudaStream_t
   const int unit = a->basic_unit == 0 ? 7 : a->basic_unit;
   if (unit < 1 || e->H % unit != 0) fail("basic_unit=%d does not divide the image size %d", unit, e->H);
   e->unit = unit;
+  e->forward_clobbered();
   e->ensure_samples(N);
   if (!a->xform_host) e->ensure_net_in_all(N);
   // per-sample labels / criterion flags / rectangles -> pinned staging.  Layout:
@@ -1333,6 +1347,162 @@ int32_t dp_attack_step_host(dp_engine* e, const dp_attack_args* g, const dp_upda
   DP_CATCH
 }
 
+/* ---- differentiable classifier: model(occlude(img)) and its input gradient as two calls ------------------------- */
+// Forward: dp_predict's chunk loop with the activations kept (train=true); K1 once for the whole call when its output
+// fits net_in_all, as dp_attack_grad does.  Lane l ends up holding its last chunk.
+static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const int16_t* rects_host, float* logits,
+                             cudaStream_t st) {
+  NvtxRange nvtx_("dorpatch.eot_forward");
+  if (!img || !logits) fail("dp_eot_forward: null pointer");
+  e->check_B(B);
+  if (S < 1) fail("dp_eot_forward: S=%d < 1", S);
+  if (!rects_host && S != 1) fail("dp_eot_forward: S=%d without rectangles (plain classification needs S=1)", S);
+  const int N = B * S, H = e->H;
+  e->forward_clobbered();
+  e->eot = dp_engine::EotSig{};
+  if (rects_host) {
+    if (N > e->eot_rects_cap) {                          // the old table stays in `allocs` until destroy
+      e->eot_rects_cap = std::max(N, e->eot_rects_cap * 2);
+      e->eot_rects_d = (int16_t*)e->dmalloc((size_t)e->eot_rects_cap * 16 * sizeof(int16_t));
+    }
+    const size_t bytes = (size_t)N * 16 * sizeof(int16_t);
+    e->ensure_pin(bytes);
+    memcpy(e->pin, rects_host, bytes);
+    CUDA_OK(cudaMemcpyAsync(e->eot_rects_d, e->pin, bytes, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaStreamSynchronize(st));                  // `pin` is reused right after
+  }
+  const int16_t* rects = rects_host ? e->eot_rects_d : nullptr;
+  const bool whole = e->ensure_net_in_all(N);
+  if (whole) {
+    PROF(e, "expand_k1", (double)N * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)B, 0, st,
+         dp::launch_expand(img, nullptr, nullptr, nullptr, nullptr, rects, e->net_in_all, B, S, 0, N, H, H, e->Cp, e->bf16, false, e->num_sms, st));
+    KERNEL_OK(); ++e->launches;
+  }
+  cudaStream_t const user_st = st;
+  const bool dual = e->lanes.size() == 2 && N > e->chunk && !e->prof_on;
+  if (dual) {
+    CUDA_OK(cudaEventRecord(e->ev_prep, user_st));
+    for (auto& L : e->lanes) CUDA_OK(cudaStreamWaitEvent(L.stream, e->ev_prep, 0));
+  }
+  int chunk_id = 0;
+  for (int n0 = 0; n0 < N; n0 += e->chunk, ++chunk_id) {
+    const int n = std::min(e->chunk, N - n0);
+    const int lane = dual ? (chunk_id & 1) : 0;
+    e->use_lane(lane);
+    if (dual) st = e->lanes[lane].stream;
+    const void* chunk_in = e->net_in;
+    if (whole) {
+      chunk_in = (const char*)e->net_in_all + (size_t)n0 * e->sample_in_bytes();
+    } else {
+      PROF(e, "expand_k1", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
+           dp::launch_expand(img, nullptr, nullptr, nullptr, nullptr, rects, e->net_in, B, S, n0, n, H, H, e->Cp, e->bf16, false, e->num_sms, st));
+      KERNEL_OK(); ++e->launches;
+    }
+    e->forward(n, chunk_in, true, st);
+    CUDA_OK(cudaMemcpyAsync(logits + (size_t)n0 * e->K, e->logits, (size_t)n * e->K * 4, cudaMemcpyDeviceToDevice, st));
+    e->eot_held[lane] = chunk_id;
+  }
+  if (dual) {
+    for (auto& L : e->lanes) {
+      CUDA_OK(cudaEventRecord(L.done, L.stream));
+      CUDA_OK(cudaStreamWaitEvent(user_st, L.done, 0));
+    }
+  }
+  e->use_lane(0);
+  e->eot.gen = e->fwd_gen; e->eot.img = img; e->eot.B = B; e->eot.S = S; e->eot.rects = rects_host != nullptr;
+}
+
+// Backward: every chunk through dp_engine::backward and K1^T.  A chunk no lane holds any more is recomputed first (its
+// K1 slice, then the forward) in the lane whose held chunk is needed latest.  With whole images per chunk the lanes run
+// on their own streams, resident chunks first (each G[b] is written by one chunk); otherwise the chunks run in order on
+// the caller's stream, since an image's gradient is accumulated across its chunks and the first one overwrites it.
+static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cudaStream_t st) {
+  NvtxRange nvtx_("dorpatch.eot_backward");
+  if (!dlogits || !G) fail("dp_eot_backward: null pointer");
+  if (e->eot.gen < 0) fail("dp_eot_backward: no dp_eot_forward has run on this engine");
+  if (e->eot.gen != e->fwd_gen)
+    fail("dp_eot_backward: stale forward: another forward-type call (dp_predict, dp_attack_grad, dp_net_forward_backward, "
+         "dp_eot_forward or new weights) ran on this engine since the dp_eot_forward it would differentiate");
+  e->check_B(e->eot.B);
+  const int B = e->eot.B, S = e->eot.S, N = B * S, H = e->H, K = e->K;
+  const int n_chunks = (N + e->chunk - 1) / e->chunk, nl = (int)e->lanes.size();
+  const int16_t* rects = e->eot.rects ? e->eot_rects_d : nullptr;
+  const bool dual = nl == 2 && N > e->chunk && (e->chunk % S == 0) && !e->prof_on;
+  std::vector<int> order;
+  if (dual) {
+    for (int l = 0; l < nl; ++l) if (e->eot_held[l] >= 0) order.push_back(e->eot_held[l]);
+    for (int c = 0; c < n_chunks; ++c) if (c != e->eot_held[0] && c != e->eot_held[1]) order.push_back(c);
+  } else {
+    for (int c = 0; c < n_chunks; ++c) order.push_back(c);
+  }
+  cudaStream_t const user_st = st;
+  if (dual) {
+    CUDA_OK(cudaEventRecord(e->ev_prep, user_st));
+    for (auto& L : e->lanes) CUDA_OK(cudaStreamWaitEvent(L.stream, e->ev_prep, 0));
+  }
+  int last_lane = nl - 1;
+  for (size_t i = 0; i < order.size(); ++i) {
+    const int c = order[i], n0 = c * e->chunk, n = std::min(e->chunk, N - n0);
+    int lane = -1;
+    for (int l = 0; l < nl; ++l) if (e->eot_held[l] == c) lane = l;
+    const bool recompute = lane < 0;
+    if (recompute) {                                     // evict the held chunk needed latest (never again: latest)
+      size_t best_next = 0;
+      for (int k = 1; k <= nl; ++k) {
+        const int l = (last_lane + k) % nl;              // ties go round-robin, so recomputed chunks alternate lanes
+        size_t next = order.size();
+        for (size_t j = i + 1; j < order.size(); ++j) if (order[j] == e->eot_held[l]) { next = j; break; }
+        if (lane < 0 || next > best_next) { lane = l; best_next = next; }
+      }
+    }
+    last_lane = lane;
+    e->use_lane(lane);
+    if (dual) st = e->lanes[lane].stream;
+    if (recompute) {
+      e->eot_held[lane] = -1;
+      PROF(e, "expand_k1", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
+           dp::launch_expand(e->eot.img, nullptr, nullptr, nullptr, nullptr, rects, e->net_in, B, S, n0, n, H, H, e->Cp, e->bf16, false, e->num_sms, st));
+      KERNEL_OK(); ++e->launches;
+      e->forward(n, e->net_in, true, st);
+      e->eot_held[lane] = c;
+    }
+    // the caller's rows go to the lane's dlogits buffer: the head GEMM then reads what it reads in dp_attack_grad
+    CUDA_OK(cudaMemcpyAsync(e->dlogits, dlogits + (size_t)n0 * K, (size_t)n * K * 4, cudaMemcpyDeviceToDevice, st));
+    const bool fuse = e->stem_bwd_fused_ok();
+    dp_engine::FusedReduce fr{rects, G, B, S, n0};
+    e->backward(n, e->dlogits, st, fuse ? &fr : nullptr);
+    if (!fuse) {
+      PROF(e, "reduce_k1t", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
+           dp::launch_reduce(e->d_input, rects, G, B, S, n0, n, H, H, e->Cpd, e->bf16, st));
+      KERNEL_OK(); ++e->launches;
+    }
+  }
+  if (dual) {
+    for (auto& L : e->lanes) {
+      CUDA_OK(cudaEventRecord(L.done, L.stream));
+      CUDA_OK(cudaStreamWaitEvent(user_st, L.done, 0));
+    }
+  }
+  e->use_lane(0);
+}
+
+int32_t dp_eot_forward(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host, float* logits_dev,
+                       void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  eot_forward_impl(e, img, B, S, rects_host, logits_dev, (cudaStream_t)stream);
+  DP_CATCH
+}
+
+int32_t dp_eot_backward(dp_engine* e, const float* dlogits_dev, float* grad_img_dev, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  eot_backward_impl(e, dlogits_dev, grad_img_dev, (cudaStream_t)stream);
+  DP_CATCH
+}
+
 int32_t dp_net_forward_backward(dp_engine* e, const float* z, int32_t N, float* logits_dev, const float* dlogits_dev,
                                 float* dz_dev, void* stream) {
   DP_TRY
@@ -1340,6 +1510,7 @@ int32_t dp_net_forward_backward(dp_engine* e, const float* z, int32_t N, float* 
   CUDA_OK(cudaSetDevice(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   if (N < 1 || N > e->chunk) fail("N=%d outside [1, chunk=%d]", N, e->chunk);
+  e->forward_clobbered();
   dp::launch_pack_nchw(z, e->net_in, N, e->H, e->H, e->Cp, e->bf16, st); KERNEL_OK(); ++e->launches;
   e->forward(N, e->net_in, dlogits_dev != nullptr, st);
   if (logits_dev) CUDA_OK(cudaMemcpyAsync(logits_dev, e->logits, (size_t)N * e->K * 4, cudaMemcpyDeviceToDevice, st));

@@ -51,6 +51,8 @@ class Engine:
         _lib.check(self.lib.dp_input_layout(self.handle, C.byref(cp), C.byref(eb)))
         self.c_pad, self.elem_bytes = cp.value, eb.value
         self.failed_masks = 4096                 # capacity of the failed-mask sets until failed_reset
+        self.eot_forwards = 0                    # eot_forward calls so far (ops.eot_logits pairs a backward with its forward)
+        self._eot_shape = None
 
     def close(self):
         if getattr(self, "handle", None):
@@ -164,6 +166,26 @@ class Engine:
         return (preds, logits) if return_logits else preds
 
     # ------------------------------------------------------------------------------
+    def eot_forward(self, img, S=1, rects=None):
+        """model(occlude(img)) as [B*S, K] logits on the device (dp_predict's values), keeping what eot_backward needs.
+        img [B,3,H,W] fp32 in [0,1]; rects [B,S,4,4] int16 or None (then S must be 1)."""
+        B = img.shape[0]
+        N = B * int(S)
+        logits = torch.empty((N, self.n_classes), dtype=torch.float32, device=img.device)
+        rp = None
+        if rects is not None:
+            rects, rp = _host(np.asarray(rects).reshape(N, 4, 4), np.int16)
+        _lib.check(self.lib.dp_eot_forward(self.handle, _dev_ptr(img), B, int(S), rp, _dev_ptr(logits), self._stream()))
+        self.eot_forwards += 1
+        self._eot_shape = tuple(img.shape)
+        return logits
+
+    def eot_backward(self, dlogits, out=None):
+        """d<dlogits, logits>/d img of the last eot_forward, [B,3,H,W] (no weight gradients)."""
+        out = torch.empty(self._eot_shape, dtype=torch.float32, device=dlogits.device) if out is None else out
+        _lib.check(self.lib.dp_eot_backward(self.handle, _dev_ptr(dlogits), _dev_ptr(out), self._stream()))
+        return out
+
     def attack_grad(self, x, mask, pattern, rects, y, crit_targeted, confidence, eps, stage, grad_adv,
                     S_total=None, host=False, xforms=None, basic_unit=7):
         """attack.py:184-247.  rects [B,S,4,4] int16; y [B]; crit_targeted [B] bool; basic_unit: side of the

@@ -155,9 +155,14 @@ class ResNetV2(nn.Module):
         self._adopted = eng
 
     def forward(self, z):
-        """Logits of an already-normalised batch [N,3,H,W] (what timm's module computes)."""
+        """Logits of an already-normalised batch [N,3,H,W] (what timm's module computes).  Differentiable with
+        respect to z when z requires grad (``ops.eot_logits`` on z * 0.5 + 0.5, so the engine sees z up to one
+        rounding); the parameters get no gradient."""
         if not z.is_cuda:
             raise RuntimeError("dorpatch_b200.ResNetV2 runs on the native CUDA engine only (no CPU fallback)")
+        if torch.is_grad_enabled() and z.requires_grad:
+            from .ops import eot_logits
+            return eot_logits(self, z.float() * 0.5 + 0.5)
         eng = self.engine(z.shape[-1])
         z = z.contiguous().float()
         outs = [eng.net_forward_backward(z[i:i + eng.chunk]) for i in range(0, z.shape[0], eng.chunk)]

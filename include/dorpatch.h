@@ -16,6 +16,8 @@
  *                       utils.py:77-78 NormModel's (x-0.5)/0.5, fused       [K1]
  *   dp_predict          `model(adv_x_masked)` forward (attack.py:222,397;
  *                       defenses/PatchCleanser.py:72,86,109; main.py:91,156)  [K1+K2]
+ *   dp_eot_forward /    `logits = model(adv_x_masked); loss.backward()` with a
+ *   dp_eot_backward     loss of the caller's choosing (attack.py:222-247)  [K1,K2 | K2^T,K1^T]
  *   dp_attack_grad      attack.py:184-247: paste, EOT expansion, classifier
  *                       fwd + backward-to-input, CW loss (attack.py:16-23),
  *                       structural / density / group-lasso terms (:227-245),
@@ -35,7 +37,7 @@
 extern "C" {
 #endif
 
-#define DP_ABI_VERSION 8
+#define DP_ABI_VERSION 9
 
 enum dp_precision {
   DP_PREC_FP32 = 0, /* fp32 storage, fp32 FMA math (no tensor cores): parity checks   */
@@ -126,6 +128,18 @@ int32_t dp_input_layout(const dp_engine* e, int32_t* c_pad, int32_t* elem_bytes)
 /* preds_host[B*S] = argmax logits; logits_host[B*S*n_classes] optional (NULL to skip). */
 int32_t dp_predict(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host,
                    int32_t* preds_host, float* logits_host, void* stream);
+
+/* ---- differentiable classifier: forward and backward-to-input as two calls ---------------- */
+/* logits_dev[B*S, K] = model(occlude(img_b, rects[b*S+s])), img [B,3,H,W] fp32 dev in [0,1] (NormModel's 0.5/0.5
+ * normalisation fused, as in dp_predict); rects_host [B*S][4][4] or NULL (S must then be 1: plain classification).
+ * Keeps what dp_eot_backward needs.  The logits are dp_predict's, bit for bit. */
+int32_t dp_eot_forward(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host,
+                       float* logits_dev, void* stream);
+/* grad_img_dev[B,3,H,W] (overwritten) = sum_s d(<dlogits, logits>)/d img_b for the LAST dp_eot_forward on this engine.
+ * dlogits_dev [B*S, K] fp32 dev.  Fails if another forward-type call (dp_predict, dp_attack_grad,
+ * dp_net_forward_backward, weights) ran since.  May be called more than once per forward; reads img again for the
+ * chunks whose activations the engine no longer holds, so img must be unchanged.  No weight gradients. */
+int32_t dp_eot_backward(dp_engine* e, const float* dlogits_dev, float* grad_img_dev, void* stream);
 
 /* ---- hot loop ------------------------------------------------------------------------ */
 typedef struct dp_attack_args {
