@@ -61,6 +61,7 @@ SIGNATURES = {
     "dp_predict": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp]),
     "dp_eot_forward": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "dp_eot_backward": (c_i32, [c_vp, c_vp, c_vp, c_vp]),
+    "dp_eot_forward_xform": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp]),
     "dp_attack_grad": (c_i32, [c_vp, C.POINTER(DpAttackArgs), c_vp]),
     "dp_attack_update": (c_i32, [c_vp, C.POINTER(DpUpdateArgs), c_vp]),
     "dp_attack_step_host": (c_i32, [c_vp, C.POINTER(DpAttackArgs), C.POINTER(DpUpdateArgs), c_vp]),

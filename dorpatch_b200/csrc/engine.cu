@@ -13,6 +13,7 @@
 #include <cudnn.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -202,11 +203,13 @@ struct dp_engine {
   // call that overwrites the lane arenas (dp_predict, dp_attack_grad, dp_net_forward_backward, dp_eot_forward, new
   // weights); a backward whose forward recorded an older generation is refused.  eot_held[l] is the chunk whose saved
   // activations (pre-norm outputs, GroupNorm statistics, max-pool argmax) lane l still holds, -1 none.
-  struct EotSig { int64_t gen = -1; const float* img = nullptr; int B = 0, S = 0; bool rects = false; };
+  // xf: the forward warped its samples (dp_eot_forward_xform) with the transforms in eot_xf_d.
+  struct EotSig { int64_t gen = -1; const float* img = nullptr; int B = 0, S = 0; bool rects = false, xf = false; };
   int64_t fwd_gen = 0;
   EotSig eot;
   int eot_held[2] = {-1, -1};
   int16_t* eot_rects_d = nullptr; int eot_rects_cap = 0;   // the forward's rectangles (rects_d is shared scratch)
+  float* eot_xf_d = nullptr; int eot_xf_cap = 0;           // the forward's transforms (xf_d is dp_attack_grad's)
   void forward_clobbered() { ++fwd_gen; eot_held[0] = eot_held[1] = -1; }
 
   // ---- optional per-category profiler (CUDA events around every launch) --------------
@@ -1350,14 +1353,21 @@ int32_t dp_attack_step_host(dp_engine* e, const dp_attack_args* g, const dp_upda
 /* ---- differentiable classifier: model(occlude(img)) and its input gradient as two calls ------------------------- */
 // Forward: dp_predict's chunk loop with the activations kept (train=true); K1 once for the whole call when its output
 // fits net_in_all, as dp_attack_grad does.  Lane l ends up holding its last chunk.
-static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const int16_t* rects_host, float* logits,
-                             cudaStream_t st) {
-  NvtxRange nvtx_("dorpatch.eot_forward");
-  if (!img || !logits) fail("dp_eot_forward: null pointer");
+// With transforms (xf_host, [N][8]) each chunk's input is dp_attack_grad's affine expansion instead, read from img.
+static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const int16_t* rects_host, const float* xf_host,
+                             float* logits, cudaStream_t st) {
+  NvtxRange nvtx_(xf_host ? "dorpatch.eot_forward_xform" : "dorpatch.eot_forward");
+  const char* fn = xf_host ? "dp_eot_forward_xform" : "dp_eot_forward";
+  if (!img || !logits) fail("%s: null pointer", fn);
   e->check_B(B);
-  if (S < 1) fail("dp_eot_forward: S=%d < 1", S);
-  if (!rects_host && S != 1) fail("dp_eot_forward: S=%d without rectangles (plain classification needs S=1)", S);
+  if (S < 1) fail("%s: S=%d < 1", fn, S);
+  if (!rects_host && !xf_host && S != 1) fail("dp_eot_forward: S=%d without rectangles (plain classification needs S=1)", S);
   const int N = B * S, H = e->H;
+  if (xf_host)
+    for (size_t i = 0; i < (size_t)N * 8; ++i)
+      if (!std::isfinite(xf_host[i]))
+        fail("dp_eot_forward_xform: transform of sample %d has a non-finite value %g at position %d", (int)(i / 8),
+             (double)xf_host[i], (int)(i % 8));
   e->forward_clobbered();
   e->eot = dp_engine::EotSig{};
   if (rects_host) {
@@ -1371,8 +1381,19 @@ static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const
     CUDA_OK(cudaMemcpyAsync(e->eot_rects_d, e->pin, bytes, cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaStreamSynchronize(st));                  // `pin` is reused right after
   }
+  if (xf_host) {
+    if (N > e->eot_xf_cap) {                             // the old table stays in `allocs` until destroy
+      e->eot_xf_cap = std::max(N, e->eot_xf_cap * 2);
+      e->eot_xf_d = (float*)e->dmalloc((size_t)e->eot_xf_cap * 8 * sizeof(float));
+    }
+    const size_t bytes = (size_t)N * 8 * sizeof(float);
+    e->ensure_pin(bytes);
+    memcpy(e->pin, xf_host, bytes);
+    CUDA_OK(cudaMemcpyAsync(e->eot_xf_d, e->pin, bytes, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaStreamSynchronize(st));                  // `pin` is reused right after
+  }
   const int16_t* rects = rects_host ? e->eot_rects_d : nullptr;
-  const bool whole = e->ensure_net_in_all(N);
+  const bool whole = !xf_host && e->ensure_net_in_all(N);
   if (whole) {
     PROF(e, "expand_k1", (double)N * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)B, 0, st,
          dp::launch_expand(img, nullptr, nullptr, nullptr, nullptr, rects, e->net_in_all, B, S, 0, N, H, H, e->Cp, e->bf16, false, e->num_sms, st));
@@ -1393,6 +1414,10 @@ static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const
     const void* chunk_in = e->net_in;
     if (whole) {
       chunk_in = (const char*)e->net_in_all + (size_t)n0 * e->sample_in_bytes();
+    } else if (xf_host) {
+      PROF(e, "expand_affine", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
+           dp::launch_expand_affine(img, e->eot_xf_d, rects, e->net_in, S, n0, n, H, H, e->Cp, e->bf16, st));
+      KERNEL_OK(); ++e->launches;
     } else {
       PROF(e, "expand_k1", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
            dp::launch_expand(img, nullptr, nullptr, nullptr, nullptr, rects, e->net_in, B, S, n0, n, H, H, e->Cp, e->bf16, false, e->num_sms, st));
@@ -1410,12 +1435,16 @@ static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const
   }
   e->use_lane(0);
   e->eot.gen = e->fwd_gen; e->eot.img = img; e->eot.B = B; e->eot.S = S; e->eot.rects = rects_host != nullptr;
+  e->eot.xf = xf_host != nullptr;
 }
 
 // Backward: every chunk through dp_engine::backward and K1^T.  A chunk no lane holds any more is recomputed first (its
 // K1 slice, then the forward) in the lane whose held chunk is needed latest.  With whole images per chunk the lanes run
 // on their own streams, resident chunks first (each G[b] is written by one chunk); otherwise the chunks run in order on
 // the caller's stream, since an image's gradient is accumulated across its chunks and the first one overwrites it.
+// After a dp_eot_forward_xform, K1^T is the warp adjoint reduce_affine (after the unfused stem dgrad: the fused bf16
+// stem_bwd_reduce has no affine variant), which adds into G with atomics: G is zeroed first, and the same lane rule
+// keeps two streams from adding into one image.
 static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cudaStream_t st) {
   NvtxRange nvtx_("dorpatch.eot_backward");
   if (!dlogits || !G) fail("dp_eot_backward: null pointer");
@@ -1427,6 +1456,7 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
   const int B = e->eot.B, S = e->eot.S, N = B * S, H = e->H, K = e->K;
   const int n_chunks = (N + e->chunk - 1) / e->chunk, nl = (int)e->lanes.size();
   const int16_t* rects = e->eot.rects ? e->eot_rects_d : nullptr;
+  const bool xf = e->eot.xf;
   const bool dual = nl == 2 && N > e->chunk && (e->chunk % S == 0) && !e->prof_on;
   std::vector<int> order;
   if (dual) {
@@ -1436,6 +1466,7 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
     for (int c = 0; c < n_chunks; ++c) order.push_back(c);
   }
   cudaStream_t const user_st = st;
+  if (xf) CUDA_OK(cudaMemsetAsync(G, 0, (size_t)B * 3 * H * H * sizeof(float), user_st));
   if (dual) {
     CUDA_OK(cudaEventRecord(e->ev_prep, user_st));
     for (auto& L : e->lanes) CUDA_OK(cudaStreamWaitEvent(L.stream, e->ev_prep, 0));
@@ -1460,18 +1491,27 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
     if (dual) st = e->lanes[lane].stream;
     if (recompute) {
       e->eot_held[lane] = -1;
-      PROF(e, "expand_k1", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
-           dp::launch_expand(e->eot.img, nullptr, nullptr, nullptr, nullptr, rects, e->net_in, B, S, n0, n, H, H, e->Cp, e->bf16, false, e->num_sms, st));
+      if (xf) {
+        PROF(e, "expand_affine", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
+             dp::launch_expand_affine(e->eot.img, e->eot_xf_d, rects, e->net_in, S, n0, n, H, H, e->Cp, e->bf16, st));
+      } else {
+        PROF(e, "expand_k1", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
+             dp::launch_expand(e->eot.img, nullptr, nullptr, nullptr, nullptr, rects, e->net_in, B, S, n0, n, H, H, e->Cp, e->bf16, false, e->num_sms, st));
+      }
       KERNEL_OK(); ++e->launches;
       e->forward(n, e->net_in, true, st);
       e->eot_held[lane] = c;
     }
     // the caller's rows go to the lane's dlogits buffer: the head GEMM then reads what it reads in dp_attack_grad
     CUDA_OK(cudaMemcpyAsync(e->dlogits, dlogits + (size_t)n0 * K, (size_t)n * K * 4, cudaMemcpyDeviceToDevice, st));
-    const bool fuse = e->stem_bwd_fused_ok();
+    const bool fuse = !xf && e->stem_bwd_fused_ok();
     dp_engine::FusedReduce fr{rects, G, B, S, n0};
     e->backward(n, e->dlogits, st, fuse ? &fr : nullptr);
-    if (!fuse) {
+    if (xf) {
+      PROF(e, "reduce_affine", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
+           dp::launch_reduce_affine(e->d_input, e->eot.img, e->eot_xf_d, rects, G, S, n0, n, H, H, e->Cpd, e->bf16, st));
+      KERNEL_OK(); ++e->launches;
+    } else if (!fuse) {
       PROF(e, "reduce_k1t", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
            dp::launch_reduce(e->d_input, rects, G, B, S, n0, n, H, H, e->Cpd, e->bf16, st));
       KERNEL_OK(); ++e->launches;
@@ -1491,7 +1531,16 @@ int32_t dp_eot_forward(dp_engine* e, const float* img, int32_t B, int32_t S, con
   DP_TRY
   if (!e) fail("null engine");
   CUDA_OK(cudaSetDevice(e->cfg.device));
-  eot_forward_impl(e, img, B, S, rects_host, logits_dev, (cudaStream_t)stream);
+  eot_forward_impl(e, img, B, S, rects_host, nullptr, logits_dev, (cudaStream_t)stream);
+  DP_CATCH
+}
+
+int32_t dp_eot_forward_xform(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host,
+                             const float* xform_host, float* logits_dev, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  eot_forward_impl(e, img, B, S, rects_host, xform_host, logits_dev, (cudaStream_t)stream);
   DP_CATCH
 }
 

@@ -166,16 +166,25 @@ class Engine:
         return (preds, logits) if return_logits else preds
 
     # ------------------------------------------------------------------------------
-    def eot_forward(self, img, S=1, rects=None):
+    def eot_forward(self, img, S=1, rects=None, xforms=None):
         """model(occlude(img)) as [B*S, K] logits on the device (dp_predict's values), keeping what eot_backward needs.
-        img [B,3,H,W] fp32 in [0,1]; rects [B,S,4,4] int16 or None (then S must be 1)."""
+        img [B,3,H,W] fp32 in [0,1]; rects [B,S,4,4] int16 or None (then S must be 1 unless xforms are given).
+        xforms: [B,S,8] affine / colour transforms (eot.sample's layout) applied before the occlusion, or None."""
         B = img.shape[0]
         N = B * int(S)
         logits = torch.empty((N, self.n_classes), dtype=torch.float32, device=img.device)
         rp = None
         if rects is not None:
             rects, rp = _host(np.asarray(rects).reshape(N, 4, 4), np.int16)
-        _lib.check(self.lib.dp_eot_forward(self.handle, _dev_ptr(img), B, int(S), rp, _dev_ptr(logits), self._stream()))
+        if xforms is None:
+            _lib.check(self.lib.dp_eot_forward(self.handle, _dev_ptr(img), B, int(S), rp, _dev_ptr(logits),
+                                               self._stream()))
+        else:
+            if isinstance(xforms, torch.Tensor):
+                xforms = xforms.detach().cpu().numpy()
+            xf, xp = _host(np.asarray(xforms).reshape(N, 8), np.float32)
+            _lib.check(self.lib.dp_eot_forward_xform(self.handle, _dev_ptr(img), B, int(S), rp, xp, _dev_ptr(logits),
+                                                     self._stream()))
         self.eot_forwards += 1
         self._eot_shape = tuple(img.shape)
         return logits

@@ -9,12 +9,14 @@ adaptive attack on the PatchCleanser decision, ...), not only the CW loss that `
 The forward is ``dp_eot_forward`` (K1 + the classifier, the logits bit for bit those of ``dp_predict``); the
 backward is ``dp_eot_backward`` (classifier backward + K1^T on the current stream).  What is differentiated:
 
-- the image only.  The classifier's parameters get no ``.grad``: the engine has no weight-gradient pass.
+- the image only.  The classifier's parameters get no ``.grad``: the engine has no weight-gradient pass.  With
+  ``xforms`` (affine / colour EOT, ``dp_eot_forward_xform``) the transform parameters get none either.
 - once.  ``create_graph=True`` (double backward) raises.
 - the engine's last forward.  A backward after another forward on the same engine (``eot_logits`` again,
   ``dp_predict`` / PatchCleanser, ``generate``) raises instead of returning a gradient of the wrong activations.
   ``retain_graph=True`` and repeated backwards of the same forward are fine.
 """
+import numpy as np
 import torch
 
 from .utils import unwrap_native
@@ -22,8 +24,8 @@ from .utils import unwrap_native
 
 class _EotLogits(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, img, eng, S, rects):
-        logits = eng.eot_forward(img, S, rects)
+    def forward(ctx, img, eng, S, rects, xforms):
+        logits = eng.eot_forward(img, S, rects, xforms)
         ctx.eng, ctx.token = eng, eng.eot_forwards
         ctx.save_for_backward(img)                    # autograd then refuses a backward after an in-place change
         return logits
@@ -38,23 +40,47 @@ class _EotLogits(torch.autograd.Function):
         if eng.eot_forwards != ctx.token:
             raise RuntimeError("eot_logits: the engine ran another eot_forward after this one; its activations are "
                                "gone, so this graph can no longer be differentiated (run the forward again)")
-        return eng.eot_backward(dlogits.contiguous().float()), None, None, None
+        return eng.eot_backward(dlogits.contiguous().float()), None, None, None, None
 
 
-def eot_logits(model, img, rects=None, S=1):
+def _check_xforms(xforms, img, S):
+    """[B, S, 8] float32 host array of the transforms, or TypeError / ValueError."""
+    if isinstance(xforms, torch.Tensor):
+        if not xforms.dtype.is_floating_point:
+            raise TypeError("eot_logits: xforms must be a float tensor, got %s" % xforms.dtype)
+        xforms = xforms.detach().cpu().numpy()
+    xforms = np.asarray(xforms)
+    if xforms.dtype.kind != "f":
+        raise TypeError("eot_logits: xforms must be a float array, got %s" % xforms.dtype)
+    B = img.shape[0] if isinstance(img, torch.Tensor) and img.dim() >= 1 else None
+    if xforms.ndim != 3 or xforms.shape[1:] != (S, 8) or (B is not None and xforms.shape[0] != B):
+        raise ValueError("eot_logits: xforms must be [B, S, 8] with B = %s, S = %d, got %s" % (B, S, xforms.shape))
+    return np.ascontiguousarray(xforms, dtype=np.float32)
+
+
+def eot_logits(model, img, rects=None, S=1, xforms=None):
     """Differentiable ``model(occlude(img))``: [B*S, K] logits, sample b*S+s occluding image b with rects[b, s].
 
     model: ``ResNetV2``, ``NormModel(ResNetV2)`` or ``DataParallel`` of either (the native engine; anything else
     raises TypeError).  img: [B, 3, H, W] CUDA tensor in [0, 1]; NormModel's (x - 0.5) / 0.5 is fused into K1.
-    rects: [B, S, 4, 4] int16 rectangle tables (``masks.gather``), or None for plain classification (S = 1).
-    Differentiable with respect to ``img`` only (see the module docstring)."""
+    rects: [B, S, 4, 4] int16 rectangle tables (``masks.gather``), or None: plain classification (S = 1), or no
+    occlusion when xforms are given.
+    xforms: [B, S, 8] float tensor or array of affine / colour transforms, e.g. ``eot.sample(rng, B, S, affine,
+    colour)``: sample b*S+s is ``clamp(c * (grid_sample(img_b, affine_grid(theta)) - 0.5) + 0.5 + br, 0, 1)``
+    (bilinear, border padding, align_corners=False; theta = xforms[b, s, :6] as 2 x 3, c, br = xforms[b, s, 6:]),
+    then occluded -- what ``generate(eot_affine=..., eot_colour=...)`` optimises against.  None: no transform.
+    Differentiable with respect to ``img`` only: the transform parameters get no gradient (see the module docstring).
+    With xforms the input gradient is summed with fp32 atomics, so its last bits can differ from run to run."""
     net = unwrap_native(model)
+    if xforms is not None:
+        xforms = _check_xforms(xforms, img, int(S))
     if not (isinstance(img, torch.Tensor) and img.is_cuda):
         raise RuntimeError("eot_logits runs on the native CUDA engine only (no CPU fallback)")
     S = int(S)
-    if rects is None and S != 1:
-        raise ValueError("eot_logits: S=%d needs rectangle tables (rects=None is plain classification, S=1)" % S)
+    if rects is None and S != 1 and xforms is None:
+        raise ValueError("eot_logits: S=%d needs rectangle tables or xforms (rects=None without xforms is plain "
+                         "classification, S=1)" % S)
     if img.dim() != 4 or img.shape[1] != 3:
         raise ValueError("eot_logits: img must be [B, 3, H, W], got %s" % (tuple(img.shape),))
     eng = net.engine(img.shape[-1], max_images=img.shape[0])
-    return _EotLogits.apply(img.contiguous().float(), eng, S, rects)
+    return _EotLogits.apply(img.contiguous().float(), eng, S, rects, xforms)

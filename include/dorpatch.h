@@ -18,6 +18,7 @@
  *                       defenses/PatchCleanser.py:72,86,109; main.py:91,156)  [K1+K2]
  *   dp_eot_forward /    `logits = model(adv_x_masked); loss.backward()` with a
  *   dp_eot_backward     loss of the caller's choosing (attack.py:222-247)  [K1,K2 | K2^T,K1^T]
+ *   dp_eot_forward_xform  the same forward under affine / colour EOT (not in the reference)
  *   dp_attack_grad      attack.py:184-247: paste, EOT expansion, classifier
  *                       fwd + backward-to-input, CW loss (attack.py:16-23),
  *                       structural / density / group-lasso terms (:227-245),
@@ -140,6 +141,14 @@ int32_t dp_eot_forward(dp_engine* e, const float* img, int32_t B, int32_t S, con
  * dp_net_forward_backward, weights) ran since.  May be called more than once per forward; reads img again for the
  * chunks whose activations the engine no longer holds, so img must be unchanged.  No weight gradients. */
 int32_t dp_eot_backward(dp_engine* e, const float* dlogits_dev, float* grad_img_dev, void* stream);
+/* dp_eot_forward with the affine / colour EOT of dp_attack_args.xform_host before the occlusion:
+ * logits_dev[B*S, K] = model(occlude(colour(warp(img_b)), rects[b*S+s])).  xform_host [B*S][8] host, same layout as
+ * dp_attack_args.xform_host; NULL makes the call exactly dp_eot_forward.  With transforms, rects_host may be NULL at
+ * any S (the transforms make the samples differ).  Non-finite transform values are refused.  dp_eot_backward then
+ * differentiates this forward (the transforms get no gradient); its warp adjoint adds with fp32 atomics, so the last
+ * bits of the gradient may vary from run to run.  Added without changing any other entry point: the ABI stays 9. */
+int32_t dp_eot_forward_xform(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host,
+                             const float* xform_host, float* logits_dev, void* stream);
 
 /* ---- hot loop ------------------------------------------------------------------------ */
 typedef struct dp_attack_args {

@@ -1,8 +1,8 @@
 """Workload for compute-sanitizer (tools/sanitize.sh): every hand-written kernel family once, at sizes the tools finish in
 about a minute -- K1 (bulk-copy tiles + mbarriers), the cluster GroupNorm kernels (TMA slab, DSMEM reduce, split cluster
 barriers) through dp_debug_gn at cluster-1 / multi-CTA shapes, the bf16 stem kernels, one whole stage-0 and stage-1 attack
-step (paste, K1, net forward/backward, CW, fused stem-dgrad + reduce, regularisers, sign step), dp_predict, the failed-set
-bitmaps.  usage: python tools/sanitize_run.py [bf16|fp32|tf32] [img]"""
+step (paste, K1, net forward/backward, CW, fused stem-dgrad + reduce, regularisers, sign step), dp_predict, one
+dp_eot_forward_xform + dp_eot_backward (affine expansion and its atomic adjoint), the failed-set bitmaps.  usage: python tools/sanitize_run.py [bf16|fp32|tf32] [img]"""
 import ctypes as C
 import os
 import sys
@@ -44,6 +44,11 @@ def main():
         assert np.isfinite(r["loss_adv"]).all()
     if not light:
         eng.predict(x, S, rects)
+        # the differentiable classifier under affine / colour EOT: expand_affine, unfused stem dgrad, reduce_affine
+        # (two chunks, the first recomputed in the backward)
+        from dorpatch_b200 import eot as PE
+        logits = eng.eot_forward(x, S, rects, xforms=PE.sample(np.random.RandomState(1), B, S, 0.5, 0.5))
+        eng.eot_backward(torch.randn_like(logits))
     eng.expand(x, S, rects)
     eng.paste(x, m, p, 4.0)
     # the in-step K1 variant (paste fused in), both store paths
