@@ -62,6 +62,11 @@ SIGNATURES = {
     "dp_eot_forward": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "dp_eot_backward": (c_i32, [c_vp, c_vp, c_vp, c_vp]),
     "dp_eot_forward_xform": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    "dp_eot_backward_params": (c_i32, [c_vp, c_vp, c_vp, c_i32, C.POINTER(C.c_char_p), C.POINTER(c_vp), c_i32, c_vp]),
+    "dp_engine_load_weights_dev": (c_i32, [c_vp, c_i32, C.POINTER(C.c_char_p), C.POINTER(c_vp), C.POINTER(c_i64), c_vp]),
+    "dp_debug_stem_wgrad": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_vp]),
+    "dp_debug_gn_wgrad": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
+    "dp_debug_ws_backward": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp]),
     "dp_attack_grad": (c_i32, [c_vp, C.POINTER(DpAttackArgs), c_vp]),
     "dp_attack_update": (c_i32, [c_vp, C.POINTER(DpUpdateArgs), c_vp]),
     "dp_attack_step_host": (c_i32, [c_vp, C.POINTER(DpAttackArgs), C.POINTER(DpUpdateArgs), c_vp]),

@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libdorpatch.so")
-SOURCES = ["kernels_net.cu", "kernels_patch.cu", "kernels_stem.cu", "kernels_gemm.cu", "engine.cu"]
+SOURCES = ["kernels_net.cu", "kernels_patch.cu", "kernels_stem.cu", "kernels_gemm.cu", "kernels_wgrad.cu", "engine.cu"]
 HEADERS = ["common.cuh", "kernels.h", os.path.join("..", "..", "include", "dorpatch.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 

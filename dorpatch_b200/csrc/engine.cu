@@ -5,8 +5,8 @@
 // The classifier's 3x3 / 7x7 convolutions run on tensor cores through cuDNN, the 1x1
 // convolutions (36 of 53) are plain NHWC GEMMs through cublasLt (the residual add is fused
 // as the GEMM's C operand); everything else is the hand-written kernels of kernels_*.cu.
-// Backward is data-gradient only (the weights are frozen during the attack; the reference's
-// unused weight-gradient, SURVEY quirk Q7, is not computed).
+// The attack's backward is data-gradient only (the weights are frozen; the reference's unused weight gradient, SURVEY
+// quirk Q7, is not computed there).  dp_eot_backward_params adds an opt-in weight-gradient pass (fine-tuning).
 #include <cublasLt.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -78,10 +78,13 @@ struct NvtxRange {
 struct ConvW {            // one convolution's weights (device, KRSC, activation dtype)
   int cin = 0, cin_pad = 0, cout = 0, k = 1, stride = 1, pad = 0;
   void* w = nullptr;
+  float* raw = nullptr;     // the fp32 OIHW weights as loaded (the weight-standardisation adjoint reads them)
+  int pid = -1;             // index into dp_engine::wparams
   cudnnFilterDescriptor_t wdesc = nullptr;
   cudnnConvolutionDescriptor_t cdesc = nullptr;
 };
-struct GNW { int C = 0; float* gamma = nullptr; float* beta = nullptr; bool pos = false; };   // pos: every gamma > 0 (packed bf16 ReLU gate allowed)
+// pos: every gamma > 0 (packed bf16 ReLU gate allowed).  pid: gamma's wparams index (beta's is pid + 1).
+struct GNW { int C = 0; float* gamma = nullptr; float* beta = nullptr; bool pos = false; int pid = -1; };
 struct Block {
   int cin, mid, cout, stride, hin, hout;
   bool has_ds;
@@ -97,6 +100,7 @@ struct CudnnPlan {
   cudnnTensorDescriptor_t xdesc = nullptr, ydesc = nullptr;
   cudnnConvolutionFwdAlgo_t fwd_algo; cudnnMathType_t fwd_math; size_t fwd_ws = 0; bool fwd_ready = false;
   cudnnConvolutionBwdDataAlgo_t bwd_algo; cudnnMathType_t bwd_math; size_t bwd_ws = 0; bool bwd_ready = false;
+  cudnnConvolutionBwdFilterAlgo_t wgd_algo; cudnnMathType_t wgd_math; size_t wgd_ws = 0; bool wgd_ready = false;
 };
 struct GemmPlan {
   cublasLtMatmulDesc_t op = nullptr;
@@ -166,6 +170,7 @@ struct dp_engine {
   std::vector<LaneBufs> lanes;
   cudaEvent_t ev_prep = nullptr;
   void use_lane(int l) {
+    cur_lane = l;
     LaneBufs& L = lanes[l];
     net_in = L.net_in; act = L.act; act2 = L.act2; x0 = L.x0; pool_amax = L.pool_amax;
     for (int i = 0; i < 4; ++i) g[i] = L.g[i];
@@ -204,7 +209,8 @@ struct dp_engine {
   // weights); a backward whose forward recorded an older generation is refused.  eot_held[l] is the chunk whose saved
   // activations (pre-norm outputs, GroupNorm statistics, max-pool argmax) lane l still holds, -1 none.
   // xf: the forward warped its samples (dp_eot_forward_xform) with the transforms in eot_xf_d.
-  struct EotSig { int64_t gen = -1; const float* img = nullptr; int B = 0, S = 0; bool rects = false, xf = false; };
+  // whole: the forward's K1 wrote every sample to net_in_all (a held chunk's input is its slice there).
+  struct EotSig { int64_t gen = -1; const float* img = nullptr; int B = 0, S = 0; bool rects = false, xf = false, whole = false; };
   int64_t fwd_gen = 0;
   EotSig eot;
   int eot_held[2] = {-1, -1};
@@ -349,6 +355,7 @@ struct dp_engine {
   void make_conv(ConvW& c, int cin, int cout, int k, int stride, int pad, int cin_pad) {
     c.cin = cin; c.cin_pad = cin_pad; c.cout = cout; c.k = k; c.stride = stride; c.pad = pad;
     c.w = dmalloc((size_t)cout * k * k * cin_pad * es);
+    c.raw = (float*)dmalloc((size_t)cout * k * k * cin * 4);
     if (k > 1) {   // cuDNN path
       CUDNN_OK(cudnnCreateFilterDescriptor(&c.wdesc));
       CUDNN_OK(cudnnSetFilter4dDescriptor(c.wdesc, cudnn_dt, CUDNN_TENSOR_NHWC, cout, cin_pad, k, k));
@@ -441,14 +448,103 @@ struct dp_engine {
     grp_ss = (float*)dmalloc(B * HW * 4);
     ensure_samples(chunk);
     ensure_pin((size_t)4 << 20);
+    build_wparams();
   }
 
+  // ---- named parameters and the weight-gradient accumulators (dp_eot_backward_params) -------------------------
+  // One entry per timm state-dict tensor.  Each has a slot in the fp32 accumulators: conv weights as d/d(standardised
+  // weight) in the engine's KRSC, channel-padded layout (the standardisation adjoint runs once per call at the end),
+  // GroupNorm gamma | beta adjacent, the fc weight [K][2048] and bias.  The head's four tensors come last.
+  enum WKind { W_CONV = 0, W_GAMMA, W_BETA, W_FCW, W_FCB };
+  struct WParam { std::string name; int kind; ConvW* conv; GNW* gn; int64_t numel; size_t off; };
+  std::vector<WParam> wparams;
+  std::map<std::string, int> wparam_idx;
+  size_t wacc_floats = 0, wacc_trunk_end = 0;    // [0, wacc_trunk_end): stem + blocks; the rest: head
+  float* wacc[2] = {nullptr, nullptr};           // per lane
+  float* wg_partial[2] = {nullptr, nullptr};     // per lane: GroupNorm / stem partial sums
+  void* wg_half[2] = {nullptr, nullptr};         // per lane: bf16 cuDNN filter gradient before it is added in fp32
+  std::vector<char> want;                        // per wparam: requested by the current call
+  // acc_floats: the slot's size (0: the entry lives inside the slot just reserved, at `inner` floats from its start)
+  void add_wparam(const std::string& name, int kind, ConvW* c, GNW* g, int64_t numel, size_t acc_floats, size_t inner = 0) {
+    wparam_idx[name] = (int)wparams.size();
+    if (c) c->pid = (int)wparams.size();
+    if (g && kind == W_GAMMA) g->pid = (int)wparams.size();
+    if (acc_floats == 0) {
+      wparams.push_back(WParam{name, kind, c, g, numel, wparams.back().off + inner});
+      return;
+    }
+    wparams.push_back(WParam{name, kind, c, g, numel, wacc_floats});
+    wacc_floats += (acc_floats + 63) / 64 * 64;
+  }
+  void add_conv_param(const std::string& name, ConvW& c) {
+    add_wparam(name, W_CONV, &c, nullptr, (int64_t)c.cout * c.cin * c.k * c.k, (size_t)c.cout * c.k * c.k * c.cin_pad);
+  }
+  void add_gn_params(const std::string& pre, GNW& g) {   // one slot [gamma | beta]: gn_wgrad adds both halves at once
+    add_wparam(pre + ".weight", W_GAMMA, nullptr, &g, g.C, 2 * (size_t)g.C);
+    add_wparam(pre + ".bias", W_BETA, nullptr, &g, g.C, 0, g.C);
+  }
+  void build_wparams() {
+    add_conv_param("stem.conv.weight", stem);
+    int s = 0, bi = 0;
+    for (auto& b : blocks) {
+      char pre[64];
+      snprintf(pre, sizeof(pre), "stages.%d.blocks.%d.", s, bi);
+      const std::string P(pre);
+      if (b.has_ds) add_conv_param(P + "downsample.conv.weight", b.ds);
+      add_conv_param(P + "conv1.weight", b.c1);
+      add_conv_param(P + "conv2.weight", b.c2);
+      add_conv_param(P + "conv3.weight", b.c3);
+      add_gn_params(P + "norm1", b.n1);
+      add_gn_params(P + "norm2", b.n2);
+      add_gn_params(P + "norm3", b.n3);
+      if (++bi == DEPTHS[s]) { bi = 0; ++s; }
+    }
+    wacc_trunk_end = wacc_floats;
+    add_gn_params("norm", head_gn);
+    add_wparam("head.fc.weight", W_FCW, nullptr, nullptr, (int64_t)K * WIDTHS[3], (size_t)K * WIDTHS[3]);
+    add_wparam("head.fc.bias", W_FCB, nullptr, nullptr, K, K);
+    want.assign(wparams.size(), 0);
+  }
+  const WParam& wparam(const char* name) const {
+    auto it = wparam_idx.find(name);
+    if (it == wparam_idx.end()) fail("unknown parameter name '%s' (timm resnetv2_50x1_bit state-dict names)", name);
+    return wparams[it->second];
+  }
+  void ensure_wgrad_buffers() {
+    if (wacc[0]) return;
+    size_t part = std::max((size_t)chunk * 2 * WIDTHS[3], dp::stem_wgrad_partial_floats());
+    part = std::max(part, (size_t)chunk * 2 * 2048);
+    size_t half = 0;
+    for (auto& b : blocks) half = std::max(half, (size_t)b.c2.cout * 9 * b.c2.cin_pad);
+    half = std::max(half, (size_t)STEM_CH * 49 * stem.cin_pad);
+    for (size_t l = 0; l < lanes.size(); ++l) {
+      wacc[l] = (float*)dmalloc(wacc_floats * 4);
+      wg_partial[l] = (float*)dmalloc(part * 4);
+      wg_half[l] = dmalloc(half * 2);
+    }
+  }
+  bool want_conv(const ConvW& c) const { return c.pid >= 0 && want[c.pid]; }
+  bool want_gn(const GNW& g) const { return g.pid >= 0 && (want[g.pid] || want[g.pid + 1]); }
+  // accumulator span of wparam i: [off, end); a GroupNorm's gamma and beta share one slot, zeroed and filled together
+  std::pair<size_t, size_t> wspan(size_t i) const {
+    const WParam& w = wparams[i];
+    if (w.kind == W_GAMMA || w.kind == W_BETA) {
+      const size_t g0 = wparams[w.gn->pid].off;
+      return {g0, g0 + 2 * (size_t)w.gn->C};
+    }
+    size_t end = wacc_floats;
+    for (size_t j = i + 1; j < wparams.size(); ++j) if (wparams[j].off > w.off) { end = wparams[j].off; break; }
+    return {w.off, end};
+  }
+  float* acc_of(int pid) const { return wacc[cur_lane] + wparams[pid].off; }
+  int cur_lane = 0;
+
   // ---- weights -------------------------------------------------------------------------
-  void upload_conv(ConvW& c, const float* host, int64_t numel, cudaStream_t st, float* tmp) {
+  void upload_conv(ConvW& c, const float* host, int64_t numel, cudaStream_t st) {
     const int64_t want = (int64_t)c.cout * c.cin * c.k * c.k;
     if (numel != want) fail("conv weight numel %lld != expected %lld", (long long)numel, (long long)want);
-    CUDA_OK(cudaMemcpyAsync(tmp, host, (size_t)numel * 4, cudaMemcpyHostToDevice, st));
-    dp::launch_weight_standardize(tmp, c.w, c.cout, c.cin, c.k, c.k, c.cin_pad, bf16, true, st);
+    CUDA_OK(cudaMemcpyAsync(c.raw, host, (size_t)numel * 4, cudaMemcpyHostToDevice, st));
+    dp::launch_weight_standardize(c.raw, c.w, c.cout, c.cin, c.k, c.k, c.cin_pad, bf16, true, st);
     KERNEL_OK();
     CUDA_OK(cudaStreamSynchronize(st));
   }
@@ -469,22 +565,20 @@ struct dp_engine {
       if (it == idx.end()) fail("missing weight tensor '%s'", k.c_str());
       return it->second;
     };
-    float* tmp = nullptr;
-    CUDA_OK(cudaMalloc((void**)&tmp, (size_t)2048 * 2048 * 9 * 4 / 4 + (size_t)K * 2048 * 4));
     cudaStream_t st = 0;
-    try {
+    {
       int i = get("stem.conv.weight");
-      upload_conv(stem, ptrs[i], numels[i], st, tmp);
+      upload_conv(stem, ptrs[i], numels[i], st);
       if (own_stem) { dp::launch_stem_pack(stem.w, stem_w_kn, stem.cin_pad, st); KERNEL_OK(); CUDA_OK(cudaStreamSynchronize(st)); }
       int s = 0, bi = 0;
       for (auto& b : blocks) {
         char pre[64];
         snprintf(pre, sizeof(pre), "stages.%d.blocks.%d.", s, bi);
         auto P = [&](const char* suffix) { return std::string(pre) + suffix; };
-        if (b.has_ds) { i = get(P("downsample.conv.weight")); upload_conv(b.ds, ptrs[i], numels[i], st, tmp); }
-        i = get(P("conv1.weight")); upload_conv(b.c1, ptrs[i], numels[i], st, tmp);
-        i = get(P("conv2.weight")); upload_conv(b.c2, ptrs[i], numels[i], st, tmp);
-        i = get(P("conv3.weight")); upload_conv(b.c3, ptrs[i], numels[i], st, tmp);
+        if (b.has_ds) { i = get(P("downsample.conv.weight")); upload_conv(b.ds, ptrs[i], numels[i], st); }
+        i = get(P("conv1.weight")); upload_conv(b.c1, ptrs[i], numels[i], st);
+        i = get(P("conv2.weight")); upload_conv(b.c2, ptrs[i], numels[i], st);
+        i = get(P("conv3.weight")); upload_conv(b.c3, ptrs[i], numels[i], st);
         if (fused_gemm) {
           dp::launch_gn_gemm_pack(b.c1.w, b.c1p, b.mid, b.cin, st); KERNEL_OK();
           dp::launch_gn_gemm_pack(b.c3.w, b.c3p, b.cout, b.mid, st); KERNEL_OK();
@@ -502,13 +596,56 @@ struct dp_engine {
       i = get("norm.bias"); upload_vec(head_gn.beta, ptrs[i], numels[i], WIDTHS[3]);
       i = get("head.fc.weight"); upload_vec(fc_w, ptrs[i], numels[i], (int64_t)K * WIDTHS[3]);
       i = get("head.fc.bias"); upload_vec(fc_b, ptrs[i], numels[i], K);
-    } catch (...) {
-      cudaFree(tmp);
-      throw;
     }
-    cudaFree(tmp);
     weights_loaded = true;
     forward_clobbered();
+  }
+
+  // Reload named tensors from fp32 device buffers (after an optimizer step): no host copy of the weights; the convs are
+  // re-standardised on the stream and re-packed for the own stem / fused GEMM; each reloaded GroupNorm's gamma > 0
+  // flag (the packed bf16 ReLU gate) is recomputed from the new values.
+  void load_weights_dev(int n, const char* const* names, const float* const* ptrs, const int64_t* numels, cudaStream_t st) {
+    if (!weights_loaded) fail("dp_engine_load_weights_dev: load the full set with dp_engine_load_weights first");
+    if (n < 0 || (n > 0 && (!names || !ptrs || !numels))) fail("dp_engine_load_weights_dev: null argument");
+    for (int i = 0; i < n; ++i) {                        // check everything before anything changes
+      if (!names[i]) fail("dp_engine_load_weights_dev: null name at position %d", i);
+      const WParam& w = wparam(names[i]);
+      if (!ptrs[i]) fail("dp_engine_load_weights_dev: null pointer for '%s'", names[i]);
+      if (numels[i] != w.numel) fail("dp_engine_load_weights_dev: '%s' has %lld elements, expected %lld", names[i], (long long)numels[i], (long long)w.numel);
+    }
+    drop_graphs();
+    forward_clobbered();
+    std::vector<GNW*> gammas;
+    for (int i = 0; i < n; ++i) {
+      const WParam& w = wparam(names[i]);
+      const size_t bytes = (size_t)w.numel * 4;
+      switch (w.kind) {
+        case W_CONV: {
+          ConvW& c = *w.conv;
+          CUDA_OK(cudaMemcpyAsync(c.raw, ptrs[i], bytes, cudaMemcpyDeviceToDevice, st));
+          dp::launch_weight_standardize(c.raw, c.w, c.cout, c.cin, c.k, c.k, c.cin_pad, bf16, true, st); KERNEL_OK();
+          if (&c == &stem && own_stem) { dp::launch_stem_pack(stem.w, stem_w_kn, stem.cin_pad, st); KERNEL_OK(); }
+          if (fused_gemm)
+            for (auto& b : blocks) {
+              if (&c == &b.c1) { dp::launch_gn_gemm_pack(b.c1.w, b.c1p, b.mid, b.cin, st); KERNEL_OK(); }
+              if (&c == &b.c3) { dp::launch_gn_gemm_pack(b.c3.w, b.c3p, b.cout, b.mid, st); KERNEL_OK(); }
+            }
+          break;
+        }
+        case W_GAMMA: CUDA_OK(cudaMemcpyAsync(w.gn->gamma, ptrs[i], bytes, cudaMemcpyDeviceToDevice, st)); gammas.push_back(w.gn); break;
+        case W_BETA: CUDA_OK(cudaMemcpyAsync(w.gn->beta, ptrs[i], bytes, cudaMemcpyDeviceToDevice, st)); break;
+        case W_FCW: CUDA_OK(cudaMemcpyAsync(fc_w, ptrs[i], bytes, cudaMemcpyDeviceToDevice, st)); break;
+        default: CUDA_OK(cudaMemcpyAsync(fc_b, ptrs[i], bytes, cudaMemcpyDeviceToDevice, st)); break;
+      }
+    }
+    CUDA_OK(cudaStreamSynchronize(st));
+    std::vector<float> h;
+    for (GNW* g_ : gammas) {
+      h.resize(g_->C);
+      CUDA_OK(cudaMemcpy(h.data(), g_->gamma, (size_t)g_->C * 4, cudaMemcpyDeviceToHost));
+      g_->pos = true;
+      for (float v : h) g_->pos = g_->pos && (v > 0.f);
+    }
   }
 
   // ---- cuDNN convolution -------------------------------------------------------------
@@ -661,6 +798,81 @@ struct dp_engine {
     ++launches;
   }
 
+  // ---- weight gradients ----------------------------------------------------------------------
+  // 3x3 / stem: acc (KRSC, fp32) += dW through cuDNN, deterministic algorithms only, the engine's precision rules.
+  // cuDNN's filter gradient has the filter's data type: at bf16 it goes through the lane's bf16 scratch.
+  void conv_wgrad(int layer_id, const ConvW& c, int N, int hin, int hout, const void* x, const void* dy, float* acc, cudaStream_t st) {
+    CudnnPlan& p = conv_plan(layer_id, c, N, hin, hout);
+    if (!p.wgd_ready) {
+      cudnnConvolutionBwdFilterAlgoPerf_t perf[16];
+      int got = 0;
+      CUDNN_OK(cudnnGetConvolutionBackwardFilterAlgorithm_v7(cudnn, p.xdesc, p.ydesc, c.cdesc, c.wdesc, 16, &got, perf));
+      for (int i = 0; i < got && !p.wgd_ready; ++i) {
+        if (perf[i].status != CUDNN_STATUS_SUCCESS || perf[i].memory > lib_ws_bytes || !math_ok(perf[i].mathType) ||
+            perf[i].determinism != CUDNN_DETERMINISTIC) continue;
+        p.wgd_algo = perf[i].algo; p.wgd_math = perf[i].mathType; p.wgd_ws = perf[i].memory; p.wgd_ready = true;
+      }
+      if (!p.wgd_ready) fail("no usable deterministic cuDNN backward-filter algorithm (cin=%d cout=%d k=%d stride=%d, %d candidates)",
+                             c.cin_pad, c.cout, c.k, c.stride, got);
+    }
+    CUDNN_OK(cudnnSetConvolutionMathType(c.cdesc, p.wgd_math));
+    const float one = 1.f, zero = 0.f;
+    const size_t wn = (size_t)c.cout * c.k * c.k * c.cin_pad;
+    const double fl = 2.0 * N * hout * hout * c.cout * c.k * c.k * c.cin;
+    const double by = ((double)N * hin * hin * c.cin_pad + (double)N * hout * hout * c.cout) * es + (double)wn * 8;
+    PROF(this, c.k == 7 ? "stem_wgrad" : "conv3x3_wgrad", by, fl, st,
+         CUDNN_OK(cudnnConvolutionBackwardFilter(cudnn, &one, p.xdesc, x, p.ydesc, dy, c.cdesc, p.wgd_algo, lib_ws, lib_ws_bytes,
+                                                 bf16 ? &zero : &one, c.wdesc, bf16 ? wg_half[cur_lane] : (void*)acc)));
+    ++launches;
+    if (bf16) { dp::launch_add_bf16(wg_half[cur_lane], acc, wn, st); KERNEL_OK(); ++launches; }
+  }
+  // 1x1 convolutions and the fc layer: D[cout][cin] (fp32) += dY^T X over `rows` pixels.  Column-major view:
+  // D [cin x cout] = X [cin x rows] * (dY [cout x rows])^T.  head: fp32 operands and math (the fc layer is fp32).
+  std::map<std::tuple<int, int, int, int>, GemmPlan> wgrad_plans;
+  void wgrad_gemm(int rows, int cout, int cin, const void* X, const void* dY, float* D, bool head, cudaStream_t st) {
+    auto key = std::make_tuple(rows, cout, cin, head ? 1 : 0);
+    auto it = wgrad_plans.find(key);
+    if (it == wgrad_plans.end()) {
+      GemmPlan p;
+      const cudaDataType_t ab = head ? CUDA_R_32F : cuda_dt;
+      CUBLAS_OK(cublasLtMatmulDescCreate(&p.op, head ? CUBLAS_COMPUTE_32F : lt_compute, CUDA_R_32F));
+      const cublasOperation_t ta = CUBLAS_OP_N, tb = CUBLAS_OP_T;
+      CUBLAS_OK(cublasLtMatmulDescSetAttribute(p.op, CUBLASLT_MATMUL_DESC_TRANSA, &ta, sizeof(ta)));
+      CUBLAS_OK(cublasLtMatmulDescSetAttribute(p.op, CUBLASLT_MATMUL_DESC_TRANSB, &tb, sizeof(tb)));
+      CUBLAS_OK(cublasLtMatrixLayoutCreate(&p.a, ab, cin, rows, cin));
+      CUBLAS_OK(cublasLtMatrixLayoutCreate(&p.b, ab, cout, rows, cout));
+      CUBLAS_OK(cublasLtMatrixLayoutCreate(&p.c, CUDA_R_32F, cin, cout, cin));
+      cublasLtMatmulPreference_t pref;
+      CUBLAS_OK(cublasLtMatmulPreferenceCreate(&pref));
+      CUBLAS_OK(cublasLtMatmulPreferenceSetAttribute(pref, CUBLASLT_MATMUL_PREF_MAX_WORKSPACE_BYTES, &lib_ws_bytes, sizeof(lib_ws_bytes)));
+      cublasLtMatmulHeuristicResult_t res[1];
+      int got = 0;
+      cublasStatus_t s = cublasLtMatmulAlgoGetHeuristic(lt, p.op, p.a, p.b, p.c, p.c, pref, 1, res, &got);
+      cublasLtMatmulPreferenceDestroy(pref);
+      if (s != CUBLAS_STATUS_SUCCESS || got == 0) fail("cublasLt: no algorithm for the weight-gradient GEMM rows=%d cout=%d cin=%d (status %d)", rows, cout, cin, (int)s);
+      p.algo = res[0].algo;
+      it = wgrad_plans.emplace(key, p).first;
+    }
+    GemmPlan& p = it->second;
+    const float one = 1.f;
+    const double by = ((double)rows * (cin + cout)) * (head ? 4 : es) + (double)cin * cout * 8;
+    PROF(this, head ? "fc_wgrad" : "gemm1x1_wgrad", by, 2.0 * rows * cout * cin, st,
+         CUBLAS_OK(cublasLtMatmul(lt, p.op, &one, X, p.a, dY, p.b, &one, D, p.c, D, p.c, &p.algo, lib_ws, lib_ws_bytes, st)));
+    ++launches;
+  }
+  // GroupNorm affine gradients of one norm: dy at its (ReLU) output, x its input, stats the forward's
+  void gn_wgrad(const GNW& g, const void* dy, const void* x, const float* stats, int N, int P, cudaStream_t st) {
+    float* part = wg_partial[cur_lane];
+    PROF(this, "gn_affine_wgrad", 2.0 * N * P * g.C * es + (double)N * 2 * g.C * 8, 0, st, {
+      dp::launch_gn_affine_partial(dy, x, g.gamma, g.beta, stats, part, N, P, g.C, bf16, st);
+      dp::launch_colsum_add(part, acc_of(g.pid), N, 2 * g.C, st);
+    }); KERNEL_OK(); launches += 2;
+  }
+  void gn_apply(const GNW& g, const void* x, const float* stats, void* y, int N, int P, cudaStream_t st) {
+    PROF(this, "gn_apply_wgrad", 2.0 * N * P * g.C * es, 0, st, dp::launch_gn_apply(x, y, g.gamma, g.beta, stats, N, P, g.C, bf16, st));
+    KERNEL_OK(); ++launches;
+  }
+
   // ---- classifier forward ------------------------------------------------------------------
   // input: [N,H,H,Cp] T.  train: keep what backward needs.  Leaves logits in `logits`.
   void forward(int N, const void* input, bool train, cudaStream_t st) {
@@ -748,29 +960,67 @@ struct dp_engine {
   bool fused_stem_bwd = false;     // set at create: own_stem && DORPATCH_STEM_BWD != "cudnn"
   bool fused_pool_bwd = false;     // ... && DORPATCH_POOL_BWD == "fused": max-pool backward fused in as well (slower, off)
   bool stem_bwd_fused_ok() const { return fused_stem_bwd; }
-  void backward(int N, const float* dlog, cudaStream_t st, const FusedReduce* fused = nullptr) {
+  // Weight-gradient pass of one chunk (dp_eot_backward_params): accumulates d/d(parameter) of the requested
+  // parameters (`want`) into the current lane's accumulators.  input: the chunk's network input.  need_dx: the
+  // input gradient is wanted too (else the backward stops at block `lo`, the lowest block whose gradients are wanted).
+  struct Wgrad { const void* input; bool need_dx; int lo; };
+  void backward(int N, const float* dlog, cudaStream_t st, const FusedReduce* fused = nullptr, const Wgrad* wg = nullptr) {
     NvtxRange nvtx_("dorpatch.classifier_backward");
     CUDNN_OK(cudnnSetStream(cudnn, st));
     const Block& last = blocks.back();
     const int pl = last.hout * last.hout;
     void *GA = g[0], *GB = g[1], *GC = g[2], *GD = g[3];
+    const bool W = wg != nullptr;
+    if (W) {                                                                     // fc: dW += dlogits^T pooled, db += sum dlogits
+      const WParam& fw = wparams[wparam_idx.at("head.fc.weight")];
+      const WParam& fb = wparams[wparam_idx.at("head.fc.bias")];
+      if (want[wparam_idx.at("head.fc.weight")]) wgrad_gemm(N, K, last.cout, pooled, dlog, wacc[cur_lane] + fw.off, true, st);
+      if (want[wparam_idx.at("head.fc.bias")]) {
+        PROF(this, "fc_wgrad", (double)N * K * 4, 0, st, dp::launch_colsum_add(dlog, wacc[cur_lane] + fb.off, N, K, st));
+        KERNEL_OK(); ++launches;
+      }
+      if (!wg->need_dx && wg->lo >= (int)blocks.size() && !want_gn(head_gn)) return;
+    }
     gemm(N, last.cout, K, 3, fc_w, dlog, nullptr, 0.f, dpooled, st);           // dpooled = dlogits * Wfc (fp32)
     PROF(this, "head_bwd", 2.0 * N * pl * last.cout * es, 0, st, {
       dp::launch_pool_grad_bcast(dpooled, GB, N, pl, last.cout, bf16, st);
       dp::launch_gn_relu_backward(GB, last.out, nullptr, GA, head_gn.gamma, head_gn.beta, head_stats, gn_partial, N, pl, last.cout, bf16, st, head_gn.pos);
     }); KERNEL_OK(); launches += 3;
-    for (int bi = (int)blocks.size() - 1; bi >= 0; --bi) {
+    if (W && want_gn(head_gn)) gn_wgrad(head_gn, GB, last.out, head_stats, N, pl, st);
+    const int lo = W && !wg->need_dx ? wg->lo : 0;
+    for (int bi = (int)blocks.size() - 1; bi >= lo; --bi) {
       Block& b = blocks[bi];
       const int lid = bi + 1;
       const int pin_ = b.hin * b.hin, pout = b.hout * b.hout;
       const void* xin = (bi == 0) ? x0 : blocks[bi - 1].out;
+      // conv3: dY = d_out (GA), X = relu(gn3(h2)) recomputed into act
+      if (W && want_conv(b.c3)) {
+        gn_apply(b.n3, b.h2, b.st3, act, N, pout, st);
+        wgrad_gemm(N * pout, b.cout, b.mid, act, GA, acc_of(b.c3.pid), false, st);
+      }
       // d_a3 = d_out * W3
       gemm(N * pout, b.mid, b.cout, 1, b.c3.w, GA, nullptr, 0.f, GB, st);
       PROF(this, "gn_relu_bwd", 3.0 * N * pout * b.mid * es, 0, st,
            dp::launch_gn_relu_backward(GB, b.h2, nullptr, GC, b.n3.gamma, b.n3.beta, b.st3, gn_partial, N, pout, b.mid, bf16, st, b.n3.pos)); KERNEL_OK(); launches += 2;
+      if (W && want_gn(b.n3)) gn_wgrad(b.n3, GB, b.h2, b.st3, N, pout, st);
+      if (W && want_conv(b.c2)) {                                                // conv2: dY = GC, X = relu(gn2(h1))
+        gn_apply(b.n2, b.h1, b.st2, act, N, pin_, st);
+        conv_wgrad(lid, b.c2, N, b.hin, b.hout, act, GC, acc_of(b.c2.pid), st);
+      }
       conv_bwd(lid, b.c2, N, b.hin, b.hout, GC, GB, st);
       PROF(this, "gn_relu_bwd", 3.0 * N * pin_ * b.mid * es, 0, st,
            dp::launch_gn_relu_backward(GB, b.h1, nullptr, GC, b.n2.gamma, b.n2.beta, b.st2, gn_partial, N, pin_, b.mid, bf16, st, b.n2.pos)); KERNEL_OK(); launches += 2;
+      if (W && want_gn(b.n2)) gn_wgrad(b.n2, GB, b.h1, b.st2, N, pin_, st);
+      if (W && (want_conv(b.c1) || (b.has_ds && want_conv(b.ds)))) gn_apply(b.n1, xin, b.st1, act, N, pin_, st);   // relu(gn1(xin))
+      if (W && want_conv(b.c1)) wgrad_gemm(N * pin_, b.mid, b.cin, act, GC, acc_of(b.c1.pid), false, st);   // conv1: dY = GC
+      if (W && b.has_ds && want_conv(b.ds)) {                                    // downsample: dY = GA, X = (subsampled) act
+        const void* src = act;
+        if (b.stride == 2) {
+          PROF(this, "subsample", 2.0 * N * pout * b.cin * es, 0, st, dp::launch_subsample2(act, act2, N, b.hin, b.hin, b.cin, bf16, st));
+          KERNEL_OK(); ++launches; src = act2;
+        }
+        wgrad_gemm(N * pout, b.cout, b.cin, src, GA, acc_of(b.ds.pid), false, st);
+      }
       gemm(N * pin_, b.cin, b.mid, 1, b.c1.w, GC, nullptr, 0.f, GB, st);          // d_xp (conv1 path)
       if (b.has_ds) {
         if (b.stride == 2) {
@@ -785,10 +1035,13 @@ struct dp_engine {
         PROF(this, "gn_relu_bwd", 4.0 * N * pin_ * b.cin * es, 0, st,
              dp::launch_gn_relu_backward(GB, xin, GA, GD, b.n1.gamma, b.n1.beta, b.st1, gn_partial, N, pin_, b.cin, bf16, st, b.n1.pos)); KERNEL_OK(); launches += 2;
       }
+      if (W && want_gn(b.n1)) gn_wgrad(b.n1, GB, xin, b.st1, N, pin_, st);
       std::swap(GA, GD);
     }
     const int hs = Hs();
-    if (fused != nullptr && fused_pool_bwd) {
+    if (W && lo > 0) return;                                                     // nothing below block lo is wanted
+    if (W && !wg->need_dx && !want_conv(stem)) return;
+    if (fused != nullptr && fused_pool_bwd && !W) {
       // max-pool backward + stem dgrad + masked EOT reduce in one kernel: neither d_stem nor d_input is written
       PROF(this, "stem_bwd_reduce", (double)N * (hs / 2) * (hs / 2) * STEM_CH * (es + 1) + 3.0 * H * H * 4 * (double)N / fused->S,
            2.0 * N * hs * hs * STEM_CH * 147, st,
@@ -799,6 +1052,20 @@ struct dp_engine {
     }
     PROF(this, "maxpool_bwd", (double)N * (hs * hs + (hs / 2) * (hs / 2)) * STEM_CH * es, 0, st,
          dp::launch_maxpool_backward(GA, pool_amax, GB, N, hs, hs, STEM_CH, bf16, st)); KERNEL_OK(); ++launches;
+    if (W && want_conv(stem)) {                                                  // stem: dY = the max-pool adjoint (GB)
+      if (own_stem) {
+        PROF(this, "stem_wgrad", (double)N * (H * H * 3 + hs * hs * STEM_CH) * es, 2.0 * N * hs * hs * STEM_CH * 147, st,
+             dp::launch_stem_wgrad(wg->input, GB, wg_partial[cur_lane], acc_of(stem.pid), N, H, H, stem.cin_pad, st));
+        KERNEL_OK(); launches += 2;
+      } else {
+        for (int n0 = 0; n0 < N; n0 += STEM_SUB) {
+          const int n = std::min(STEM_SUB, N - n0);
+          conv_wgrad(0, stem, n, H, hs, (const char*)wg->input + (size_t)n0 * H * H * Cp * es, (const char*)GB + (size_t)n0 * hs * hs * STEM_CH * es,
+                     acc_of(stem.pid), st);
+        }
+      }
+      if (!wg->need_dx) return;
+    }
     if (fused != nullptr) {
       PROF(this, "stem_bwd_reduce", (double)N * hs * hs * STEM_CH * es + 3.0 * H * H * 4 * (double)N / fused->S,
            2.0 * N * hs * hs * STEM_CH * 147, st,
@@ -911,6 +1178,12 @@ void dp_engine_destroy(dp_engine* e) {
     if (kv.second.xdesc) cudnnDestroyTensorDescriptor(kv.second.xdesc);
     if (kv.second.ydesc) cudnnDestroyTensorDescriptor(kv.second.ydesc);
   }
+  for (auto& kv : e->wgrad_plans) {
+    cublasLtMatmulDescDestroy(kv.second.op);
+    cublasLtMatrixLayoutDestroy(kv.second.a);
+    cublasLtMatrixLayoutDestroy(kv.second.b);
+    cublasLtMatrixLayoutDestroy(kv.second.c);
+  }
   for (auto& kv : e->gemm_plans) {
     cublasLtMatmulDescDestroy(kv.second.op);
     cublasLtMatrixLayoutDestroy(kv.second.a);
@@ -947,6 +1220,15 @@ int32_t dp_engine_load_weights(dp_engine* e, int32_t n, const char* const* names
   if (!e) fail("null engine");
   CUDA_OK(cudaSetDevice(e->cfg.device));
   e->load_weights(n, names, ptrs, numels);
+  DP_CATCH
+}
+
+int32_t dp_engine_load_weights_dev(dp_engine* e, int32_t n, const char* const* names, const float* const* dev_ptrs,
+                                   const int64_t* numels, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  e->load_weights_dev(n, names, dev_ptrs, numels, (cudaStream_t)stream);
   DP_CATCH
 }
 
@@ -1436,6 +1718,7 @@ static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const
   e->use_lane(0);
   e->eot.gen = e->fwd_gen; e->eot.img = img; e->eot.B = B; e->eot.S = S; e->eot.rects = rects_host != nullptr;
   e->eot.xf = xf_host != nullptr;
+  e->eot.whole = whole;
 }
 
 // Backward: every chunk through dp_engine::backward and K1^T.  A chunk no lane holds any more is recomputed first (its
@@ -1445,28 +1728,66 @@ static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const
 // After a dp_eot_forward_xform, K1^T is the warp adjoint reduce_affine (after the unfused stem dgrad: the fused bf16
 // stem_bwd_reduce has no affine variant), which adds into G with atomics: G is zeroed first, and the same lane rule
 // keeps two streams from adding into one image.
-static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cudaStream_t st) {
-  NvtxRange nvtx_("dorpatch.eot_backward");
-  if (!dlogits || !G) fail("dp_eot_backward: null pointer");
-  if (e->eot.gen < 0) fail("dp_eot_backward: no dp_eot_forward has run on this engine");
+//
+// With parameter gradients (pc, dp_eot_backward_params) every chunk also runs the weight-gradient pass into the
+// accumulators of lane c % lanes, in an order fixed by the shapes (descending chunks per lane with two streams,
+// ascending on one), so that repeated backwards give the same bits whichever chunks the lanes still hold; the lanes'
+// accumulators are added in lane order at the end, by the weight-standardisation adjoint for the convolutions.
+// G may then be null: no input gradient, and the backward stops at the lowest block whose parameters are wanted.
+struct ParamCall { int n; const char* const* names; float* const* grads; int accumulate; };
+static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cudaStream_t st, const ParamCall* pc = nullptr) {
+  NvtxRange nvtx_(pc ? "dorpatch.eot_backward_params" : "dorpatch.eot_backward");
+  const char* fn = pc ? "dp_eot_backward_params" : "dp_eot_backward";
+  if (!dlogits || (!G && !pc)) fail("%s: null pointer", fn);
+  if (e->eot.gen < 0) fail("%s: no dp_eot_forward has run on this engine", fn);
   if (e->eot.gen != e->fwd_gen)
-    fail("dp_eot_backward: stale forward: another forward-type call (dp_predict, dp_attack_grad, dp_net_forward_backward, "
-         "dp_eot_forward or new weights) ran on this engine since the dp_eot_forward it would differentiate");
+    fail("%s: stale forward: another forward-type call (dp_predict, dp_attack_grad, dp_net_forward_backward, "
+         "dp_eot_forward or new weights) ran on this engine since the dp_eot_forward it would differentiate", fn);
   e->check_B(e->eot.B);
   const int B = e->eot.B, S = e->eot.S, N = B * S, H = e->H, K = e->K;
   const int n_chunks = (N + e->chunk - 1) / e->chunk, nl = (int)e->lanes.size();
   const int16_t* rects = e->eot.rects ? e->eot_rects_d : nullptr;
   const bool xf = e->eot.xf;
   const bool dual = nl == 2 && N > e->chunk && (e->chunk % S == 0) && !e->prof_on;
+  cudaStream_t const user_st = st;
+  dp_engine::Wgrad wg{nullptr, G != nullptr, (int)e->blocks.size()};
+  if (pc) {
+    if (pc->n < 0 || (pc->n > 0 && (!pc->names || !pc->grads))) fail("%s: null name / gradient list", fn);
+    std::vector<char> want(e->wparams.size(), 0);
+    for (int i = 0; i < pc->n; ++i) {
+      if (!pc->names[i]) fail("%s: null name at position %d", fn, i);
+      const int pid = (int)(&e->wparam(pc->names[i]) - e->wparams.data());
+      if (!pc->grads[i]) fail("%s: null gradient pointer for '%s'", fn, pc->names[i]);
+      if (want[pid]) fail("%s: '%s' is named twice", fn, pc->names[i]);
+      want[pid] = 1;
+    }
+    e->ensure_wgrad_buffers();
+    e->want = want;
+    size_t lo_off = e->wacc_floats, hi_off = 0;
+    for (size_t i = 0; i < want.size(); ++i) {
+      if (!want[i]) continue;
+      const auto sp = e->wspan(i);
+      lo_off = std::min(lo_off, sp.first); hi_off = std::max(hi_off, sp.second);
+    }
+    if (want[e->stem.pid]) wg.lo = 0;
+    for (int bi = (int)e->blocks.size() - 1; bi >= 0; --bi) {
+      const Block& b = e->blocks[bi];
+      if (e->want_conv(b.c1) || e->want_conv(b.c2) || e->want_conv(b.c3) || (b.has_ds && e->want_conv(b.ds)) ||
+          e->want_gn(b.n1) || e->want_gn(b.n2) || e->want_gn(b.n3)) wg.lo = std::min(wg.lo, bi);
+    }
+    if (hi_off > lo_off)
+      for (int l = 0; l < nl; ++l) CUDA_OK(cudaMemsetAsync(e->wacc[l] + lo_off, 0, (hi_off - lo_off) * 4, user_st));
+  }
   std::vector<int> order;
-  if (dual) {
+  if (pc) {
+    for (int c = 0; c < n_chunks; ++c) order.push_back(dual ? n_chunks - 1 - c : c);
+  } else if (dual) {
     for (int l = 0; l < nl; ++l) if (e->eot_held[l] >= 0) order.push_back(e->eot_held[l]);
     for (int c = 0; c < n_chunks; ++c) if (c != e->eot_held[0] && c != e->eot_held[1]) order.push_back(c);
   } else {
     for (int c = 0; c < n_chunks; ++c) order.push_back(c);
   }
-  cudaStream_t const user_st = st;
-  if (xf) CUDA_OK(cudaMemsetAsync(G, 0, (size_t)B * 3 * H * H * sizeof(float), user_st));
+  if (xf && G) CUDA_OK(cudaMemsetAsync(G, 0, (size_t)B * 3 * H * H * sizeof(float), user_st));
   if (dual) {
     CUDA_OK(cudaEventRecord(e->ev_prep, user_st));
     for (auto& L : e->lanes) CUDA_OK(cudaStreamWaitEvent(L.stream, e->ev_prep, 0));
@@ -1476,8 +1797,10 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
     const int c = order[i], n0 = c * e->chunk, n = std::min(e->chunk, N - n0);
     int lane = -1;
     for (int l = 0; l < nl; ++l) if (e->eot_held[l] == c) lane = l;
+    if (pc) lane = e->eot_held[c % nl] == c ? c % nl : -(1 + c % nl);   // the accumulators of lane c % nl
     const bool recompute = lane < 0;
-    if (recompute) {                                     // evict the held chunk needed latest (never again: latest)
+    if (pc && recompute) lane = -lane - 1;
+    else if (recompute) {                                // evict the held chunk needed latest (never again: latest)
       size_t best_next = 0;
       for (int k = 1; k <= nl; ++k) {
         const int l = (last_lane + k) % nl;              // ties go round-robin, so recomputed chunks alternate lanes
@@ -1504,10 +1827,12 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
     }
     // the caller's rows go to the lane's dlogits buffer: the head GEMM then reads what it reads in dp_attack_grad
     CUDA_OK(cudaMemcpyAsync(e->dlogits, dlogits + (size_t)n0 * K, (size_t)n * K * 4, cudaMemcpyDeviceToDevice, st));
-    const bool fuse = !xf && e->stem_bwd_fused_ok();
+    const bool fuse = !xf && e->stem_bwd_fused_ok() && G;
     dp_engine::FusedReduce fr{rects, G, B, S, n0};
-    e->backward(n, e->dlogits, st, fuse ? &fr : nullptr);
-    if (xf) {
+    wg.input = (!recompute && e->eot.whole) ? (const void*)((const char*)e->net_in_all + (size_t)n0 * e->sample_in_bytes()) : e->net_in;
+    e->backward(n, e->dlogits, st, fuse ? &fr : nullptr, pc ? &wg : nullptr);
+    if (!G) {
+    } else if (xf) {
       PROF(e, "reduce_affine", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
            dp::launch_reduce_affine(e->d_input, e->eot.img, e->eot_xf_d, rects, G, S, n0, n, H, H, e->Cpd, e->bf16, st));
       KERNEL_OK(); ++e->launches;
@@ -1524,6 +1849,22 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
     }
   }
   e->use_lane(0);
+  if (pc) {                                            // lanes added in order; conv weights through the WS adjoint
+    for (int i = 0; i < pc->n; ++i) {
+      const dp_engine::WParam& w = e->wparam(pc->names[i]);
+      const float* a = e->wacc[0] + w.off;
+      const float* b = nl > 1 ? e->wacc[1] + w.off : nullptr;
+      if (w.kind == dp_engine::W_CONV) {
+        const ConvW& c = *w.conv;
+        PROF(e, "ws_wgrad", (double)w.numel * 8 + (double)c.cout * c.k * c.k * c.cin_pad * 4 * nl, 0, user_st,
+             dp::launch_ws_backward(c.raw, a, b, pc->grads[i], c.cout, c.cin, c.k, c.k, c.cin_pad, pc->accumulate != 0, user_st));
+      } else {
+        PROF(e, "vec_wgrad", (double)w.numel * 4 * (nl + 2), 0, user_st,
+             dp::launch_vec_finish(a, b, pc->grads[i], (size_t)w.numel, pc->accumulate != 0, user_st));
+      }
+      KERNEL_OK(); ++e->launches;
+    }
+  }
 }
 
 int32_t dp_eot_forward(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host, float* logits_dev,
@@ -1549,6 +1890,16 @@ int32_t dp_eot_backward(dp_engine* e, const float* dlogits_dev, float* grad_img_
   if (!e) fail("null engine");
   CUDA_OK(cudaSetDevice(e->cfg.device));
   eot_backward_impl(e, dlogits_dev, grad_img_dev, (cudaStream_t)stream);
+  DP_CATCH
+}
+
+int32_t dp_eot_backward_params(dp_engine* e, const float* dlogits_dev, float* grad_img_dev, int32_t n, const char* const* names,
+                               float* const* grad_dev_ptrs, int32_t accumulate, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  ParamCall pc{n, names, grad_dev_ptrs, accumulate};
+  eot_backward_impl(e, dlogits_dev, grad_img_dev, (cudaStream_t)stream, &pc);
   DP_CATCH
 }
 
@@ -1674,6 +2025,47 @@ int32_t dp_debug_stem_bwd_reduce(dp_engine* e, const void* dY, const int16_t* re
   CUDA_OK(cudaMemsetAsync(G, 0, (size_t)B * 3 * e->H * e->H * 4, st));
   dp::launch_stem_bwd_reduce(dY, e->stem.w, e->stem.cin_pad, rects_host ? e->rects_d : nullptr, G, B, S, 0, N, e->H, e->H, st);
   KERNEL_OK(); ++e->launches;
+  DP_CATCH
+}
+
+int32_t dp_debug_stem_wgrad(dp_engine* e, const void* in, const void* dY, int32_t N, float* dW, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  if (!in || !dY || !dW || N < 1) fail("dp_debug_stem_wgrad: bad arguments");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  e->ensure_wgrad_buffers();
+  CUDA_OK(cudaMemsetAsync(dW, 0, (size_t)STEM_CH * 49 * 3 * 4, st));
+  dp::launch_stem_wgrad(in, dY, e->wg_partial[0], dW, N, e->H, e->H, 3, st);
+  KERNEL_OK(); e->launches += 2;
+  DP_CATCH
+}
+
+int32_t dp_debug_gn_wgrad(dp_engine* e, const void* x, const void* dy, const float* gamma, const float* beta, const float* stats,
+                          int32_t N, int32_t P, int32_t C, float* dgb, void* y, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  if (!x || !dy || !gamma || !beta || !stats || !dgb || N < 1 || N > e->chunk || P < 1 || C % dp::GN_GROUPS != 0 || C > 2048)
+    fail("dp_debug_gn_wgrad: bad arguments");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  e->ensure_wgrad_buffers();
+  CUDA_OK(cudaMemsetAsync(dgb, 0, (size_t)2 * C * 4, st));
+  dp::launch_gn_affine_partial(dy, x, gamma, beta, stats, e->wg_partial[0], N, P, C, e->bf16, st); KERNEL_OK();
+  dp::launch_colsum_add(e->wg_partial[0], dgb, N, 2 * C, st); KERNEL_OK();
+  if (y) { dp::launch_gn_apply(x, y, gamma, beta, stats, N, P, C, e->bf16, st); KERNEL_OK(); }
+  e->launches += y ? 3 : 2;
+  DP_CATCH
+}
+
+int32_t dp_debug_ws_backward(dp_engine* e, const float* w_raw, const float* g_a, const float* g_b, int32_t O, int32_t I, int32_t k,
+                             int32_t Ipad, float* out, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  if (!w_raw || !g_a || !out || O < 1 || I < 1 || k < 1 || Ipad < I) fail("dp_debug_ws_backward: bad arguments");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  dp::launch_ws_backward(w_raw, g_a, g_b, out, O, I, k, k, Ipad, false, (cudaStream_t)stream); KERNEL_OK();
+  ++e->launches;
   DP_CATCH
 }
 

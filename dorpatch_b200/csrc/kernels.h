@@ -66,6 +66,27 @@ void launch_gn_gemm_pack(const void* w_nk, void* w_packed, int Nout, int K, cuda
 bool launch_gn_gemm_forward(const void* x, const void* w_packed, const float* stats, const float* gamma, const float* beta,
                             const void* shortcut, void* out, int N, int P, int K, int Nout, cudaStream_t st);
 
+// ---- weight-gradient pass (kernels_wgrad.cu) -------------------------------------------
+// y = relu(gn(x)) from the saved stats [N][32][2] (the forward's arithmetic)
+void launch_gn_apply(const void* x, void* y, const float* gamma, const float* beta, const float* stats, int N, int P,
+                     int C, bool bf16, cudaStream_t st);
+// partial [N][2C]: per sample sum_p dyg * xhat | sum_p dyg, dyg = dy behind the ReLU gate
+void launch_gn_affine_partial(const void* dy, const void* x, const float* gamma, const float* beta, const float* stats,
+                              float* partial, int N, int P, int C, bool bf16, cudaStream_t st);
+// acc[j] += sum_r src[r*M + j] (rows in order)
+void launch_colsum_add(const float* src, float* acc, int rows, int M, cudaStream_t st);
+void launch_add_bf16(const void* src, float* acc, size_t n, cudaStream_t st);
+// out = (accumulate ? out : 0) + a (+ b)
+void launch_vec_finish(const float* a, const float* b, float* out, size_t n, bool accumulate, cudaStream_t st);
+// weight-standardisation adjoint: g (KRSC, Ipad; lanes a + b, b may be null) -> d/d raw weight (OIHW) into out
+void launch_ws_backward(const float* w_raw, const float* g_a, const float* g_b, float* out, int O, int I, int kh, int kw,
+                        int Ipad, bool accumulate, cudaStream_t st);
+// bf16 stem weight gradient: acc [64][7][7][cin_pad] += dW from in [N,H,W,3] and dY [N,H/2,W/2,64];
+// partial: stem_wgrad_partial_floats() floats of scratch
+size_t stem_wgrad_partial_floats();
+void launch_stem_wgrad(const void* in, const void* dY, float* partial, float* acc, int N, int H, int W, int cin_pad,
+                       cudaStream_t st);
+
 // ---- patch-side kernels (kernels_patch.cu) -------------------------------------------
 // utils.clip + add: adv_x = x + min(eps/||m(p-x)||,1) * m(p-x); l2[b], scale[b] dev outputs.
 void launch_paste(const float* x, const float* mask, const float* pattern, float* adv_x, float* l2, float* scale,

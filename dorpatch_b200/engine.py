@@ -118,6 +118,23 @@ class Engine:
         c_num = (C.c_int64 * n)(*[a.size for a in arrs])
         _lib.check(self.lib.dp_engine_load_weights(self.handle, n, c_names, c_ptrs, c_num))
 
+    def load_state_dict_dev(self, state_dict, names=None):
+        """Reload timm-named tensors (any subset) from fp32 CUDA tensors on this engine's device, without a host copy
+        and without rebuilding the engine (dp_engine_load_weights_dev).  Invalidates the last eot_forward."""
+        keys = list(state_dict.keys()) if names is None else list(names)
+        tens = []
+        for k in keys:
+            v = state_dict[k].detach()
+            if not v.is_cuda or v.device.index != self.device:
+                v = v.to("cuda:%d" % self.device)
+            tens.append(v.float().contiguous())
+        n = len(keys)
+        c_names = (C.c_char_p * n)(*[k.encode() for k in keys])
+        c_ptrs = (C.c_void_p * n)(*[t.data_ptr() for t in tens])
+        c_num = (C.c_int64 * n)(*[t.numel() for t in tens])
+        _lib.check(self.lib.dp_engine_load_weights_dev(self.handle, n, c_names, c_ptrs, c_num, self._stream()))
+        self.eot_forwards += 1                   # the engine's last forward is gone
+
     # ------------------------------------------------------------------------------
     def paste(self, x, mask, pattern, eps, out=None):
         """adv_x = x + clip(mask, pattern, x, eps); returns (adv_x, l2[B], scale[B])."""
@@ -190,9 +207,38 @@ class Engine:
         return logits
 
     def eot_backward(self, dlogits, out=None):
-        """d<dlogits, logits>/d img of the last eot_forward, [B,3,H,W] (no weight gradients)."""
+        """d<dlogits, logits>/d img of the last eot_forward, [B,3,H,W] (weight gradients: eot_backward_params)."""
         out = torch.empty(self._eot_shape, dtype=torch.float32, device=dlogits.device) if out is None else out
         _lib.check(self.lib.dp_eot_backward(self.handle, _dev_ptr(dlogits), _dev_ptr(out), self._stream()))
+        return out
+
+    def eot_backward_params(self, dlogits, names, grads, grad_img=True, accumulate=False):
+        """eot_backward plus parameter gradients (dp_eot_backward_params): grads[i] (fp32 CUDA, contiguous, the shape of
+        timm tensor names[i]) receives d<dlogits, logits>/d tensor (written, or added with accumulate=True).
+        grad_img: True -> return the image gradient [B,3,H,W]; a tensor -> written there; False / None -> skipped."""
+        out = None
+        if grad_img is True:
+            out = torch.empty(self._eot_shape, dtype=torch.float32, device=dlogits.device)
+        elif isinstance(grad_img, torch.Tensor):
+            out = grad_img
+        n = len(names)
+        if len(grads) != n:
+            raise ValueError("eot_backward_params: %d names but %d gradient buffers" % (n, len(grads)))
+        from .resnetv2 import param_shapes
+        shapes = param_shapes(self.n_classes)
+        for k, g in zip(names, grads):          # the C ABI carries no sizes: a short buffer would be written past its end
+            if k not in shapes:
+                raise ValueError("eot_backward_params: unknown parameter name %r" % (k,))
+            want = int(np.prod(shapes[k]))
+            if not (isinstance(g, torch.Tensor) and g.is_cuda and g.dtype == torch.float32 and g.is_contiguous()):
+                raise TypeError("eot_backward_params: the gradient buffer of %s must be a contiguous fp32 CUDA tensor" % k)
+            if g.numel() != want:
+                raise ValueError("eot_backward_params: the gradient buffer of %s has %d elements, %s has %d"
+                                 % (k, g.numel(), k, want))
+        c_names = (C.c_char_p * n)(*[k.encode() for k in names])
+        c_ptrs = (C.c_void_p * n)(*[_dev_ptr(g).value for g in grads])
+        _lib.check(self.lib.dp_eot_backward_params(self.handle, _dev_ptr(dlogits), _dev_ptr(out), n, c_names, c_ptrs,
+                                                   1 if accumulate else 0, self._stream()))
         return out
 
     def attack_grad(self, x, mask, pattern, rects, y, crit_targeted, confidence, eps, stage, grad_adv,

@@ -9,8 +9,12 @@ adaptive attack on the PatchCleanser decision, ...), not only the CW loss that `
 The forward is ``dp_eot_forward`` (K1 + the classifier, the logits bit for bit those of ``dp_predict``); the
 backward is ``dp_eot_backward`` (classifier backward + K1^T on the current stream).  What is differentiated:
 
-- the image only.  The classifier's parameters get no ``.grad``: the engine has no weight-gradient pass.  With
-  ``xforms`` (affine / colour EOT, ``dp_eot_forward_xform``) the transform parameters get none either.
+- the image.  The classifier's parameters get no ``.grad`` by default.  With ``param_grads=True`` (or
+  ``ResNetV2.param_grads_(True)`` for ``model(x)``) the parameters that require grad are inputs too, and the backward
+  is ``dp_eot_backward_params``: the engine's weight-gradient pass, run only for those parameters (fine-tuning under
+  cutout / adversarial fine-tuning).  ``.grad`` then accumulates exactly as for an ``nn.Module``; after
+  ``optimizer.step()`` the engine reloads the changed weights on its next use.  With ``xforms`` (affine / colour EOT,
+  ``dp_eot_forward_xform``) the transform parameters get no gradient.
 - once.  ``create_graph=True`` (double backward) raises.
 - the engine's last forward.  A backward after another forward on the same engine (``eot_logits`` again,
   ``dp_predict`` / PatchCleanser, ``generate``) raises instead of returning a gradient of the wrong activations.
@@ -24,10 +28,10 @@ from .utils import unwrap_native
 
 class _EotLogits(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, img, eng, S, rects, xforms):
+    def forward(ctx, img, eng, S, rects, xforms, names, *params):
         logits = eng.eot_forward(img, S, rects, xforms)
-        ctx.eng, ctx.token = eng, eng.eot_forwards
-        ctx.save_for_backward(img)                    # autograd then refuses a backward after an in-place change
+        ctx.eng, ctx.token, ctx.names = eng, eng.eot_forwards, names
+        ctx.save_for_backward(img, *params)           # autograd then refuses a backward after an in-place change
         return logits
 
     @staticmethod
@@ -35,12 +39,22 @@ class _EotLogits(torch.autograd.Function):
         if torch.is_grad_enabled():
             raise RuntimeError("eot_logits: double backward (create_graph=True) is not supported; the engine computes "
                                "first-order input gradients only")
-        img, = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        params = saved[1:]
         eng = ctx.eng
         if eng.eot_forwards != ctx.token:
             raise RuntimeError("eot_logits: the engine ran another eot_forward after this one; its activations are "
                                "gone, so this graph can no longer be differentiated (run the forward again)")
-        return eng.eot_backward(dlogits.contiguous().float()), None, None, None, None
+        d = dlogits.contiguous().float()
+        if ctx.names is None:
+            return eng.eot_backward(d), None, None, None, None, None
+        live = [i for i in range(len(params)) if ctx.needs_input_grad[6 + i]]
+        grads = [torch.empty(params[i].shape, dtype=torch.float32, device=d.device) for i in live]
+        g_img = eng.eot_backward_params(d, [ctx.names[i] for i in live], grads, grad_img=ctx.needs_input_grad[0])
+        out = [None] * len(params)
+        for i, g in zip(live, grads):
+            out[i] = g if g.device == params[i].device else g.to(params[i].device)
+        return (g_img, None, None, None, None, None) + tuple(out)
 
 
 def _check_xforms(xforms, img, S):
@@ -58,7 +72,7 @@ def _check_xforms(xforms, img, S):
     return np.ascontiguousarray(xforms, dtype=np.float32)
 
 
-def eot_logits(model, img, rects=None, S=1, xforms=None):
+def eot_logits(model, img, rects=None, S=1, xforms=None, param_grads=False):
     """Differentiable ``model(occlude(img))``: [B*S, K] logits, sample b*S+s occluding image b with rects[b, s].
 
     model: ``ResNetV2``, ``NormModel(ResNetV2)`` or ``DataParallel`` of either (the native engine; anything else
@@ -69,9 +83,20 @@ def eot_logits(model, img, rects=None, S=1, xforms=None):
     colour)``: sample b*S+s is ``clamp(c * (grid_sample(img_b, affine_grid(theta)) - 0.5) + 0.5 + br, 0, 1)``
     (bilinear, border padding, align_corners=False; theta = xforms[b, s, :6] as 2 x 3, c, br = xforms[b, s, 6:]),
     then occluded -- what ``generate(eot_affine=..., eot_colour=...)`` optimises against.  None: no transform.
-    Differentiable with respect to ``img`` only: the transform parameters get no gradient (see the module docstring).
-    With xforms the input gradient is summed with fp32 atomics, so its last bits can differ from run to run."""
+    Differentiable with respect to ``img``; the transform parameters get no gradient (see the module docstring).
+    With xforms the input gradient is summed with fp32 atomics, so its last bits can differ from run to run.
+    param_grads: also differentiate the classifier's fp32 parameters that require grad (frozen ones get None and
+    cost nothing); the logits are then differentiable even when img does not require grad."""
     net = unwrap_native(model)
+    if not isinstance(param_grads, bool):
+        raise TypeError("eot_logits: param_grads must be True or False, got %r" % (param_grads,))
+    names, params = None, ()
+    if param_grads:
+        named = [(k, p) for k, p in net.named_parameters() if p.requires_grad]
+        for k, p in named:
+            if p.dtype != torch.float32:
+                raise TypeError("eot_logits: param_grads needs fp32 parameters; %s is %s" % (k, p.dtype))
+        names, params = tuple(k for k, _ in named), tuple(p for _, p in named)
     if xforms is not None:
         xforms = _check_xforms(xforms, img, int(S))
     if not (isinstance(img, torch.Tensor) and img.is_cuda):
@@ -83,4 +108,4 @@ def eot_logits(model, img, rects=None, S=1, xforms=None):
     if img.dim() != 4 or img.shape[1] != 3:
         raise ValueError("eot_logits: img must be [B, 3, H, W], got %s" % (tuple(img.shape),))
     eng = net.engine(img.shape[-1], max_images=img.shape[0])
-    return _EotLogits.apply(img.contiguous().float(), eng, S, rects, xforms)
+    return _EotLogits.apply(img.contiguous().float(), eng, S, rects, xforms, names, *params)

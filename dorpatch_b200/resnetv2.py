@@ -24,6 +24,28 @@ WIDTHS = (256, 512, 1024, 2048)
 STEM_CH = 64
 
 
+def param_shapes(num_classes=1000):
+    """{timm name: shape} of every parameter, in state-dict order (no tensors allocated)."""
+    sh = {"stem.conv.weight": (STEM_CH, 3, 7, 7)}
+    cin = STEM_CH
+    for s, (depth, cout) in enumerate(zip(DEPTHS, WIDTHS)):
+        for b in range(depth):
+            c0, mid, p = (cin if b == 0 else cout), cout // 4, "stages.%d.blocks.%d." % (s, b)
+            if b == 0:
+                sh[p + "downsample.conv.weight"] = (cout, c0, 1, 1)
+            sh[p + "norm1.weight"] = sh[p + "norm1.bias"] = (c0,)
+            sh[p + "conv1.weight"] = (mid, c0, 1, 1)
+            sh[p + "norm2.weight"] = sh[p + "norm2.bias"] = (mid,)
+            sh[p + "conv2.weight"] = (mid, mid, 3, 3)
+            sh[p + "norm3.weight"] = sh[p + "norm3.bias"] = (mid,)
+            sh[p + "conv3.weight"] = (cout, mid, 1, 1)
+        cin = cout
+    sh["norm.weight"] = sh["norm.bias"] = (cin,)
+    sh["head.fc.weight"] = (num_classes, cin, 1, 1)
+    sh["head.fc.bias"] = (num_classes,)
+    return sh
+
+
 class _Conv(nn.Module):          # holds `.weight` (OIHW), standardised by the engine at load time
     def __init__(self, cin, cout, k):
         super().__init__()
@@ -88,6 +110,7 @@ class ResNetV2(nn.Module):
         self.head = _Head(cin, num_classes)
         self._engines = {}
         self._version = 0
+        self._param_grads = False
         self.init_weights(seed)
 
     def reset_classifier(self, num_classes):
@@ -126,13 +149,38 @@ class ResNetV2(nn.Module):
         """Weights changed: engines must re-standardise them."""
         self._version += 1
 
+    def param_grads_(self, on=True):
+        """Weight gradients through the engine for ``model(x)`` / ``NormModel`` / ``DataParallel`` (fine-tuning): the
+        parameters that require grad get ``.grad`` (``ops.eot_logits(..., param_grads=True)``), and the logits are
+        differentiable even when x does not require grad.  Off by default; returns self."""
+        self._param_grads = bool(on)
+        return self
+
+    def _param_state(self):
+        return {k: (p._version, p.data_ptr()) for k, p in self.named_parameters()}
+
+    def _refresh(self, eng):
+        """Reload the parameters changed in place since `eng` was loaded (an optimizer step, ``p.copy_``): their
+        ``_version`` counters / storage moved.  Through the device, into the same engine."""
+        cur = self._param_state()
+        held = getattr(eng, "_weights_state", None)
+        if held is None:
+            eng._weights_state = cur
+            return eng
+        changed = [k for k, v in cur.items() if held.get(k) != v]
+        if changed:
+            params = dict(self.named_parameters())
+            eng.load_state_dict_dev({k: params[k] for k in changed})
+            eng._weights_state = cur
+        return eng
+
     # ------------------------------------------------------------------------------
     def engine(self, img, max_images=1, precision=None, chunk=None):
         """The native engine for this model at image size `img` (created on first use)."""
         from .engine import Engine
         forced = getattr(self, "_adopted", None)
         if forced is not None and forced.handle and forced.img == int(img) and forced.max_images >= max_images:
-            return forced
+            return self._refresh(forced)
         precision = precision or os.environ.get("DORPATCH_PRECISION", DEFAULT_PRECISION)
         chunk = int(chunk or os.environ.get("DORPATCH_CHUNK", "128"))
         key = (int(img), precision, chunk, torch.cuda.current_device() if torch.cuda.is_available() else -1)
@@ -144,25 +192,27 @@ class ResNetV2(nn.Module):
             eng = Engine(img=img, n_classes=self.num_classes, precision=precision, chunk=chunk,
                          max_images=max(int(max_images), 1))
             eng.load_state_dict({k: v for k, v in self.state_dict().items()})
+            eng._weights_state = self._param_state()
             from . import runtime
             runtime.register(eng)          # weight-free helpers (utils.clip, patch_selection) reuse it
             ent = (eng, self._version)
             self._engines[key] = ent
-        return ent[0]
+        return self._refresh(ent[0])
 
     def adopt_engine(self, eng):
         """Use an engine the caller already built (and loaded with THESE weights) instead of creating one."""
         self._adopted = eng
+        eng._weights_state = self._param_state()
 
     def forward(self, z):
         """Logits of an already-normalised batch [N,3,H,W] (what timm's module computes).  Differentiable with
         respect to z when z requires grad (``ops.eot_logits`` on z * 0.5 + 0.5, so the engine sees z up to one
-        rounding); the parameters get no gradient."""
+        rounding); the parameters get no gradient unless ``param_grads_(True)``."""
         if not z.is_cuda:
             raise RuntimeError("dorpatch_b200.ResNetV2 runs on the native CUDA engine only (no CPU fallback)")
-        if torch.is_grad_enabled() and z.requires_grad:
+        if torch.is_grad_enabled() and (z.requires_grad or self._param_grads):
             from .ops import eot_logits
-            return eot_logits(self, z.float() * 0.5 + 0.5)
+            return eot_logits(self, z.float() * 0.5 + 0.5, param_grads=self._param_grads)
         eng = self.engine(z.shape[-1])
         z = z.contiguous().float()
         outs = [eng.net_forward_backward(z[i:i + eng.chunk]) for i in range(0, z.shape[0], eng.chunk)]

@@ -106,7 +106,8 @@ def get_normalize(dataset_name, model_name):
 class NormModel(torch.nn.Module):
     """utils.py:71-78.  When the wrapped model is the native ResNetV2 and the normalisation is
     the reference's (0.5, 0.5), the normalisation is fused into the K1 kernel.  There the logits are
-    differentiable with respect to x when x requires grad (``ops.eot_logits``); the parameters get no gradient."""
+    differentiable with respect to x when x requires grad (``ops.eot_logits``); the parameters get no gradient unless
+    the model's ``param_grads_(True)`` is on."""
 
     def __init__(self, model, normalize):
         super(NormModel, self).__init__()
@@ -115,9 +116,9 @@ class NormModel(torch.nn.Module):
 
     def forward(self, x):
         if isinstance(self.model, ResNetV2) and isinstance(self.normalize, Normalize) and self.normalize.is_half_half():
-            if torch.is_grad_enabled() and x.requires_grad:
+            if torch.is_grad_enabled() and (x.requires_grad or self.model._param_grads):
                 from .ops import eot_logits
-                return eot_logits(self, x)
+                return eot_logits(self, x, param_grads=self.model._param_grads)
             return self.model.forward_unit(x)
         return self.model(self.normalize(x))
 

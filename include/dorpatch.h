@@ -71,6 +71,12 @@ void    dp_engine_destroy(dp_engine* e);
  * Conv weights are standardised (timm StdConv2d, eps 1e-8) once on the device. */
 int32_t dp_engine_load_weights(dp_engine* e, int32_t n_tensors, const char* const* names,
                                const float* const* host_ptrs, const int64_t* numels);
+/* Reload the named tensors (any subset of the names above) from fp32 DEVICE buffers, e.g. after an optimizer step,
+ * without rebuilding the engine: conv weights are re-standardised on `stream`, the own-stem / fused-GEMM copies re-packed,
+ * each reloaded GroupNorm's "every gamma > 0" flag recomputed.  Invalidates the last forward.  Requires a prior
+ * dp_engine_load_weights; returns after the copies completed.  Added without changing any other entry point (ABI 9). */
+int32_t dp_engine_load_weights_dev(dp_engine* e, int32_t n_tensors, const char* const* names,
+                                   const float* const* dev_ptrs, const int64_t* numels, void* stream);
 
 /* bytes of device memory the engine holds (workspace + weights) */
 int64_t dp_engine_device_bytes(const dp_engine* e);
@@ -149,6 +155,16 @@ int32_t dp_eot_backward(dp_engine* e, const float* dlogits_dev, float* grad_img_
  * bits of the gradient may vary from run to run.  Added without changing any other entry point: the ABI stays 9. */
 int32_t dp_eot_forward_xform(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host,
                              const float* xform_host, float* logits_dev, void* stream);
+/* dp_eot_backward plus the gradients of the classifier's parameters (fine-tuning).  For each of the n timm names
+ * (dp_engine_load_weights's names) grad_dev_ptrs[i] (fp32 dev, OIHW / vector, the tensor's shape) receives
+ * d<dlogits, logits>/d tensor of the last dp_eot_forward[_xform]: written (accumulate = 0) or added (accumulate = 1).
+ * Unnamed tensors are not computed (a frozen trunk costs nothing below the lowest named block when grad_img_dev is
+ * NULL, which skips the input gradient).  Conv weights get the gradient with respect to the RAW weight (through the
+ * standardisation).  A configuration gives the same bits on every call.  Unknown or repeated names, null pointers and
+ * a stale forward are refused.  Allocates the fp32 accumulators (about 25.5 M floats per lane) on first use.
+ * Added without changing any other entry point: the ABI stays 9. */
+int32_t dp_eot_backward_params(dp_engine* e, const float* dlogits_dev, float* grad_img_dev, int32_t n, const char* const* names,
+                               float* const* grad_dev_ptrs, int32_t accumulate, void* stream);
 
 /* ---- hot loop ------------------------------------------------------------------------ */
 typedef struct dp_attack_args {
@@ -247,6 +263,19 @@ int32_t dp_failed_set_read(dp_engine* e, int32_t b, int32_t* idx_host_out, int32
  *   kernel in front of the wgmma GEMM and the classifier head). */
 int32_t dp_debug_stem_bwd_reduce(dp_engine* e, const void* dY, const int16_t* rects_host, int32_t B, int32_t S, float* G,
                                  void* stream);
+/* bf16 stem weight-gradient kernel of dp_eot_backward_params on caller-supplied operands (tests/test_gpu_param_grad.py):
+ * dW [64,7,7,3] fp32 dev (overwritten) = sum over samples and output pixels of dY [N,H/2,H/2,64] x im2col(in [N,H,H,3]),
+ * both bf16 dev (the tight network input of the bf16 engine). */
+int32_t dp_debug_stem_wgrad(dp_engine* e, const void* in, const void* dY, int32_t N, float* dW, void* stream);
+/* GroupNorm side of the weight-gradient pass on caller-supplied [N,P,C] tensors in the engine's activation dtype, with
+ * caller-supplied stats [N,32,2] (mean, rstd): dgb [2C] fp32 (overwritten) = (sum dyg * xhat | sum dyg) over samples and
+ * pixels, dyg = dy behind the ReLU gate; y (optional, [N,P,C]) = relu(gn(x)) re-applied from those stats. */
+int32_t dp_debug_gn_wgrad(dp_engine* e, const void* x, const void* dy, const float* gamma, const float* beta, const float* stats,
+                          int32_t N, int32_t P, int32_t C, float* dgb, void* y, void* stream);
+/* Weight-standardisation adjoint: out [O,I,k,k] fp32 = d/d raw weight, from w_raw [O,I,k,k] fp32 and the gradient with
+ * respect to the standardised weight g_a (+ g_b, may be NULL) in KRSC [O,k,k,Ipad] fp32 (pad channels ignored). */
+int32_t dp_debug_ws_backward(dp_engine* e, const float* w_raw, const float* g_a, const float* g_b, int32_t O, int32_t I, int32_t k,
+                             int32_t Ipad, float* out, void* stream);
 /* K1 launch-shape sweep hook (tools/k1_step_sweep.py): tile rows / sample groups (0 = the wave-efficiency heuristic) and the
  * store path (0 = bulk stores + 16-byte stores for occluded rows, 1 = 16-byte stores only).  Process-wide. */
 int32_t dp_debug_k1_tuning(int32_t rows, int32_t sg, int32_t mode);

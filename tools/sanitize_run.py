@@ -49,6 +49,15 @@ def main():
         from dorpatch_b200 import eot as PE
         logits = eng.eot_forward(x, S, rects, xforms=PE.sample(np.random.RandomState(1), B, S, 0.5, 0.5))
         eng.eot_backward(torch.randn_like(logits))
+        # the weight-gradient pass over every parameter (two chunks, the first recomputed), with and without the input
+        # gradient: recomputed GroupNorm inputs, GroupNorm affine partials, stem / 1x1 / 3x3 / fc wgrad, WS adjoint
+        from dorpatch_b200.resnetv2 import param_shapes
+        shapes = param_shapes(1000)
+        names = list(shapes)
+        grads = [torch.zeros(shapes[k], device=dev) for k in names]
+        logits = eng.eot_forward(x, S, rects)
+        eng.eot_backward_params(torch.randn_like(logits), names, grads, grad_img=True)
+        eng.eot_backward_params(torch.randn_like(logits), names, grads, grad_img=False, accumulate=True)
     eng.expand(x, S, rects)
     eng.paste(x, m, p, 4.0)
     # the in-step K1 variant (paste fused in), both store paths
