@@ -90,9 +90,6 @@ struct Block {
   bool has_ds;
   GNW n1, n2, n3;
   ConvW ds, c1, c2, c3;
-  // saved tensors / stats for backward (device, per chunk)
-  void* h1 = nullptr; void* h2 = nullptr; void* out = nullptr;
-  float* st1 = nullptr; float* st2 = nullptr; float* st3 = nullptr;
   void* c1p = nullptr; void* c3p = nullptr;   // conv1 / conv3 weights as wgmma operand tiles (DORPATCH_FUSED_GEMM=1)
 };
 
@@ -123,7 +120,6 @@ struct dp_engine {
   void* stem_w_kn = nullptr;
   int H = 224, K = 1000, chunk = 64;
   int num_sms = 132;
-  cudnnHandle_t cudnn = nullptr;
   cublasLtHandle_t lt = nullptr;
   cudnnDataType_t cudnn_dt = CUDNN_DATA_FLOAT;
   cudaDataType_t cuda_dt = CUDA_R_32F;
@@ -137,50 +133,33 @@ struct dp_engine {
   GNW head_gn;
   float* fc_w = nullptr; float* fc_b = nullptr;
 
-  // workspace (sized for `chunk` samples)
-  void* net_in = nullptr;          // [chunk,H,H,Cp]
-  void* act = nullptr;             // scratch activation (stem out / GN outputs)
-  void* act2 = nullptr;            // scratch (subsampled shortcut input)
-  void* x0 = nullptr;              // pooled stem output (saved)
-  int8_t* pool_amax = nullptr;
-  void* g[4] = {nullptr, nullptr, nullptr, nullptr};   // gradient scratch
-  float* gn_partial = nullptr;
-  float* head_stats = nullptr;
-  float* pooled = nullptr; float* dpooled = nullptr;
-  float* logits = nullptr; float* dlogits = nullptr;
-  void* d_input = nullptr;         // result of backward: [n,H,H,Cp]
-  void* lib_ws = nullptr; size_t lib_ws_bytes = 0;
+  size_t lib_ws_bytes = 0;         // each lane's cuDNN / cublasLt workspace
 
-  // ---- lanes: complete per-chunk workspaces.  dp_attack_grad alternates its chunks between two lanes on
-  // two internal streams so that one chunk's kernel tails / memory-bound GroupNorm passes overlap the other
-  // chunk's tensor-core convolutions.  The members above (net_in, act, ..., Block::h1...) always alias the
-  // lane selected by use_lane(); launches capture the pointers at enqueue time, so switching between chunks is safe.
-  struct LaneBufs {
-    void *net_in = nullptr, *act = nullptr, *act2 = nullptr, *x0 = nullptr;
+  // ---- lanes: complete per-chunk workspaces (sized for `chunk` samples).  A chunk loop runs every chunk on lane 0
+  // and the caller's stream, or alternates its chunks between two lanes on two internal streams (LaneWalk) so that one
+  // chunk's kernel tails / memory-bound GroupNorm passes overlap the other chunk's tensor-core convolutions.  Every
+  // classifier pass is given the lane whose buffers, cuDNN handle and weight-gradient accumulators it uses.
+  struct Lane {
+    void* net_in = nullptr;          // [chunk,H,H,Cp]
+    void* act = nullptr;             // scratch activation (stem out / GN outputs)
+    void* act2 = nullptr;            // scratch (subsampled shortcut input)
+    void* x0 = nullptr;              // pooled stem output (saved)
     int8_t* pool_amax = nullptr;
-    void* g[4] = {nullptr, nullptr, nullptr, nullptr};
+    void* g[4] = {nullptr, nullptr, nullptr, nullptr};   // gradient scratch
     float *gn_partial = nullptr, *head_stats = nullptr, *pooled = nullptr, *dpooled = nullptr, *logits = nullptr, *dlogits = nullptr;
     void* lib_ws = nullptr;
-    std::vector<void*> h1, h2, out;
-    std::vector<float*> st1, st2, st3;
+    struct Saved { void *h1, *h2, *out; float *st1, *st2, *st3; };   // per block: saved tensors / stats for backward
+    std::vector<Saved> saved;
     cudaStream_t stream = nullptr;
     cudaEvent_t done = nullptr;
     cudnnHandle_t cudnn = nullptr;
+    // weight gradients (dp_eot_backward_params; allocated on first use): fp32 accumulators, GroupNorm / stem partial
+    // sums, bf16 cuDNN filter gradient before it is added in fp32
+    float* wacc = nullptr; float* wg_partial = nullptr; void* wg_half = nullptr;
+    int held = -1;                   // the dp_eot_forward chunk whose saved activations this lane holds, -1 none
   };
-  std::vector<LaneBufs> lanes;
+  std::vector<Lane> lanes;
   cudaEvent_t ev_prep = nullptr;
-  void use_lane(int l) {
-    cur_lane = l;
-    LaneBufs& L = lanes[l];
-    net_in = L.net_in; act = L.act; act2 = L.act2; x0 = L.x0; pool_amax = L.pool_amax;
-    for (int i = 0; i < 4; ++i) g[i] = L.g[i];
-    gn_partial = L.gn_partial; head_stats = L.head_stats; pooled = L.pooled; dpooled = L.dpooled;
-    logits = L.logits; dlogits = L.dlogits; lib_ws = L.lib_ws; cudnn = L.cudnn;
-    for (size_t i = 0; i < blocks.size(); ++i) {
-      blocks[i].h1 = L.h1[i]; blocks[i].h2 = L.h2[i]; blocks[i].out = L.out[i];
-      blocks[i].st1 = L.st1[i]; blocks[i].st2 = L.st2[i]; blocks[i].st3 = L.st3[i];
-    }
-  }
 
   // per-image buffers (max_images)
   float* adv_x = nullptr; float* dLs = nullptr; float* scale = nullptr; float* l2 = nullptr;
@@ -206,17 +185,19 @@ struct dp_engine {
 
   // ---- dp_eot_forward / dp_eot_backward: what the backward needs of the last forward.  fwd_gen is bumped by every
   // call that overwrites the lane arenas (dp_predict, dp_attack_grad, dp_net_forward_backward, dp_eot_forward, new
-  // weights); a backward whose forward recorded an older generation is refused.  eot_held[l] is the chunk whose saved
-  // activations (pre-norm outputs, GroupNorm statistics, max-pool argmax) lane l still holds, -1 none.
+  // weights); a backward whose forward recorded an older generation is refused.  Lane::held is the chunk whose saved
+  // activations (pre-norm outputs, GroupNorm statistics, max-pool argmax) the lane still holds.
   // xf: the forward warped its samples (dp_eot_forward_xform) with the transforms in eot_xf_d.
   // whole: the forward's K1 wrote every sample to net_in_all (a held chunk's input is its slice there).
   struct EotSig { int64_t gen = -1; const float* img = nullptr; int B = 0, S = 0; bool rects = false, xf = false, whole = false; };
   int64_t fwd_gen = 0;
   EotSig eot;
-  int eot_held[2] = {-1, -1};
   int16_t* eot_rects_d = nullptr; int eot_rects_cap = 0;   // the forward's rectangles (rects_d is shared scratch)
   float* eot_xf_d = nullptr; int eot_xf_cap = 0;           // the forward's transforms (xf_d is dp_attack_grad's)
-  void forward_clobbered() { ++fwd_gen; eot_held[0] = eot_held[1] = -1; }
+  void forward_clobbered() {
+    ++fwd_gen;
+    for (auto& L : lanes) L.held = -1;
+  }
 
   // ---- optional per-category profiler (CUDA events around every launch) --------------
   bool prof_on = false;
@@ -298,6 +279,7 @@ struct dp_engine {
   void* net_in_all = nullptr;
   size_t net_in_all_cap = 0, k1_whole_max = (size_t)4096 << 20;
   size_t sample_in_bytes() const { return (size_t)H * H * Cp * es; }
+  const void* whole_slice(int n0) const { return (const char*)net_in_all + (size_t)n0 * sample_in_bytes(); }
   bool k1_whole_ok(int n) const { return k1_whole_max > 0 && n > chunk && (size_t)n * sample_in_bytes() <= k1_whole_max; }
   bool ensure_net_in_all(int n) {
     if (!k1_whole_ok(n)) return false;
@@ -403,15 +385,11 @@ struct dp_engine {
     CUDA_OK(cudaEventCreateWithFlags(&ev_prep, cudaEventDisableTiming));
     CUDA_OK(cudaStreamCreateWithFlags(&cap_stream, cudaStreamNonBlocking));
     for (int l = 0; l < n_lanes; ++l) {
-      LaneBufs& L = lanes[l];
-      for (auto& b : blocks) {
-        L.h1.push_back(dmalloc(n * b.hin * b.hin * b.mid * es));
-        L.h2.push_back(dmalloc(n * b.hout * b.hout * b.mid * es));
-        L.out.push_back(dmalloc(n * b.hout * b.hout * b.cout * es));
-        L.st1.push_back((float*)dmalloc(n * dp::GN_GROUPS * 2 * 4));
-        L.st2.push_back((float*)dmalloc(n * dp::GN_GROUPS * 2 * 4));
-        L.st3.push_back((float*)dmalloc(n * dp::GN_GROUPS * 2 * 4));
-      }
+      Lane& L = lanes[l];
+      for (auto& b : blocks)
+        L.saved.push_back(Lane::Saved{dmalloc(n * b.hin * b.hin * b.mid * es), dmalloc(n * b.hout * b.hout * b.mid * es),
+                                      dmalloc(n * b.hout * b.hout * b.cout * es), (float*)dmalloc(n * dp::GN_GROUPS * 2 * 4),
+                                      (float*)dmalloc(n * dp::GN_GROUPS * 2 * 4), (float*)dmalloc(n * dp::GN_GROUPS * 2 * 4)});
       L.net_in = dmalloc(n * H * H * Cp * es);
       L.act = dmalloc(n * ma * es);
       L.act2 = dmalloc(n * ma * es / 4 + 256);
@@ -427,10 +405,8 @@ struct dp_engine {
       L.lib_ws = dmalloc(lib_ws_bytes);
       CUDA_OK(cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking));
       CUDA_OK(cudaEventCreateWithFlags(&L.done, cudaEventDisableTiming));
-      if (l == 0) L.cudnn = cudnn;
-      else CUDNN_OK(cudnnCreate(&L.cudnn));
+      CUDNN_OK(cudnnCreate(&L.cudnn));
     }
-    use_lane(0);
     const size_t B = (size_t)cfg.max_images, HW = (size_t)H * H;
     adv_x = (float*)dmalloc(B * 3 * HW * 4);
     dLs = (float*)dmalloc(B * 3 * HW * 4);
@@ -460,9 +436,6 @@ struct dp_engine {
   std::vector<WParam> wparams;
   std::map<std::string, int> wparam_idx;
   size_t wacc_floats = 0, wacc_trunk_end = 0;    // [0, wacc_trunk_end): stem + blocks; the rest: head
-  float* wacc[2] = {nullptr, nullptr};           // per lane
-  float* wg_partial[2] = {nullptr, nullptr};     // per lane: GroupNorm / stem partial sums
-  void* wg_half[2] = {nullptr, nullptr};         // per lane: bf16 cuDNN filter gradient before it is added in fp32
   std::vector<char> want;                        // per wparam: requested by the current call
   // acc_floats: the slot's size (0: the entry lives inside the slot just reserved, at `inner` floats from its start)
   void add_wparam(const std::string& name, int kind, ConvW* c, GNW* g, int64_t numel, size_t acc_floats, size_t inner = 0) {
@@ -511,16 +484,16 @@ struct dp_engine {
     return wparams[it->second];
   }
   void ensure_wgrad_buffers() {
-    if (wacc[0]) return;
+    if (lanes[0].wacc) return;
     size_t part = std::max((size_t)chunk * 2 * WIDTHS[3], dp::stem_wgrad_partial_floats());
     part = std::max(part, (size_t)chunk * 2 * 2048);
     size_t half = 0;
     for (auto& b : blocks) half = std::max(half, (size_t)b.c2.cout * 9 * b.c2.cin_pad);
     half = std::max(half, (size_t)STEM_CH * 49 * stem.cin_pad);
-    for (size_t l = 0; l < lanes.size(); ++l) {
-      wacc[l] = (float*)dmalloc(wacc_floats * 4);
-      wg_partial[l] = (float*)dmalloc(part * 4);
-      wg_half[l] = dmalloc(half * 2);
+    for (auto& L : lanes) {
+      L.wacc = (float*)dmalloc(wacc_floats * 4);
+      L.wg_partial = (float*)dmalloc(part * 4);
+      L.wg_half = dmalloc(half * 2);
     }
   }
   bool want_conv(const ConvW& c) const { return c.pid >= 0 && want[c.pid]; }
@@ -536,8 +509,7 @@ struct dp_engine {
     for (size_t j = i + 1; j < wparams.size(); ++j) if (wparams[j].off > w.off) { end = wparams[j].off; break; }
     return {w.off, end};
   }
-  float* acc_of(int pid) const { return wacc[cur_lane] + wparams[pid].off; }
-  int cur_lane = 0;
+  float* acc_of(const Lane& L, int pid) const { return L.wacc + wparams[pid].off; }
 
   // ---- weights -------------------------------------------------------------------------
   void upload_conv(ConvW& c, const float* host, int64_t numel, cudaStream_t st) {
@@ -668,13 +640,13 @@ struct dp_engine {
     if (cfg.precision == DP_PREC_FP32) return m == CUDNN_FMA_MATH;   // parity mode: no TF32 down-conversion
     return true;
   }
-  void pick_fwd(CudnnPlan& p, const ConvW& c, const void* x, void* y) {
+  void pick_fwd(const Lane& L, CudnnPlan& p, const ConvW& c, const void* x, void* y) {
     cudnnConvolutionFwdAlgoPerf_t perf[16];
     int got = 0;
     if (cfg.autotune)
-      CUDNN_OK(cudnnFindConvolutionForwardAlgorithmEx(cudnn, p.xdesc, x, c.wdesc, c.w, c.cdesc, p.ydesc, y, 16, &got, perf, lib_ws, lib_ws_bytes));
+      CUDNN_OK(cudnnFindConvolutionForwardAlgorithmEx(L.cudnn, p.xdesc, x, c.wdesc, c.w, c.cdesc, p.ydesc, y, 16, &got, perf, L.lib_ws, lib_ws_bytes));
     else
-      CUDNN_OK(cudnnGetConvolutionForwardAlgorithm_v7(cudnn, p.xdesc, c.wdesc, c.cdesc, p.ydesc, 16, &got, perf));
+      CUDNN_OK(cudnnGetConvolutionForwardAlgorithm_v7(L.cudnn, p.xdesc, c.wdesc, c.cdesc, p.ydesc, 16, &got, perf));
     for (int i = 0; i < got; ++i) {
       if (perf[i].status != CUDNN_STATUS_SUCCESS || perf[i].memory > lib_ws_bytes || !math_ok(perf[i].mathType)) continue;
       p.fwd_algo = perf[i].algo; p.fwd_math = perf[i].mathType; p.fwd_ws = perf[i].memory; p.fwd_ready = true;
@@ -682,13 +654,13 @@ struct dp_engine {
     }
     fail("no usable cuDNN forward algorithm (cin=%d cout=%d k=%d stride=%d, %d candidates)", c.cin_pad, c.cout, c.k, c.stride, got);
   }
-  void pick_bwd(CudnnPlan& p, const ConvW& c, const void* dy, void* dx) {
+  void pick_bwd(const Lane& L, CudnnPlan& p, const ConvW& c, const void* dy, void* dx) {
     cudnnConvolutionBwdDataAlgoPerf_t perf[16];
     int got = 0;
     if (cfg.autotune)
-      CUDNN_OK(cudnnFindConvolutionBackwardDataAlgorithmEx(cudnn, c.wdesc, c.w, p.ydesc, dy, c.cdesc, p.xdesc, dx, 16, &got, perf, lib_ws, lib_ws_bytes));
+      CUDNN_OK(cudnnFindConvolutionBackwardDataAlgorithmEx(L.cudnn, c.wdesc, c.w, p.ydesc, dy, c.cdesc, p.xdesc, dx, 16, &got, perf, L.lib_ws, lib_ws_bytes));
     else
-      CUDNN_OK(cudnnGetConvolutionBackwardDataAlgorithm_v7(cudnn, c.wdesc, p.ydesc, c.cdesc, p.xdesc, 16, &got, perf));
+      CUDNN_OK(cudnnGetConvolutionBackwardDataAlgorithm_v7(L.cudnn, c.wdesc, p.ydesc, c.cdesc, p.xdesc, 16, &got, perf));
     // results are sorted by time: take the fastest usable one, but prefer a deterministic algorithm
     // when it is within 25 % of it (a slow "deterministic" dgrad once cost 688 ms on the stem).
     int fastest = -1, det = -1;
@@ -705,26 +677,26 @@ struct dp_engine {
     }
     fail("no usable cuDNN backward-data algorithm (cin=%d cout=%d k=%d stride=%d, %d candidates)", c.cin_pad, c.cout, c.k, c.stride, got);
   }
-  void conv_fwd(int layer_id, const ConvW& c, int N, int hin, int hout, const void* x, void* y, cudaStream_t st) {
+  void conv_fwd(const Lane& L, int layer_id, const ConvW& c, int N, int hin, int hout, const void* x, void* y, cudaStream_t st) {
     CudnnPlan& p = conv_plan(layer_id, c, N, hin, hout);
-    if (!p.fwd_ready) pick_fwd(p, c, x, y);
+    if (!p.fwd_ready) pick_fwd(L, p, c, x, y);
     CUDNN_OK(cudnnSetConvolutionMathType(c.cdesc, p.fwd_math));
     const float one = 1.f, zero = 0.f;
     const double fl = 2.0 * N * hout * hout * c.cout * c.k * c.k * c.cin;
     const double by = ((double)N * hin * hin * c.cin_pad + (double)N * hout * hout * c.cout + (double)c.cout * c.k * c.k * c.cin_pad) * es;
     PROF(this, c.k == 7 ? "stem_conv_fwd" : "conv3x3_fwd", by, fl, st,
-         CUDNN_OK(cudnnConvolutionForward(cudnn, &one, p.xdesc, x, c.wdesc, c.w, c.cdesc, p.fwd_algo, lib_ws, lib_ws_bytes, &zero, p.ydesc, y)));
+         CUDNN_OK(cudnnConvolutionForward(L.cudnn, &one, p.xdesc, x, c.wdesc, c.w, c.cdesc, p.fwd_algo, L.lib_ws, lib_ws_bytes, &zero, p.ydesc, y)));
     ++launches;
   }
-  void conv_bwd(int layer_id, const ConvW& c, int N, int hin, int hout, const void* dy, void* dx, cudaStream_t st) {
+  void conv_bwd(const Lane& L, int layer_id, const ConvW& c, int N, int hin, int hout, const void* dy, void* dx, cudaStream_t st) {
     CudnnPlan& p = conv_plan(layer_id, c, N, hin, hout);
-    if (!p.bwd_ready) pick_bwd(p, c, dy, dx);
+    if (!p.bwd_ready) pick_bwd(L, p, c, dy, dx);
     CUDNN_OK(cudnnSetConvolutionMathType(c.cdesc, p.bwd_math));
     const float one = 1.f, zero = 0.f;
     const double fl = 2.0 * N * hout * hout * c.cout * c.k * c.k * c.cin;
     const double by = ((double)N * hin * hin * c.cin_pad + (double)N * hout * hout * c.cout + (double)c.cout * c.k * c.k * c.cin_pad) * es;
     PROF(this, c.k == 7 ? "stem_conv_bwd" : "conv3x3_bwd", by, fl, st,
-         CUDNN_OK(cudnnConvolutionBackwardData(cudnn, &one, c.wdesc, c.w, p.ydesc, dy, c.cdesc, p.bwd_algo, lib_ws, lib_ws_bytes, &zero, p.xdesc, dx)));
+         CUDNN_OK(cudnnConvolutionBackwardData(L.cudnn, &one, c.wdesc, c.w, p.ydesc, dy, c.cdesc, p.bwd_algo, L.lib_ws, lib_ws_bytes, &zero, p.xdesc, dx)));
     ++launches;
   }
 
@@ -767,7 +739,7 @@ struct dp_engine {
       if (res[i].state == CUBLAS_STATUS_SUCCESS) p.candidates.push_back(res[i].algo);
     return gemm_plans.emplace(key, p).first->second;
   }
-  void gemm(int rows, int nout, int k, int mode, const void* W, const void* X, const void* Cres, float beta, void* D, cudaStream_t st) {
+  void gemm(const Lane& L, int rows, int nout, int k, int mode, const void* W, const void* X, const void* Cres, float beta, void* D, cudaStream_t st) {
     GemmPlan& p = gemm_plan(rows, nout, k, mode);
     const float one = 1.f;
     // Autotune (once per shape): time the heuristic's top candidates on the real operands.  Skipped
@@ -781,7 +753,7 @@ struct dp_engine {
         bool ok = true;
         for (int rep = 0; rep < 3 && ok; ++rep) {
           if (rep == 1) CUDA_OK(cudaEventRecord(e0, st));
-          ok = cublasLtMatmul(lt, p.op, &one, W, p.a, X, p.b, &beta, Cres ? Cres : D, p.c, D, p.c, &cand, lib_ws, lib_ws_bytes, st) == CUBLAS_STATUS_SUCCESS;
+          ok = cublasLtMatmul(lt, p.op, &one, W, p.a, X, p.b, &beta, Cres ? Cres : D, p.c, D, p.c, &cand, L.lib_ws, lib_ws_bytes, st) == CUBLAS_STATUS_SUCCESS;
         }
         if (!ok) continue;
         CUDA_OK(cudaEventRecord(e1, st));
@@ -794,19 +766,19 @@ struct dp_engine {
     }
     const double by = ((double)rows * k + (double)rows * nout * (beta != 0.f ? 2 : 1) + (double)nout * k) * (mode >= 2 ? 4 : es);
     PROF(this, mode == 0 ? "gemm1x1_fwd" : (mode == 1 ? "gemm1x1_bwd" : (mode == 2 ? "fc_fwd" : "fc_bwd")), by, 2.0 * rows * nout * k, st,
-         CUBLAS_OK(cublasLtMatmul(lt, p.op, &one, W, p.a, X, p.b, &beta, Cres ? Cres : D, p.c, D, p.c, &p.algo, lib_ws, lib_ws_bytes, st)));
+         CUBLAS_OK(cublasLtMatmul(lt, p.op, &one, W, p.a, X, p.b, &beta, Cres ? Cres : D, p.c, D, p.c, &p.algo, L.lib_ws, lib_ws_bytes, st)));
     ++launches;
   }
 
   // ---- weight gradients ----------------------------------------------------------------------
   // 3x3 / stem: acc (KRSC, fp32) += dW through cuDNN, deterministic algorithms only, the engine's precision rules.
   // cuDNN's filter gradient has the filter's data type: at bf16 it goes through the lane's bf16 scratch.
-  void conv_wgrad(int layer_id, const ConvW& c, int N, int hin, int hout, const void* x, const void* dy, float* acc, cudaStream_t st) {
+  void conv_wgrad(const Lane& L, int layer_id, const ConvW& c, int N, int hin, int hout, const void* x, const void* dy, float* acc, cudaStream_t st) {
     CudnnPlan& p = conv_plan(layer_id, c, N, hin, hout);
     if (!p.wgd_ready) {
       cudnnConvolutionBwdFilterAlgoPerf_t perf[16];
       int got = 0;
-      CUDNN_OK(cudnnGetConvolutionBackwardFilterAlgorithm_v7(cudnn, p.xdesc, p.ydesc, c.cdesc, c.wdesc, 16, &got, perf));
+      CUDNN_OK(cudnnGetConvolutionBackwardFilterAlgorithm_v7(L.cudnn, p.xdesc, p.ydesc, c.cdesc, c.wdesc, 16, &got, perf));
       for (int i = 0; i < got && !p.wgd_ready; ++i) {
         if (perf[i].status != CUDNN_STATUS_SUCCESS || perf[i].memory > lib_ws_bytes || !math_ok(perf[i].mathType) ||
             perf[i].determinism != CUDNN_DETERMINISTIC) continue;
@@ -821,15 +793,15 @@ struct dp_engine {
     const double fl = 2.0 * N * hout * hout * c.cout * c.k * c.k * c.cin;
     const double by = ((double)N * hin * hin * c.cin_pad + (double)N * hout * hout * c.cout) * es + (double)wn * 8;
     PROF(this, c.k == 7 ? "stem_wgrad" : "conv3x3_wgrad", by, fl, st,
-         CUDNN_OK(cudnnConvolutionBackwardFilter(cudnn, &one, p.xdesc, x, p.ydesc, dy, c.cdesc, p.wgd_algo, lib_ws, lib_ws_bytes,
-                                                 bf16 ? &zero : &one, c.wdesc, bf16 ? wg_half[cur_lane] : (void*)acc)));
+         CUDNN_OK(cudnnConvolutionBackwardFilter(L.cudnn, &one, p.xdesc, x, p.ydesc, dy, c.cdesc, p.wgd_algo, L.lib_ws, lib_ws_bytes,
+                                                 bf16 ? &zero : &one, c.wdesc, bf16 ? L.wg_half : (void*)acc)));
     ++launches;
-    if (bf16) { dp::launch_add_bf16(wg_half[cur_lane], acc, wn, st); KERNEL_OK(); ++launches; }
+    if (bf16) { dp::launch_add_bf16(L.wg_half, acc, wn, st); KERNEL_OK(); ++launches; }
   }
   // 1x1 convolutions and the fc layer: D[cout][cin] (fp32) += dY^T X over `rows` pixels.  Column-major view:
   // D [cin x cout] = X [cin x rows] * (dY [cout x rows])^T.  head: fp32 operands and math (the fc layer is fp32).
   std::map<std::tuple<int, int, int, int>, GemmPlan> wgrad_plans;
-  void wgrad_gemm(int rows, int cout, int cin, const void* X, const void* dY, float* D, bool head, cudaStream_t st) {
+  void wgrad_gemm(const Lane& L, int rows, int cout, int cin, const void* X, const void* dY, float* D, bool head, cudaStream_t st) {
     auto key = std::make_tuple(rows, cout, cin, head ? 1 : 0);
     auto it = wgrad_plans.find(key);
     if (it == wgrad_plans.end()) {
@@ -857,15 +829,14 @@ struct dp_engine {
     const float one = 1.f;
     const double by = ((double)rows * (cin + cout)) * (head ? 4 : es) + (double)cin * cout * 8;
     PROF(this, head ? "fc_wgrad" : "gemm1x1_wgrad", by, 2.0 * rows * cout * cin, st,
-         CUBLAS_OK(cublasLtMatmul(lt, p.op, &one, X, p.a, dY, p.b, &one, D, p.c, D, p.c, &p.algo, lib_ws, lib_ws_bytes, st)));
+         CUBLAS_OK(cublasLtMatmul(lt, p.op, &one, X, p.a, dY, p.b, &one, D, p.c, D, p.c, &p.algo, L.lib_ws, lib_ws_bytes, st)));
     ++launches;
   }
   // GroupNorm affine gradients of one norm: dy at its (ReLU) output, x its input, stats the forward's
-  void gn_wgrad(const GNW& g, const void* dy, const void* x, const float* stats, int N, int P, cudaStream_t st) {
-    float* part = wg_partial[cur_lane];
+  void gn_wgrad(const Lane& L, const GNW& g, const void* dy, const void* x, const float* stats, int N, int P, cudaStream_t st) {
     PROF(this, "gn_affine_wgrad", 2.0 * N * P * g.C * es + (double)N * 2 * g.C * 8, 0, st, {
-      dp::launch_gn_affine_partial(dy, x, g.gamma, g.beta, stats, part, N, P, g.C, bf16, st);
-      dp::launch_colsum_add(part, acc_of(g.pid), N, 2 * g.C, st);
+      dp::launch_gn_affine_partial(dy, x, g.gamma, g.beta, stats, L.wg_partial, N, P, g.C, bf16, st);
+      dp::launch_colsum_add(L.wg_partial, acc_of(L, g.pid), N, 2 * g.C, st);
     }); KERNEL_OK(); launches += 2;
   }
   void gn_apply(const GNW& g, const void* x, const float* stats, void* y, int N, int P, cudaStream_t st) {
@@ -874,12 +845,13 @@ struct dp_engine {
   }
 
   // ---- classifier forward ------------------------------------------------------------------
-  // input: [N,H,H,Cp] T.  train: keep what backward needs.  Leaves logits in `logits`.
-  void forward(int N, const void* input, bool train, cudaStream_t st) {
+  // input: [N,H,H,Cp] T.  train: keep what backward needs.  Leaves logits in L.logits.
+  void forward(const Lane& L, int N, const void* input, bool train, cudaStream_t st) {
     NvtxRange nvtx_("dorpatch.classifier_forward");
     if (!weights_loaded) fail("dp_engine_load_weights has not been called");
     if (N > chunk) fail("forward: N=%d exceeds chunk=%d", N, chunk);
-    CUDNN_OK(cudnnSetStream(cudnn, st));
+    CUDNN_OK(cudnnSetStream(L.cudnn, st));
+    void* const act = L.act;
     const int hs = Hs(), hp = Hp();
     if (own_stem) {
       PROF(this, "stem_conv_fwd", ((double)N * H * H * 3 + (double)N * hs * hs * STEM_CH) * es, 2.0 * N * hs * hs * STEM_CH * 147, st,
@@ -888,14 +860,16 @@ struct dp_engine {
     } else {
       for (int n0 = 0; n0 < N; n0 += STEM_SUB) {   // cuDNN's stem kernels degrade badly beyond ~128 samples of 224x224
         const int n = std::min(STEM_SUB, N - n0);
-        conv_fwd(0, stem, n, H, hs, (const char*)input + (size_t)n0 * H * H * Cp * es, (char*)act + (size_t)n0 * hs * hs * STEM_CH * es, st);
+        conv_fwd(L, 0, stem, n, H, hs, (const char*)input + (size_t)n0 * H * H * Cp * es, (char*)act + (size_t)n0 * hs * hs * STEM_CH * es, st);
       }
     }
     PROF(this, "maxpool_fwd", (double)N * (hs * hs + hp * hp) * STEM_CH * es, 0, st,
-         dp::launch_maxpool_forward(act, x0, train ? pool_amax : nullptr, N, hs, hs, STEM_CH, bf16, st)); KERNEL_OK(); ++launches;
-    const void* cur = x0;
-    int lid = 1;
-    for (auto& b : blocks) {
+         dp::launch_maxpool_forward(act, L.x0, train ? L.pool_amax : nullptr, N, hs, hs, STEM_CH, bf16, st)); KERNEL_OK(); ++launches;
+    const void* cur = L.x0;
+    for (size_t bi = 0; bi < blocks.size(); ++bi) {
+      const Block& b = blocks[bi];
+      const Lane::Saved& s = L.saved[bi];
+      const int lid = (int)bi + 1;
       const int pin_ = b.hin * b.hin, pout = b.hout * b.hout;
       // opt-in: statistics pass + wgmma GEMM that normalises its A operand on the way into shared memory
       // (the relu(gn(.)) tensors of norm1 / norm3 are never written); blocks with a downsample branch keep norm1.
@@ -903,199 +877,287 @@ struct dp_engine {
       const bool fuse3 = fused_gemm && dp::gn_gemm_supported(pout, b.mid, b.cout);
       // xp = relu(gn1(cur))
       if (fuse1) {
-        PROF(this, "gn_stats", 1.0 * N * pin_ * b.cin * es, 0, st, dp::launch_gn_stats(cur, gn_partial, b.st1, N, pin_, b.cin, bf16, st));
+        PROF(this, "gn_stats", 1.0 * N * pin_ * b.cin * es, 0, st, dp::launch_gn_stats(cur, L.gn_partial, s.st1, N, pin_, b.cin, bf16, st));
         KERNEL_OK(); launches += 2;
       } else {
         PROF(this, "gn_relu_fwd", 2.0 * N * pin_ * b.cin * es, 0, st,
-             dp::launch_gn_relu_forward(cur, act, b.n1.gamma, b.n1.beta, gn_partial, b.st1, N, pin_, b.cin, bf16, st)); KERNEL_OK(); launches += 2;
+             dp::launch_gn_relu_forward(cur, act, b.n1.gamma, b.n1.beta, L.gn_partial, s.st1, N, pin_, b.cin, bf16, st)); KERNEL_OK(); launches += 2;
       }
       const void* shortcut = cur;
       if (b.has_ds) {
         const void* src = act;
         if (b.stride == 2) {
-          PROF(this, "subsample", 2.0 * N * pout * b.cin * es, 0, st, dp::launch_subsample2(act, act2, N, b.hin, b.hin, b.cin, bf16, st));
-          KERNEL_OK(); ++launches; src = act2;
+          PROF(this, "subsample", 2.0 * N * pout * b.cin * es, 0, st, dp::launch_subsample2(act, L.act2, N, b.hin, b.hin, b.cin, bf16, st));
+          KERNEL_OK(); ++launches; src = L.act2;
         }
-        gemm(N * pout, b.cout, b.cin, 0, b.ds.w, src, nullptr, 0.f, b.out, st);
-        shortcut = b.out;
+        gemm(L, N * pout, b.cout, b.cin, 0, b.ds.w, src, nullptr, 0.f, s.out, st);
+        shortcut = s.out;
       }
       if (fuse1) {
         PROF(this, "gn_gemm1x1_fwd", ((double)N * pin_ * (b.cin + b.mid) + (double)b.mid * b.cin) * es, 2.0 * N * pin_ * b.mid * b.cin, st,
-             dp::launch_gn_gemm_forward(cur, b.c1p, b.st1, b.n1.gamma, b.n1.beta, nullptr, b.h1, N, pin_, b.cin, b.mid, st));
+             dp::launch_gn_gemm_forward(cur, b.c1p, s.st1, b.n1.gamma, b.n1.beta, nullptr, s.h1, N, pin_, b.cin, b.mid, st));
         KERNEL_OK(); ++launches;
       } else {
-        gemm(N * pin_, b.mid, b.cin, 0, b.c1.w, act, nullptr, 0.f, b.h1, st);
+        gemm(L, N * pin_, b.mid, b.cin, 0, b.c1.w, act, nullptr, 0.f, s.h1, st);
       }
       PROF(this, "gn_relu_fwd", 2.0 * N * pin_ * b.mid * es, 0, st,
-           dp::launch_gn_relu_forward(b.h1, act, b.n2.gamma, b.n2.beta, gn_partial, b.st2, N, pin_, b.mid, bf16, st)); KERNEL_OK(); launches += 2;
-      conv_fwd(lid, b.c2, N, b.hin, b.hout, act, b.h2, st);
+           dp::launch_gn_relu_forward(s.h1, act, b.n2.gamma, b.n2.beta, L.gn_partial, s.st2, N, pin_, b.mid, bf16, st)); KERNEL_OK(); launches += 2;
+      conv_fwd(L, lid, b.c2, N, b.hin, b.hout, act, s.h2, st);
       if (fuse3) {
-        PROF(this, "gn_stats", 1.0 * N * pout * b.mid * es, 0, st, dp::launch_gn_stats(b.h2, gn_partial, b.st3, N, pout, b.mid, bf16, st));
+        PROF(this, "gn_stats", 1.0 * N * pout * b.mid * es, 0, st, dp::launch_gn_stats(s.h2, L.gn_partial, s.st3, N, pout, b.mid, bf16, st));
         KERNEL_OK(); launches += 2;
         PROF(this, "gn_gemm1x1_fwd", ((double)N * pout * (b.mid + 2.0 * b.cout) + (double)b.cout * b.mid) * es, 2.0 * N * pout * b.cout * b.mid, st,
-             dp::launch_gn_gemm_forward(b.h2, b.c3p, b.st3, b.n3.gamma, b.n3.beta, shortcut, b.out, N, pout, b.mid, b.cout, st));
+             dp::launch_gn_gemm_forward(s.h2, b.c3p, s.st3, b.n3.gamma, b.n3.beta, shortcut, s.out, N, pout, b.mid, b.cout, st));
         KERNEL_OK(); ++launches;
       } else {
         PROF(this, "gn_relu_fwd", 2.0 * N * pout * b.mid * es, 0, st,
-             dp::launch_gn_relu_forward(b.h2, act, b.n3.gamma, b.n3.beta, gn_partial, b.st3, N, pout, b.mid, bf16, st)); KERNEL_OK(); launches += 2;
-        gemm(N * pout, b.cout, b.mid, 0, b.c3.w, act, shortcut, 1.f, b.out, st);   // + shortcut fused as C operand
+             dp::launch_gn_relu_forward(s.h2, act, b.n3.gamma, b.n3.beta, L.gn_partial, s.st3, N, pout, b.mid, bf16, st)); KERNEL_OK(); launches += 2;
+        gemm(L, N * pout, b.cout, b.mid, 0, b.c3.w, act, shortcut, 1.f, s.out, st);   // + shortcut fused as C operand
       }
-      cur = b.out;
-      ++lid;
+      cur = s.out;
     }
     const Block& last = blocks.back();
     const int pl = last.hout * last.hout;
     PROF(this, "head_fwd", (double)N * pl * last.cout * es, 2.0 * N * last.cout * K, st, {
-      dp::launch_gn_stats(cur, gn_partial, head_stats, N, pl, last.cout, bf16, st);
-      dp::launch_head_pool(cur, head_gn.gamma, head_gn.beta, head_stats, pooled, N, pl, last.cout, bf16, st);
+      dp::launch_gn_stats(cur, L.gn_partial, L.head_stats, N, pl, last.cout, bf16, st);
+      dp::launch_head_pool(cur, head_gn.gamma, head_gn.beta, L.head_stats, L.pooled, N, pl, last.cout, bf16, st);
     }); KERNEL_OK(); launches += 3;
-    gemm(N, K, last.cout, 2, fc_w, pooled, nullptr, 0.f, logits, st);          // logits = pooled * Wfc^T + b (fp32)
+    gemm(L, N, K, last.cout, 2, fc_w, L.pooled, nullptr, 0.f, L.logits, st);   // logits = pooled * Wfc^T + b (fp32)
   }
 
   // ---- classifier backward (to the input) -----------------------------------------------------
-  // dlog: [N,K] fp32 dev.  Leaves d/d(input) in `d_input` ([N,H,H,Cp] T).
+  // dlog: [N,K] fp32 dev.  Returns d/d(input) ([N,H,H,Cpd] T, in one of the lane's gradient buffers), or null when
+  // nothing of it was produced.
   // `fused`: non-null -> finish with the fused stem-dgrad + masked EOT reduce into fused->G instead of
-  // producing d_input (bf16 own-stem path; the per-sample input gradient is never materialised).
+  // producing d/d(input) (bf16 own-stem path; the per-sample input gradient is never materialised).
   struct FusedReduce { const int16_t* rects; float* G; int B, S, n0; };
   bool fused_stem_bwd = false;     // set at create: own_stem && DORPATCH_STEM_BWD != "cudnn"
   bool fused_pool_bwd = false;     // ... && DORPATCH_POOL_BWD == "fused": max-pool backward fused in as well (slower, off)
-  bool stem_bwd_fused_ok() const { return fused_stem_bwd; }
   // Weight-gradient pass of one chunk (dp_eot_backward_params): accumulates d/d(parameter) of the requested
-  // parameters (`want`) into the current lane's accumulators.  input: the chunk's network input.  need_dx: the
+  // parameters (`want`) into the lane's accumulators.  input: the chunk's network input.  need_dx: the
   // input gradient is wanted too (else the backward stops at block `lo`, the lowest block whose gradients are wanted).
   struct Wgrad { const void* input; bool need_dx; int lo; };
-  void backward(int N, const float* dlog, cudaStream_t st, const FusedReduce* fused = nullptr, const Wgrad* wg = nullptr) {
+  void* backward(const Lane& L, int N, const float* dlog, cudaStream_t st, const FusedReduce* fused = nullptr, const Wgrad* wg = nullptr) {
     NvtxRange nvtx_("dorpatch.classifier_backward");
-    CUDNN_OK(cudnnSetStream(cudnn, st));
+    CUDNN_OK(cudnnSetStream(L.cudnn, st));
+    void* const act = L.act;
+    float* const gn_partial = L.gn_partial;
     const Block& last = blocks.back();
+    const void* const last_out = L.saved.back().out;
     const int pl = last.hout * last.hout;
-    void *GA = g[0], *GB = g[1], *GC = g[2], *GD = g[3];
+    void *GA = L.g[0], *GB = L.g[1], *GC = L.g[2], *GD = L.g[3];
     const bool W = wg != nullptr;
     if (W) {                                                                     // fc: dW += dlogits^T pooled, db += sum dlogits
-      const WParam& fw = wparams[wparam_idx.at("head.fc.weight")];
-      const WParam& fb = wparams[wparam_idx.at("head.fc.bias")];
-      if (want[wparam_idx.at("head.fc.weight")]) wgrad_gemm(N, K, last.cout, pooled, dlog, wacc[cur_lane] + fw.off, true, st);
-      if (want[wparam_idx.at("head.fc.bias")]) {
-        PROF(this, "fc_wgrad", (double)N * K * 4, 0, st, dp::launch_colsum_add(dlog, wacc[cur_lane] + fb.off, N, K, st));
+      const int fw = wparam_idx.at("head.fc.weight"), fb = wparam_idx.at("head.fc.bias");
+      if (want[fw]) wgrad_gemm(L, N, K, last.cout, L.pooled, dlog, acc_of(L, fw), true, st);
+      if (want[fb]) {
+        PROF(this, "fc_wgrad", (double)N * K * 4, 0, st, dp::launch_colsum_add(dlog, acc_of(L, fb), N, K, st));
         KERNEL_OK(); ++launches;
       }
-      if (!wg->need_dx && wg->lo >= (int)blocks.size() && !want_gn(head_gn)) return;
+      if (!wg->need_dx && wg->lo >= (int)blocks.size() && !want_gn(head_gn)) return nullptr;
     }
-    gemm(N, last.cout, K, 3, fc_w, dlog, nullptr, 0.f, dpooled, st);           // dpooled = dlogits * Wfc (fp32)
+    gemm(L, N, last.cout, K, 3, fc_w, dlog, nullptr, 0.f, L.dpooled, st);      // dpooled = dlogits * Wfc (fp32)
     PROF(this, "head_bwd", 2.0 * N * pl * last.cout * es, 0, st, {
-      dp::launch_pool_grad_bcast(dpooled, GB, N, pl, last.cout, bf16, st);
-      dp::launch_gn_relu_backward(GB, last.out, nullptr, GA, head_gn.gamma, head_gn.beta, head_stats, gn_partial, N, pl, last.cout, bf16, st, head_gn.pos);
+      dp::launch_pool_grad_bcast(L.dpooled, GB, N, pl, last.cout, bf16, st);
+      dp::launch_gn_relu_backward(GB, last_out, nullptr, GA, head_gn.gamma, head_gn.beta, L.head_stats, gn_partial, N, pl, last.cout, bf16, st, head_gn.pos);
     }); KERNEL_OK(); launches += 3;
-    if (W && want_gn(head_gn)) gn_wgrad(head_gn, GB, last.out, head_stats, N, pl, st);
+    if (W && want_gn(head_gn)) gn_wgrad(L, head_gn, GB, last_out, L.head_stats, N, pl, st);
     const int lo = W && !wg->need_dx ? wg->lo : 0;
     for (int bi = (int)blocks.size() - 1; bi >= lo; --bi) {
-      Block& b = blocks[bi];
+      const Block& b = blocks[bi];
+      const Lane::Saved& s = L.saved[bi];
       const int lid = bi + 1;
       const int pin_ = b.hin * b.hin, pout = b.hout * b.hout;
-      const void* xin = (bi == 0) ? x0 : blocks[bi - 1].out;
+      const void* xin = (bi == 0) ? L.x0 : L.saved[bi - 1].out;
       // conv3: dY = d_out (GA), X = relu(gn3(h2)) recomputed into act
       if (W && want_conv(b.c3)) {
-        gn_apply(b.n3, b.h2, b.st3, act, N, pout, st);
-        wgrad_gemm(N * pout, b.cout, b.mid, act, GA, acc_of(b.c3.pid), false, st);
+        gn_apply(b.n3, s.h2, s.st3, act, N, pout, st);
+        wgrad_gemm(L, N * pout, b.cout, b.mid, act, GA, acc_of(L, b.c3.pid), false, st);
       }
       // d_a3 = d_out * W3
-      gemm(N * pout, b.mid, b.cout, 1, b.c3.w, GA, nullptr, 0.f, GB, st);
+      gemm(L, N * pout, b.mid, b.cout, 1, b.c3.w, GA, nullptr, 0.f, GB, st);
       PROF(this, "gn_relu_bwd", 3.0 * N * pout * b.mid * es, 0, st,
-           dp::launch_gn_relu_backward(GB, b.h2, nullptr, GC, b.n3.gamma, b.n3.beta, b.st3, gn_partial, N, pout, b.mid, bf16, st, b.n3.pos)); KERNEL_OK(); launches += 2;
-      if (W && want_gn(b.n3)) gn_wgrad(b.n3, GB, b.h2, b.st3, N, pout, st);
+           dp::launch_gn_relu_backward(GB, s.h2, nullptr, GC, b.n3.gamma, b.n3.beta, s.st3, gn_partial, N, pout, b.mid, bf16, st, b.n3.pos)); KERNEL_OK(); launches += 2;
+      if (W && want_gn(b.n3)) gn_wgrad(L, b.n3, GB, s.h2, s.st3, N, pout, st);
       if (W && want_conv(b.c2)) {                                                // conv2: dY = GC, X = relu(gn2(h1))
-        gn_apply(b.n2, b.h1, b.st2, act, N, pin_, st);
-        conv_wgrad(lid, b.c2, N, b.hin, b.hout, act, GC, acc_of(b.c2.pid), st);
+        gn_apply(b.n2, s.h1, s.st2, act, N, pin_, st);
+        conv_wgrad(L, lid, b.c2, N, b.hin, b.hout, act, GC, acc_of(L, b.c2.pid), st);
       }
-      conv_bwd(lid, b.c2, N, b.hin, b.hout, GC, GB, st);
+      conv_bwd(L, lid, b.c2, N, b.hin, b.hout, GC, GB, st);
       PROF(this, "gn_relu_bwd", 3.0 * N * pin_ * b.mid * es, 0, st,
-           dp::launch_gn_relu_backward(GB, b.h1, nullptr, GC, b.n2.gamma, b.n2.beta, b.st2, gn_partial, N, pin_, b.mid, bf16, st, b.n2.pos)); KERNEL_OK(); launches += 2;
-      if (W && want_gn(b.n2)) gn_wgrad(b.n2, GB, b.h1, b.st2, N, pin_, st);
-      if (W && (want_conv(b.c1) || (b.has_ds && want_conv(b.ds)))) gn_apply(b.n1, xin, b.st1, act, N, pin_, st);   // relu(gn1(xin))
-      if (W && want_conv(b.c1)) wgrad_gemm(N * pin_, b.mid, b.cin, act, GC, acc_of(b.c1.pid), false, st);   // conv1: dY = GC
+           dp::launch_gn_relu_backward(GB, s.h1, nullptr, GC, b.n2.gamma, b.n2.beta, s.st2, gn_partial, N, pin_, b.mid, bf16, st, b.n2.pos)); KERNEL_OK(); launches += 2;
+      if (W && want_gn(b.n2)) gn_wgrad(L, b.n2, GB, s.h1, s.st2, N, pin_, st);
+      if (W && (want_conv(b.c1) || (b.has_ds && want_conv(b.ds)))) gn_apply(b.n1, xin, s.st1, act, N, pin_, st);   // relu(gn1(xin))
+      if (W && want_conv(b.c1)) wgrad_gemm(L, N * pin_, b.mid, b.cin, act, GC, acc_of(L, b.c1.pid), false, st);   // conv1: dY = GC
       if (W && b.has_ds && want_conv(b.ds)) {                                    // downsample: dY = GA, X = (subsampled) act
         const void* src = act;
         if (b.stride == 2) {
-          PROF(this, "subsample", 2.0 * N * pout * b.cin * es, 0, st, dp::launch_subsample2(act, act2, N, b.hin, b.hin, b.cin, bf16, st));
-          KERNEL_OK(); ++launches; src = act2;
+          PROF(this, "subsample", 2.0 * N * pout * b.cin * es, 0, st, dp::launch_subsample2(act, L.act2, N, b.hin, b.hin, b.cin, bf16, st));
+          KERNEL_OK(); ++launches; src = L.act2;
         }
-        wgrad_gemm(N * pout, b.cout, b.cin, src, GA, acc_of(b.ds.pid), false, st);
+        wgrad_gemm(L, N * pout, b.cout, b.cin, src, GA, acc_of(L, b.ds.pid), false, st);
       }
-      gemm(N * pin_, b.cin, b.mid, 1, b.c1.w, GC, nullptr, 0.f, GB, st);          // d_xp (conv1 path)
+      gemm(L, N * pin_, b.cin, b.mid, 1, b.c1.w, GC, nullptr, 0.f, GB, st);       // d_xp (conv1 path)
       if (b.has_ds) {
         if (b.stride == 2) {
-          gemm(N * pout, b.cin, b.cout, 1, b.ds.w, GA, nullptr, 0.f, GC, st);
+          gemm(L, N * pout, b.cin, b.cout, 1, b.ds.w, GA, nullptr, 0.f, GC, st);
           PROF(this, "subsample", 3.0 * N * pout * b.cin * es, 0, st, dp::launch_subsample2_adjoint_add(GC, GB, N, b.hin, b.hin, b.cin, bf16, st)); KERNEL_OK(); ++launches;
         } else {
-          gemm(N * pout, b.cin, b.cout, 1, b.ds.w, GA, nullptr, 1.f, GB, st);    // accumulate
+          gemm(L, N * pout, b.cin, b.cout, 1, b.ds.w, GA, nullptr, 1.f, GB, st); // accumulate
         }
         PROF(this, "gn_relu_bwd", 3.0 * N * pin_ * b.cin * es, 0, st,
-             dp::launch_gn_relu_backward(GB, xin, nullptr, GD, b.n1.gamma, b.n1.beta, b.st1, gn_partial, N, pin_, b.cin, bf16, st, b.n1.pos)); KERNEL_OK(); launches += 2;
+             dp::launch_gn_relu_backward(GB, xin, nullptr, GD, b.n1.gamma, b.n1.beta, s.st1, gn_partial, N, pin_, b.cin, bf16, st, b.n1.pos)); KERNEL_OK(); launches += 2;
       } else {
         PROF(this, "gn_relu_bwd", 4.0 * N * pin_ * b.cin * es, 0, st,
-             dp::launch_gn_relu_backward(GB, xin, GA, GD, b.n1.gamma, b.n1.beta, b.st1, gn_partial, N, pin_, b.cin, bf16, st, b.n1.pos)); KERNEL_OK(); launches += 2;
+             dp::launch_gn_relu_backward(GB, xin, GA, GD, b.n1.gamma, b.n1.beta, s.st1, gn_partial, N, pin_, b.cin, bf16, st, b.n1.pos)); KERNEL_OK(); launches += 2;
       }
-      if (W && want_gn(b.n1)) gn_wgrad(b.n1, GB, xin, b.st1, N, pin_, st);
+      if (W && want_gn(b.n1)) gn_wgrad(L, b.n1, GB, xin, s.st1, N, pin_, st);
       std::swap(GA, GD);
     }
     const int hs = Hs();
-    if (W && lo > 0) return;                                                     // nothing below block lo is wanted
-    if (W && !wg->need_dx && !want_conv(stem)) return;
+    if (W && lo > 0) return nullptr;                                             // nothing below block lo is wanted
+    if (W && !wg->need_dx && !want_conv(stem)) return nullptr;
     if (fused != nullptr && fused_pool_bwd && !W) {
-      // max-pool backward + stem dgrad + masked EOT reduce in one kernel: neither d_stem nor d_input is written
+      // max-pool backward + stem dgrad + masked EOT reduce in one kernel: neither d_stem nor d/d(input) is written
       PROF(this, "stem_bwd_reduce", (double)N * (hs / 2) * (hs / 2) * STEM_CH * (es + 1) + 3.0 * H * H * 4 * (double)N / fused->S,
            2.0 * N * hs * hs * STEM_CH * 147, st,
-           dp::launch_stem_bwd_pool_reduce(GA, pool_amax, stem.w, stem.cin_pad, fused->rects, fused->G, fused->B, fused->S, fused->n0, N, H, H, st));
+           dp::launch_stem_bwd_pool_reduce(GA, L.pool_amax, stem.w, stem.cin_pad, fused->rects, fused->G, fused->B, fused->S, fused->n0, N, H, H, st));
       KERNEL_OK(); ++launches;
-      d_input = nullptr;
-      return;
+      return nullptr;
     }
     PROF(this, "maxpool_bwd", (double)N * (hs * hs + (hs / 2) * (hs / 2)) * STEM_CH * es, 0, st,
-         dp::launch_maxpool_backward(GA, pool_amax, GB, N, hs, hs, STEM_CH, bf16, st)); KERNEL_OK(); ++launches;
+         dp::launch_maxpool_backward(GA, L.pool_amax, GB, N, hs, hs, STEM_CH, bf16, st)); KERNEL_OK(); ++launches;
     if (W && want_conv(stem)) {                                                  // stem: dY = the max-pool adjoint (GB)
       if (own_stem) {
         PROF(this, "stem_wgrad", (double)N * (H * H * 3 + hs * hs * STEM_CH) * es, 2.0 * N * hs * hs * STEM_CH * 147, st,
-             dp::launch_stem_wgrad(wg->input, GB, wg_partial[cur_lane], acc_of(stem.pid), N, H, H, stem.cin_pad, st));
+             dp::launch_stem_wgrad(wg->input, GB, L.wg_partial, acc_of(L, stem.pid), N, H, H, stem.cin_pad, st));
         KERNEL_OK(); launches += 2;
       } else {
         for (int n0 = 0; n0 < N; n0 += STEM_SUB) {
           const int n = std::min(STEM_SUB, N - n0);
-          conv_wgrad(0, stem, n, H, hs, (const char*)wg->input + (size_t)n0 * H * H * Cp * es, (const char*)GB + (size_t)n0 * hs * hs * STEM_CH * es,
-                     acc_of(stem.pid), st);
+          conv_wgrad(L, 0, stem, n, H, hs, (const char*)wg->input + (size_t)n0 * H * H * Cp * es, (const char*)GB + (size_t)n0 * hs * hs * STEM_CH * es,
+                     acc_of(L, stem.pid), st);
         }
       }
-      if (!wg->need_dx) return;
+      if (!wg->need_dx) return nullptr;
     }
     if (fused != nullptr) {
       PROF(this, "stem_bwd_reduce", (double)N * hs * hs * STEM_CH * es + 3.0 * H * H * 4 * (double)N / fused->S,
            2.0 * N * hs * hs * STEM_CH * 147, st,
            dp::launch_stem_bwd_reduce(GB, stem.w, stem.cin_pad, fused->rects, fused->G, fused->B, fused->S, fused->n0, N, H, H, st));
       KERNEL_OK(); ++launches;
-      d_input = nullptr;
-      return;
+      return nullptr;
     }
     for (int n0 = 0; n0 < N; n0 += STEM_SUB) {
       const int n = std::min(STEM_SUB, N - n0);
-      conv_bwd(0, stem, n, H, hs, (const char*)GB + (size_t)n0 * hs * hs * STEM_CH * es, (char*)GC + (size_t)n0 * H * H * Cpd * es, st);
+      conv_bwd(L, 0, stem, n, H, hs, (const char*)GB + (size_t)n0 * hs * hs * STEM_CH * es, (char*)GC + (size_t)n0 * H * H * Cpd * es, st);
     }
-    d_input = GC;
+    return GC;
+  }
+
+  // ---- EOT input: K1 and its adjoint K1^T for the chunk loops and the dp_expand* entry points ------------------------
+  // What K1 expands into network input: `img` (plain, or warped per sample by the transforms `xf` [B*S][8]) or the
+  // attack's paste of x / mask / pattern with the clip scale (fused), repeated S times per image and occluded by
+  // `rects` [B*S][4][4] (null: none).
+  struct EotIn {
+    const float* img;
+    const float *x, *mask, *pattern, *scale;
+    const float* xf;
+    const int16_t* rects;
+    int B, S;
+    static EotIn image(const float* img, const float* xf, const int16_t* rects, int B, int S) {
+      return EotIn{img, nullptr, nullptr, nullptr, nullptr, xf, rects, B, S};
+    }
+    static EotIn paste(const float* x, const float* mask, const float* pattern, const float* scale, const int16_t* rects, int B, int S) {
+      return EotIn{nullptr, x, mask, pattern, scale, nullptr, rects, B, S};
+    }
+  };
+  // K1 for samples [n0, n0 + n) into dst.  Algorithmic bytes: the samples written, plus the fp32 planes read once per
+  // image (x, mask and pattern: 7 fused; the image's 3 otherwise).
+  void launch_k1(const EotIn& in, int n0, int n, void* dst, cudaStream_t st) {
+    const bool fused = in.x != nullptr;
+    const double bytes = (double)n * H * H * 3 * es + (fused ? 7.0 : 3.0) * H * H * 4 * (double)n / in.S;
+    if (in.xf)
+      PROF(this, "expand_affine", bytes, 0, st, dp::launch_expand_affine(in.img, in.xf, in.rects, dst, in.S, n0, n, H, H, Cp, bf16, st));
+    else
+      PROF(this, "expand_k1", bytes, 0, st,
+           dp::launch_expand(in.img, in.x, in.mask, in.pattern, in.scale, in.rects, dst, in.B, in.S, n0, n, H, H, Cp, bf16, fused, num_sms, st));
+    KERNEL_OK(); ++launches;
+  }
+  // The network input of samples [n0, n0 + n): their slice of net_in_all when K1 ran once for the whole call, otherwise
+  // K1 into the lane's net_in.
+  const void* chunk_input(const Lane& L, const EotIn& in, int n0, int n, bool whole, cudaStream_t st) {
+    if (whole) return whole_slice(n0);
+    launch_k1(in, n0, n, L.net_in, st);
+    return L.net_in;
+  }
+  // Backward of one chunk from the lane's dlogits, then K1^T into G: the fused bf16 stem dgrad + masked reduce when the
+  // input is not warped, otherwise the library stem dgrad and then reduce_affine (warped) or reduce.  G null: no input
+  // gradient (weight gradients only).
+  void backward_reduce(const Lane& L, const EotIn& in, int n0, int n, float* G, cudaStream_t st, const Wgrad* wg = nullptr) {
+    const bool fuse = G && !in.xf && fused_stem_bwd;
+    const FusedReduce fr{in.rects, G, in.B, in.S, n0};
+    const void* dx = backward(L, n, L.dlogits, st, fuse ? &fr : nullptr, wg);
+    if (!G || fuse) return;
+    const double bytes = (double)n * H * H * 3 * es + 3.0 * H * H * 4 * (double)n / in.S;
+    if (in.xf)
+      PROF(this, "reduce_affine", bytes, 0, st, dp::launch_reduce_affine(dx, in.img, in.xf, in.rects, G, in.S, n0, n, H, H, Cpd, bf16, st));
+    else
+      PROF(this, "reduce_k1t", bytes, 0, st, dp::launch_reduce(dx, in.rects, G, in.B, in.S, n0, n, H, H, Cpd, bf16, st));
+    KERNEL_OK(); ++launches;
   }
 
   // ---- helpers for the attack entry points --------------------------------------------------
-  void h2d_samples(const int16_t* rects_host, int N, cudaStream_t st) {
-    ensure_samples(N);
-    if (rects_host != nullptr) {
-      const size_t bytes = (size_t)N * 16 * sizeof(int16_t);
-      ensure_pin(bytes);
-      memcpy(pin, rects_host, bytes);
-      CUDA_OK(cudaMemcpyAsync(rects_d, pin, bytes, cudaMemcpyHostToDevice, st));
-      CUDA_OK(cudaStreamSynchronize(st));   // `pin` is reused right after
+  // Host table of n rows -> device `table`, first grown to at least n rows (the old one stays in `allocs` until
+  // destroy).  The copy goes through `pin` and is synchronised, since `pin` is reused right after.
+  template <class T>
+  void stage(T*& table, int& cap, const void* host, int n, size_t row_bytes, cudaStream_t st) {
+    if (n > cap) {
+      cap = std::max(n, cap * 2);
+      table = (T*)dmalloc((size_t)cap * row_bytes);
     }
+    const size_t bytes = (size_t)n * row_bytes;
+    ensure_pin(bytes);
+    memcpy(pin, host, bytes);
+    CUDA_OK(cudaMemcpyAsync(table, pin, bytes, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+  }
+  void h2d_samples(const int16_t* rects_host, int N, cudaStream_t st) {
+    ensure_samples(N);                   // every per-sample buffer holds N rows: rects_d does not grow on its own
+    if (rects_host != nullptr) stage(rects_d, cap_samples, rects_host, N, 16 * sizeof(int16_t), st);
   }
   void check_B(int B) const {
     if (B < 1 || B > cfg.max_images) fail("B=%d outside [1, max_images=%d]", B, cfg.max_images);
   }
 };
+
+namespace {
+// The lanes of one chunk loop.  Two lanes run when the engine has them, the call asks for them (more than one chunk,
+// and whatever else the call needs) and the profiler is off (it serialises on one lane so that category times do not
+// overlap).  Then both lane streams first wait for everything enqueued so far on the caller's stream, lane l's chunks
+// run on lane l's stream, and join() makes the caller's stream wait for both.  Otherwise every chunk runs on the
+// caller's stream.
+struct LaneWalk {
+  dp_engine* e;
+  cudaStream_t user;
+  bool dual;
+  LaneWalk(dp_engine* e_, cudaStream_t user_, bool want_dual) : e(e_), user(user_) {
+    dual = want_dual && e->lanes.size() == 2 && !e->prof_on;
+    if (!dual) return;
+    CUDA_OK(cudaEventRecord(e->ev_prep, user));
+    for (auto& L : e->lanes) CUDA_OK(cudaStreamWaitEvent(L.stream, e->ev_prep, 0));
+  }
+  int lane_of(int chunk_id) const { return dual ? chunk_id & 1 : 0; }   // chunks alternating between the lanes
+  cudaStream_t stream(int l) const { return dual ? e->lanes[l].stream : user; }
+  void join() const {
+    if (!dual) return;
+    for (auto& L : e->lanes) {
+      CUDA_OK(cudaEventRecord(L.done, L.stream));
+      CUDA_OK(cudaStreamWaitEvent(user, L.done, 0));
+    }
+  }
+};
+}  // namespace
 
 // =========================================================================================
 // C ABI
@@ -1158,7 +1220,6 @@ int32_t dp_engine_create(const dp_config* cfg, dp_engine** out) {
     e->cudnn_dt = e->bf16 ? CUDNN_DATA_BFLOAT16 : CUDNN_DATA_FLOAT;
     e->cuda_dt = e->bf16 ? CUDA_R_16BF : CUDA_R_32F;
     e->lt_compute = (cfg->precision == DP_PREC_TF32) ? CUBLAS_COMPUTE_32F_FAST_TF32 : CUBLAS_COMPUTE_32F;
-    CUDNN_OK(cudnnCreate(&e->cudnn));
     CUBLAS_OK(cublasLtCreate(&e->lt));
     e->build_arch();
     e->allocate();
@@ -1199,18 +1260,16 @@ void dp_engine_destroy(dp_engine* e) {
   e->drop_graphs();
   for (auto& r : e->prof_recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto ev : e->prof_pool) cudaEventDestroy(ev);
-  for (size_t l = 0; l < e->lanes.size(); ++l) {
-    if (e->lanes[l].stream) cudaStreamDestroy(e->lanes[l].stream);
-    if (e->lanes[l].done) cudaEventDestroy(e->lanes[l].done);
-    if (l > 0 && e->lanes[l].cudnn) cudnnDestroy(e->lanes[l].cudnn);
+  for (auto& L : e->lanes) {
+    if (L.stream) cudaStreamDestroy(L.stream);
+    if (L.done) cudaEventDestroy(L.done);
+    if (L.cudnn) cudnnDestroy(L.cudnn);
   }
-  if (!e->lanes.empty()) e->cudnn = e->lanes[0].cudnn;
   if (e->ev_prep) cudaEventDestroy(e->ev_prep);
   if (e->cap_stream) cudaStreamDestroy(e->cap_stream);
   if (e->net_in_all) cudaFree(e->net_in_all);
   for (void* p : e->allocs) cudaFree(p);
   if (e->pin) cudaFreeHost(e->pin);
-  if (e->cudnn) cudnnDestroy(e->cudnn);
   if (e->lt) cublasLtDestroy(e->lt);
   delete e;
 }
@@ -1314,10 +1373,7 @@ int32_t dp_expand(dp_engine* e, const float* img, int32_t B, int32_t S, const in
   const int N = B * S;
   if (out == nullptr && N > e->chunk) fail("dp_expand: B*S=%d exceeds chunk=%d and no output buffer was given", N, e->chunk);
   e->h2d_samples(rects_host, N, st);
-  PROF(e, "expand_k1", (double)N * e->H * e->H * 3 * e->es + 3.0 * e->H * e->H * 4 * (double)B, 0, st,
-       dp::launch_expand(img, nullptr, nullptr, nullptr, nullptr, rects_host ? e->rects_d : nullptr, out ? out : e->net_in,
-                         B, S, 0, N, e->H, e->H, e->Cp, e->bf16, false, e->num_sms, st));
-  KERNEL_OK(); ++e->launches;
+  e->launch_k1(dp_engine::EotIn::image(img, nullptr, rects_host ? e->rects_d : nullptr, B, S), 0, N, out ? out : e->lanes[0].net_in, st);
   DP_CATCH
 }
 
@@ -1327,10 +1383,7 @@ int32_t dp_expand_dev(dp_engine* e, const float* img, int32_t B, int32_t S, cons
   if (!out) fail("dp_expand_dev needs an output buffer");
   cudaStream_t st = (cudaStream_t)stream;
   CUDA_OK(cudaSetDevice(e->cfg.device));
-  const int N = B * S;
-  PROF(e, "expand_k1", (double)N * e->H * e->H * 3 * e->es + 3.0 * e->H * e->H * 4 * (double)B, 0, st,
-       dp::launch_expand(img, nullptr, nullptr, nullptr, nullptr, rects_dev, out, B, S, 0, N, e->H, e->H, e->Cp, e->bf16, false, e->num_sms, st));
-  KERNEL_OK(); ++e->launches;
+  e->launch_k1(dp_engine::EotIn::image(img, nullptr, rects_dev, B, S), 0, B * S, out, st);
   DP_CATCH
 }
 
@@ -1343,9 +1396,7 @@ int32_t dp_expand_step_dev(dp_engine* e, const float* x, const float* mask, cons
   e->check_B(B);
   cudaStream_t st = (cudaStream_t)stream;
   CUDA_OK(cudaSetDevice(e->cfg.device));
-  PROF(e, "expand_k1", (double)n * e->H * e->H * 3 * e->es + 7.0 * e->H * e->H * 4 * (double)n / S, 0, st,
-       dp::launch_expand(nullptr, x, mask, pattern, e->scale, rects_dev, out, B, S, n0, n, e->H, e->H, e->Cp, e->bf16, true, e->num_sms, st));
-  KERNEL_OK(); ++e->launches;
+  e->launch_k1(dp_engine::EotIn::paste(x, mask, pattern, e->scale, rects_dev, B, S), n0, n, out, st);
   DP_CATCH
 }
 
@@ -1365,33 +1416,18 @@ int32_t dp_predict(dp_engine* e, const float* img, int32_t B, int32_t S, const i
   if (N < 1) fail("dp_predict: empty batch");
   e->forward_clobbered();
   e->h2d_samples(rects_host, N, st);
+  const dp_engine::EotIn in = dp_engine::EotIn::image(img, nullptr, rects_host ? e->rects_d : nullptr, B, S);
   // forward-only scan (collect_failure, PatchCleanser): chunks alternate between the two lanes like dp_attack_grad
-  cudaStream_t const user_st = st;
-  const bool dual = e->lanes.size() == 2 && N > e->chunk && !e->prof_on;
-  if (dual) {
-    CUDA_OK(cudaEventRecord(e->ev_prep, user_st));
-    for (auto& L : e->lanes) CUDA_OK(cudaStreamWaitEvent(L.stream, e->ev_prep, 0));
-  }
-  int chunk_id = 0;
-  for (int n0 = 0; n0 < N; n0 += e->chunk, ++chunk_id) {
+  LaneWalk walk(e, st, N > e->chunk);
+  for (int n0 = 0, c = 0; n0 < N; n0 += e->chunk, ++c) {
     const int n = std::min(e->chunk, N - n0);
-    if (dual) { e->use_lane(chunk_id & 1); st = e->lanes[chunk_id & 1].stream; }
-    PROF(e, "expand_k1", (double)n * e->H * e->H * 3 * e->es + 3.0 * e->H * e->H * 4 * (double)n / S, 0, st,
-         dp::launch_expand(img, nullptr, nullptr, nullptr, nullptr, rects_host ? e->rects_d : nullptr, e->net_in, B, S, n0, n,
-                           e->H, e->H, e->Cp, e->bf16, false, e->num_sms, st));
-    KERNEL_OK(); ++e->launches;
-    e->forward(n, e->net_in, false, st);
-    dp::launch_argmax(e->logits, e->preds_d + n0, n, e->K, st); KERNEL_OK(); ++e->launches;
-    if (logits_host) CUDA_OK(cudaMemcpyAsync(logits_host + (size_t)n0 * e->K, e->logits, (size_t)n * e->K * 4, cudaMemcpyDeviceToHost, st));
+    const dp_engine::Lane& L = e->lanes[walk.lane_of(c)];
+    cudaStream_t const ls = walk.stream(walk.lane_of(c));
+    e->forward(L, n, e->chunk_input(L, in, n0, n, false, ls), false, ls);
+    dp::launch_argmax(L.logits, e->preds_d + n0, n, e->K, ls); KERNEL_OK(); ++e->launches;
+    if (logits_host) CUDA_OK(cudaMemcpyAsync(logits_host + (size_t)n0 * e->K, L.logits, (size_t)n * e->K * 4, cudaMemcpyDeviceToHost, ls));
   }
-  if (dual) {
-    for (auto& L : e->lanes) {
-      CUDA_OK(cudaEventRecord(L.done, L.stream));
-      CUDA_OK(cudaStreamWaitEvent(user_st, L.done, 0));
-    }
-    e->use_lane(0);
-    st = user_st;
-  }
+  walk.join();
   CUDA_OK(cudaMemcpyAsync(preds_host, e->preds_d, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
   DP_CATCH
@@ -1419,63 +1455,25 @@ static void attack_grad_enqueue(dp_engine* e, const dp_attack_args* a, const Gra
     PROF(e, "maskreg", img_bytes, 0, st, dp::launch_maskreg(a->mask, e->loss_density, e->group_lasso, e->win_dev, e->grp_ss, B, H, H, e->unit, st)); KERNEL_OK(); ++e->launches;
   }
   const float inv_s = 1.0f / (float)a->S_total;
-  // Two lanes: chunks alternate between two workspaces / internal streams (only when every chunk holds whole
-  // images, so no two chunks accumulate into the same G[b]).  Everything enqueued so far is on `st`.
-  cudaStream_t const user_st = st;
+  // with transforms each chunk's input is the pasted image adv_x warped; otherwise K1 pastes as it expands
+  const dp_engine::EotIn in = xf_bytes ? dp_engine::EotIn::image(e->adv_x, e->xf_d, rects, B, S)
+                                       : dp_engine::EotIn::paste(a->x, a->mask, a->pattern, e->scale, rects, B, S);
   // K1 once for the whole step when its output fits the budget (see ensure_net_in_all); the chunks read their slices
   const bool k1_whole = !xf_bytes && e->net_in_all != nullptr && e->k1_whole_ok(N) && (size_t)N * e->sample_in_bytes() <= e->net_in_all_cap;
-  if (k1_whole) {
-    PROF(e, "expand_k1", (double)N * H * H * 3 * e->es + 7.0 * H * H * 4 * (double)B, 0, st,
-         dp::launch_expand(nullptr, a->x, a->mask, a->pattern, e->scale, rects, e->net_in_all, B, S, 0, N, H, H, e->Cp, e->bf16, true, e->num_sms, st));
-    KERNEL_OK(); ++e->launches;
-  }
-  // (the per-category profiler serialises on one lane so that category times do not overlap)
-  const bool dual = e->lanes.size() == 2 && N > e->chunk && (e->chunk % S == 0) && !e->prof_on;
-  if (dual) {
-    CUDA_OK(cudaEventRecord(e->ev_prep, user_st));
-    for (auto& L : e->lanes) CUDA_OK(cudaStreamWaitEvent(L.stream, e->ev_prep, 0));
-  }
-  int chunk_id = 0;
-  for (int n0 = 0; n0 < N; n0 += e->chunk, ++chunk_id) {
+  if (k1_whole) e->launch_k1(in, 0, N, e->net_in_all, st);
+  // Two lanes only when every chunk holds whole images, so no two chunks accumulate into the same G[b]
+  LaneWalk walk(e, st, N > e->chunk && e->chunk % S == 0);
+  for (int n0 = 0, c = 0; n0 < N; n0 += e->chunk, ++c) {
     const int n = std::min(e->chunk, N - n0);
-    if (dual) { e->use_lane(chunk_id & 1); st = e->lanes[chunk_id & 1].stream; }
-    const void* chunk_in = e->net_in;
-    if (k1_whole) {
-      chunk_in = (const char*)e->net_in_all + (size_t)n0 * e->sample_in_bytes();
-    } else if (xf_bytes) {
-      PROF(e, "expand_affine", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
-           dp::launch_expand_affine(e->adv_x, e->xf_d, rects, e->net_in, S, n0, n, H, H, e->Cp, e->bf16, st));
-      KERNEL_OK(); ++e->launches;
-    } else {
-      PROF(e, "expand_k1", (double)n * H * H * 3 * e->es + 7.0 * H * H * 4 * (double)n / S, 0, st,
-           dp::launch_expand(nullptr, a->x, a->mask, a->pattern, e->scale, rects, e->net_in, B, S, n0, n, H, H, e->Cp, e->bf16, true, e->num_sms, st));
-      KERNEL_OK(); ++e->launches;
-    }
-    e->forward(n, chunk_in, true, st);
-    PROF(e, "cw_k4", 2.0 * n * e->K * 4, 0, st,
-         dp::launch_cw(e->logits, e->y_d + n0, e->tg_d + n0, a->confidence, inv_s, e->loss_d + n0, e->preds_d + n0, e->dlogits, n, e->K, st));
+    const dp_engine::Lane& L = e->lanes[walk.lane_of(c)];
+    cudaStream_t const ls = walk.stream(walk.lane_of(c));
+    e->forward(L, n, e->chunk_input(L, in, n0, n, k1_whole, ls), true, ls);
+    PROF(e, "cw_k4", 2.0 * n * e->K * 4, 0, ls,
+         dp::launch_cw(L.logits, e->y_d + n0, e->tg_d + n0, a->confidence, inv_s, e->loss_d + n0, e->preds_d + n0, L.dlogits, n, e->K, ls));
     KERNEL_OK(); ++e->launches;
-    const bool fuse = !xf_bytes && e->stem_bwd_fused_ok();
-    dp_engine::FusedReduce fr{rects, a->grad_adv, B, S, n0};
-    e->backward(n, e->dlogits, st, fuse ? &fr : nullptr);
-    if (fuse) continue;
-    if (xf_bytes) {
-      PROF(e, "reduce_affine", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
-           dp::launch_reduce_affine(e->d_input, e->adv_x, e->xf_d, rects, a->grad_adv, S, n0, n, H, H, e->Cpd, e->bf16, st));
-    } else {
-      PROF(e, "reduce_k1t", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
-           dp::launch_reduce(e->d_input, rects, a->grad_adv, B, S, n0, n, H, H, e->Cpd, e->bf16, st));
-    }
-    KERNEL_OK(); ++e->launches;
+    e->backward_reduce(L, in, n0, n, a->grad_adv, ls);
   }
-  if (dual) {
-    for (auto& L : e->lanes) {
-      CUDA_OK(cudaEventRecord(L.done, L.stream));
-      CUDA_OK(cudaStreamWaitEvent(user_st, L.done, 0));
-    }
-    e->use_lane(0);
-    st = user_st;
-  }
+  walk.join();
   // results -> host (pinned staging; the caller synchronises once)
   unsigned char* out = e->pin + L_.d2h_off;
   size_t off = 0;
@@ -1554,7 +1552,6 @@ static void attack_grad_impl(dp_engine* e, const dp_attack_args* a, cudaStream_t
       } else {
         cudaGetLastError();                                // clear the capture error; fall back to eager launches for this signature
         e->launches = l0;
-        e->use_lane(0);
         ent.failed = true;
       }
     }
@@ -1644,7 +1641,7 @@ static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const
   e->check_B(B);
   if (S < 1) fail("%s: S=%d < 1", fn, S);
   if (!rects_host && !xf_host && S != 1) fail("dp_eot_forward: S=%d without rectangles (plain classification needs S=1)", S);
-  const int N = B * S, H = e->H;
+  const int N = B * S;
   if (xf_host)
     for (size_t i = 0; i < (size_t)N * 8; ++i)
       if (!std::isfinite(xf_host[i]))
@@ -1652,70 +1649,21 @@ static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const
              (double)xf_host[i], (int)(i % 8));
   e->forward_clobbered();
   e->eot = dp_engine::EotSig{};
-  if (rects_host) {
-    if (N > e->eot_rects_cap) {                          // the old table stays in `allocs` until destroy
-      e->eot_rects_cap = std::max(N, e->eot_rects_cap * 2);
-      e->eot_rects_d = (int16_t*)e->dmalloc((size_t)e->eot_rects_cap * 16 * sizeof(int16_t));
-    }
-    const size_t bytes = (size_t)N * 16 * sizeof(int16_t);
-    e->ensure_pin(bytes);
-    memcpy(e->pin, rects_host, bytes);
-    CUDA_OK(cudaMemcpyAsync(e->eot_rects_d, e->pin, bytes, cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaStreamSynchronize(st));                  // `pin` is reused right after
-  }
-  if (xf_host) {
-    if (N > e->eot_xf_cap) {                             // the old table stays in `allocs` until destroy
-      e->eot_xf_cap = std::max(N, e->eot_xf_cap * 2);
-      e->eot_xf_d = (float*)e->dmalloc((size_t)e->eot_xf_cap * 8 * sizeof(float));
-    }
-    const size_t bytes = (size_t)N * 8 * sizeof(float);
-    e->ensure_pin(bytes);
-    memcpy(e->pin, xf_host, bytes);
-    CUDA_OK(cudaMemcpyAsync(e->eot_xf_d, e->pin, bytes, cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaStreamSynchronize(st));                  // `pin` is reused right after
-  }
-  const int16_t* rects = rects_host ? e->eot_rects_d : nullptr;
+  if (rects_host) e->stage(e->eot_rects_d, e->eot_rects_cap, rects_host, N, 16 * sizeof(int16_t), st);
+  if (xf_host) e->stage(e->eot_xf_d, e->eot_xf_cap, xf_host, N, 8 * sizeof(float), st);
+  const dp_engine::EotIn in = dp_engine::EotIn::image(img, xf_host ? e->eot_xf_d : nullptr, rects_host ? e->eot_rects_d : nullptr, B, S);
   const bool whole = !xf_host && e->ensure_net_in_all(N);
-  if (whole) {
-    PROF(e, "expand_k1", (double)N * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)B, 0, st,
-         dp::launch_expand(img, nullptr, nullptr, nullptr, nullptr, rects, e->net_in_all, B, S, 0, N, H, H, e->Cp, e->bf16, false, e->num_sms, st));
-    KERNEL_OK(); ++e->launches;
-  }
-  cudaStream_t const user_st = st;
-  const bool dual = e->lanes.size() == 2 && N > e->chunk && !e->prof_on;
-  if (dual) {
-    CUDA_OK(cudaEventRecord(e->ev_prep, user_st));
-    for (auto& L : e->lanes) CUDA_OK(cudaStreamWaitEvent(L.stream, e->ev_prep, 0));
-  }
-  int chunk_id = 0;
-  for (int n0 = 0; n0 < N; n0 += e->chunk, ++chunk_id) {
+  if (whole) e->launch_k1(in, 0, N, e->net_in_all, st);
+  LaneWalk walk(e, st, N > e->chunk);
+  for (int n0 = 0, c = 0; n0 < N; n0 += e->chunk, ++c) {
     const int n = std::min(e->chunk, N - n0);
-    const int lane = dual ? (chunk_id & 1) : 0;
-    e->use_lane(lane);
-    if (dual) st = e->lanes[lane].stream;
-    const void* chunk_in = e->net_in;
-    if (whole) {
-      chunk_in = (const char*)e->net_in_all + (size_t)n0 * e->sample_in_bytes();
-    } else if (xf_host) {
-      PROF(e, "expand_affine", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
-           dp::launch_expand_affine(img, e->eot_xf_d, rects, e->net_in, S, n0, n, H, H, e->Cp, e->bf16, st));
-      KERNEL_OK(); ++e->launches;
-    } else {
-      PROF(e, "expand_k1", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
-           dp::launch_expand(img, nullptr, nullptr, nullptr, nullptr, rects, e->net_in, B, S, n0, n, H, H, e->Cp, e->bf16, false, e->num_sms, st));
-      KERNEL_OK(); ++e->launches;
-    }
-    e->forward(n, chunk_in, true, st);
-    CUDA_OK(cudaMemcpyAsync(logits + (size_t)n0 * e->K, e->logits, (size_t)n * e->K * 4, cudaMemcpyDeviceToDevice, st));
-    e->eot_held[lane] = chunk_id;
+    dp_engine::Lane& L = e->lanes[walk.lane_of(c)];
+    cudaStream_t const ls = walk.stream(walk.lane_of(c));
+    e->forward(L, n, e->chunk_input(L, in, n0, n, whole, ls), true, ls);
+    CUDA_OK(cudaMemcpyAsync(logits + (size_t)n0 * e->K, L.logits, (size_t)n * e->K * 4, cudaMemcpyDeviceToDevice, ls));
+    L.held = c;
   }
-  if (dual) {
-    for (auto& L : e->lanes) {
-      CUDA_OK(cudaEventRecord(L.done, L.stream));
-      CUDA_OK(cudaStreamWaitEvent(user_st, L.done, 0));
-    }
-  }
-  e->use_lane(0);
+  walk.join();
   e->eot.gen = e->fwd_gen; e->eot.img = img; e->eot.B = B; e->eot.S = S; e->eot.rects = rects_host != nullptr;
   e->eot.xf = xf_host != nullptr;
   e->eot.whole = whole;
@@ -1746,10 +1694,8 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
   e->check_B(e->eot.B);
   const int B = e->eot.B, S = e->eot.S, N = B * S, H = e->H, K = e->K;
   const int n_chunks = (N + e->chunk - 1) / e->chunk, nl = (int)e->lanes.size();
-  const int16_t* rects = e->eot.rects ? e->eot_rects_d : nullptr;
-  const bool xf = e->eot.xf;
-  const bool dual = nl == 2 && N > e->chunk && (e->chunk % S == 0) && !e->prof_on;
-  cudaStream_t const user_st = st;
+  const dp_engine::EotIn in = dp_engine::EotIn::image(e->eot.img, e->eot.xf ? e->eot_xf_d : nullptr,
+                                                      e->eot.rects ? e->eot_rects_d : nullptr, B, S);
   dp_engine::Wgrad wg{nullptr, G != nullptr, (int)e->blocks.size()};
   if (pc) {
     if (pc->n < 0 || (pc->n > 0 && (!pc->names || !pc->grads))) fail("%s: null name / gradient list", fn);
@@ -1776,28 +1722,25 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
           e->want_gn(b.n1) || e->want_gn(b.n2) || e->want_gn(b.n3)) wg.lo = std::min(wg.lo, bi);
     }
     if (hi_off > lo_off)
-      for (int l = 0; l < nl; ++l) CUDA_OK(cudaMemsetAsync(e->wacc[l] + lo_off, 0, (hi_off - lo_off) * 4, user_st));
+      for (auto& L : e->lanes) CUDA_OK(cudaMemsetAsync(L.wacc + lo_off, 0, (hi_off - lo_off) * 4, st));
   }
+  if (in.xf && G) CUDA_OK(cudaMemsetAsync(G, 0, (size_t)B * 3 * H * H * sizeof(float), st));
+  LaneWalk walk(e, st, N > e->chunk && e->chunk % S == 0);
   std::vector<int> order;
   if (pc) {
-    for (int c = 0; c < n_chunks; ++c) order.push_back(dual ? n_chunks - 1 - c : c);
-  } else if (dual) {
-    for (int l = 0; l < nl; ++l) if (e->eot_held[l] >= 0) order.push_back(e->eot_held[l]);
-    for (int c = 0; c < n_chunks; ++c) if (c != e->eot_held[0] && c != e->eot_held[1]) order.push_back(c);
+    for (int c = 0; c < n_chunks; ++c) order.push_back(walk.dual ? n_chunks - 1 - c : c);
+  } else if (walk.dual) {
+    for (auto& L : e->lanes) if (L.held >= 0) order.push_back(L.held);
+    for (int c = 0; c < n_chunks; ++c) if (c != e->lanes[0].held && c != e->lanes[1].held) order.push_back(c);
   } else {
     for (int c = 0; c < n_chunks; ++c) order.push_back(c);
-  }
-  if (xf && G) CUDA_OK(cudaMemsetAsync(G, 0, (size_t)B * 3 * H * H * sizeof(float), user_st));
-  if (dual) {
-    CUDA_OK(cudaEventRecord(e->ev_prep, user_st));
-    for (auto& L : e->lanes) CUDA_OK(cudaStreamWaitEvent(L.stream, e->ev_prep, 0));
   }
   int last_lane = nl - 1;
   for (size_t i = 0; i < order.size(); ++i) {
     const int c = order[i], n0 = c * e->chunk, n = std::min(e->chunk, N - n0);
     int lane = -1;
-    for (int l = 0; l < nl; ++l) if (e->eot_held[l] == c) lane = l;
-    if (pc) lane = e->eot_held[c % nl] == c ? c % nl : -(1 + c % nl);   // the accumulators of lane c % nl
+    for (int l = 0; l < nl; ++l) if (e->lanes[l].held == c) lane = l;
+    if (pc) lane = e->lanes[c % nl].held == c ? c % nl : -(1 + c % nl);   // the accumulators of lane c % nl
     const bool recompute = lane < 0;
     if (pc && recompute) lane = -lane - 1;
     else if (recompute) {                                // evict the held chunk needed latest (never again: latest)
@@ -1805,62 +1748,38 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
       for (int k = 1; k <= nl; ++k) {
         const int l = (last_lane + k) % nl;              // ties go round-robin, so recomputed chunks alternate lanes
         size_t next = order.size();
-        for (size_t j = i + 1; j < order.size(); ++j) if (order[j] == e->eot_held[l]) { next = j; break; }
+        for (size_t j = i + 1; j < order.size(); ++j) if (order[j] == e->lanes[l].held) { next = j; break; }
         if (lane < 0 || next > best_next) { lane = l; best_next = next; }
       }
     }
     last_lane = lane;
-    e->use_lane(lane);
-    if (dual) st = e->lanes[lane].stream;
+    dp_engine::Lane& L = e->lanes[lane];
+    cudaStream_t const ls = walk.stream(lane);
+    const void* input = e->eot.whole ? e->whole_slice(n0) : L.net_in;   // what the forward left
     if (recompute) {
-      e->eot_held[lane] = -1;
-      if (xf) {
-        PROF(e, "expand_affine", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
-             dp::launch_expand_affine(e->eot.img, e->eot_xf_d, rects, e->net_in, S, n0, n, H, H, e->Cp, e->bf16, st));
-      } else {
-        PROF(e, "expand_k1", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
-             dp::launch_expand(e->eot.img, nullptr, nullptr, nullptr, nullptr, rects, e->net_in, B, S, n0, n, H, H, e->Cp, e->bf16, false, e->num_sms, st));
-      }
-      KERNEL_OK(); ++e->launches;
-      e->forward(n, e->net_in, true, st);
-      e->eot_held[lane] = c;
+      L.held = -1;
+      input = e->chunk_input(L, in, n0, n, false, ls);
+      e->forward(L, n, input, true, ls);
+      L.held = c;
     }
     // the caller's rows go to the lane's dlogits buffer: the head GEMM then reads what it reads in dp_attack_grad
-    CUDA_OK(cudaMemcpyAsync(e->dlogits, dlogits + (size_t)n0 * K, (size_t)n * K * 4, cudaMemcpyDeviceToDevice, st));
-    const bool fuse = !xf && e->stem_bwd_fused_ok() && G;
-    dp_engine::FusedReduce fr{rects, G, B, S, n0};
-    wg.input = (!recompute && e->eot.whole) ? (const void*)((const char*)e->net_in_all + (size_t)n0 * e->sample_in_bytes()) : e->net_in;
-    e->backward(n, e->dlogits, st, fuse ? &fr : nullptr, pc ? &wg : nullptr);
-    if (!G) {
-    } else if (xf) {
-      PROF(e, "reduce_affine", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
-           dp::launch_reduce_affine(e->d_input, e->eot.img, e->eot_xf_d, rects, G, S, n0, n, H, H, e->Cpd, e->bf16, st));
-      KERNEL_OK(); ++e->launches;
-    } else if (!fuse) {
-      PROF(e, "reduce_k1t", (double)n * H * H * 3 * e->es + 3.0 * H * H * 4 * (double)n / S, 0, st,
-           dp::launch_reduce(e->d_input, rects, G, B, S, n0, n, H, H, e->Cpd, e->bf16, st));
-      KERNEL_OK(); ++e->launches;
-    }
+    CUDA_OK(cudaMemcpyAsync(L.dlogits, dlogits + (size_t)n0 * K, (size_t)n * K * 4, cudaMemcpyDeviceToDevice, ls));
+    wg.input = input;
+    e->backward_reduce(L, in, n0, n, G, ls, pc ? &wg : nullptr);
   }
-  if (dual) {
-    for (auto& L : e->lanes) {
-      CUDA_OK(cudaEventRecord(L.done, L.stream));
-      CUDA_OK(cudaStreamWaitEvent(user_st, L.done, 0));
-    }
-  }
-  e->use_lane(0);
+  walk.join();
   if (pc) {                                            // lanes added in order; conv weights through the WS adjoint
     for (int i = 0; i < pc->n; ++i) {
       const dp_engine::WParam& w = e->wparam(pc->names[i]);
-      const float* a = e->wacc[0] + w.off;
-      const float* b = nl > 1 ? e->wacc[1] + w.off : nullptr;
+      const float* a = e->lanes[0].wacc + w.off;
+      const float* b = nl > 1 ? e->lanes[1].wacc + w.off : nullptr;
       if (w.kind == dp_engine::W_CONV) {
         const ConvW& c = *w.conv;
-        PROF(e, "ws_wgrad", (double)w.numel * 8 + (double)c.cout * c.k * c.k * c.cin_pad * 4 * nl, 0, user_st,
-             dp::launch_ws_backward(c.raw, a, b, pc->grads[i], c.cout, c.cin, c.k, c.k, c.cin_pad, pc->accumulate != 0, user_st));
+        PROF(e, "ws_wgrad", (double)w.numel * 8 + (double)c.cout * c.k * c.k * c.cin_pad * 4 * nl, 0, st,
+             dp::launch_ws_backward(c.raw, a, b, pc->grads[i], c.cout, c.cin, c.k, c.k, c.cin_pad, pc->accumulate != 0, st));
       } else {
-        PROF(e, "vec_wgrad", (double)w.numel * 4 * (nl + 2), 0, user_st,
-             dp::launch_vec_finish(a, b, pc->grads[i], (size_t)w.numel, pc->accumulate != 0, user_st));
+        PROF(e, "vec_wgrad", (double)w.numel * 4 * (nl + 2), 0, st,
+             dp::launch_vec_finish(a, b, pc->grads[i], (size_t)w.numel, pc->accumulate != 0, st));
       }
       KERNEL_OK(); ++e->launches;
     }
@@ -1911,13 +1830,14 @@ int32_t dp_net_forward_backward(dp_engine* e, const float* z, int32_t N, float* 
   cudaStream_t st = (cudaStream_t)stream;
   if (N < 1 || N > e->chunk) fail("N=%d outside [1, chunk=%d]", N, e->chunk);
   e->forward_clobbered();
-  dp::launch_pack_nchw(z, e->net_in, N, e->H, e->H, e->Cp, e->bf16, st); KERNEL_OK(); ++e->launches;
-  e->forward(N, e->net_in, dlogits_dev != nullptr, st);
-  if (logits_dev) CUDA_OK(cudaMemcpyAsync(logits_dev, e->logits, (size_t)N * e->K * 4, cudaMemcpyDeviceToDevice, st));
+  const dp_engine::Lane& L = e->lanes[0];
+  dp::launch_pack_nchw(z, L.net_in, N, e->H, e->H, e->Cp, e->bf16, st); KERNEL_OK(); ++e->launches;
+  e->forward(L, N, L.net_in, dlogits_dev != nullptr, st);
+  if (logits_dev) CUDA_OK(cudaMemcpyAsync(logits_dev, L.logits, (size_t)N * e->K * 4, cudaMemcpyDeviceToDevice, st));
   if (dlogits_dev) {
     if (!dz_dev) fail("dz_dev is required when dlogits_dev is given");
-    e->backward(N, dlogits_dev, st);
-    dp::launch_unpack_nhwc(e->d_input, dz_dev, N, e->H, e->H, e->Cpd, e->bf16, st); KERNEL_OK(); ++e->launches;
+    const void* dx = e->backward(L, N, dlogits_dev, st);
+    dp::launch_unpack_nhwc(dx, dz_dev, N, e->H, e->H, e->Cpd, e->bf16, st); KERNEL_OK(); ++e->launches;
   }
   DP_CATCH
 }
@@ -2036,7 +1956,7 @@ int32_t dp_debug_stem_wgrad(dp_engine* e, const void* in, const void* dY, int32_
   cudaStream_t st = (cudaStream_t)stream;
   e->ensure_wgrad_buffers();
   CUDA_OK(cudaMemsetAsync(dW, 0, (size_t)STEM_CH * 49 * 3 * 4, st));
-  dp::launch_stem_wgrad(in, dY, e->wg_partial[0], dW, N, e->H, e->H, 3, st);
+  dp::launch_stem_wgrad(in, dY, e->lanes[0].wg_partial, dW, N, e->H, e->H, 3, st);
   KERNEL_OK(); e->launches += 2;
   DP_CATCH
 }
@@ -2051,8 +1971,8 @@ int32_t dp_debug_gn_wgrad(dp_engine* e, const void* x, const void* dy, const flo
   cudaStream_t st = (cudaStream_t)stream;
   e->ensure_wgrad_buffers();
   CUDA_OK(cudaMemsetAsync(dgb, 0, (size_t)2 * C * 4, st));
-  dp::launch_gn_affine_partial(dy, x, gamma, beta, stats, e->wg_partial[0], N, P, C, e->bf16, st); KERNEL_OK();
-  dp::launch_colsum_add(e->wg_partial[0], dgb, N, 2 * C, st); KERNEL_OK();
+  dp::launch_gn_affine_partial(dy, x, gamma, beta, stats, e->lanes[0].wg_partial, N, P, C, e->bf16, st); KERNEL_OK();
+  dp::launch_colsum_add(e->lanes[0].wg_partial, dgb, N, 2 * C, st); KERNEL_OK();
   if (y) { dp::launch_gn_apply(x, y, gamma, beta, stats, N, P, C, e->bf16, st); KERNEL_OK(); }
   e->launches += y ? 3 : 2;
   DP_CATCH
@@ -2108,12 +2028,12 @@ int32_t dp_debug_gn(dp_engine* e, const void* x, const void* dy, const void* add
   cudaStream_t st = (cudaStream_t)stream;
   if (N > e->chunk) fail("dp_debug_gn: N=%d exceeds chunk=%d (statistics scratch)", N, e->chunk);
   if (y == nullptr) {   // statistics only: the pass in front of the wgmma GEMM / the classifier head
-    dp::launch_gn_stats(x, e->gn_partial, stats, N, P, C, e->bf16, st); KERNEL_OK();
+    dp::launch_gn_stats(x, e->lanes[0].gn_partial, stats, N, P, C, e->bf16, st); KERNEL_OK();
     e->launches += 2;
     return 0;
   }
-  dp::launch_gn_relu_forward(x, y, gamma, beta, e->gn_partial, stats, N, P, C, e->bf16, st); KERNEL_OK();
-  if (dy != nullptr) { dp::launch_gn_relu_backward(dy, x, addend, dx, gamma, beta, stats, e->gn_partial, N, P, C, e->bf16, st, gamma_positive != 0); KERNEL_OK(); }
+  dp::launch_gn_relu_forward(x, y, gamma, beta, e->lanes[0].gn_partial, stats, N, P, C, e->bf16, st); KERNEL_OK();
+  if (dy != nullptr) { dp::launch_gn_relu_backward(dy, x, addend, dx, gamma, beta, stats, e->lanes[0].gn_partial, N, P, C, e->bf16, st, gamma_positive != 0); KERNEL_OK(); }
   e->launches += 4;
   DP_CATCH
 }
