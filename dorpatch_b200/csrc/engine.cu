@@ -66,7 +66,6 @@ thread_local std::string g_last_error;
 constexpr int DEPTHS[4] = {3, 4, 6, 3};
 constexpr int WIDTHS[4] = {256, 512, 1024, 2048};
 constexpr int STEM_CH = 64;
-constexpr int STEM_SUB = 128;   // samples per cuDNN stem-conv call
 // NVTX range around the phases of the hot loop (host side; inside a graph capture they mark the capture, not the replay)
 struct NvtxRange {
   explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
@@ -113,11 +112,7 @@ struct dp_engine {
   dp_config cfg;
   bool bf16 = false;
   size_t es = 4;            // activation element size
-  int Cp = 4;               // channels per pixel of the network INPUT (3 = tight, own stem kernel)
-  int Cpd = 4;              // channels per pixel of d(input) produced by the library dgrad (4 fp32 / 8 bf16)
-  bool own_stem = false;    // bf16: hand-written tensor-core stem forward on the tight C=3 layout
   bool fused_gemm = false;  // opt-in (DORPATCH_FUSED_GEMM=1, bf16): GN+ReLU applied inside the wgmma 1x1-conv GEMM of kernels_gemm.cu
-  void* stem_w_kn = nullptr;
   int H = 224, K = 1000, chunk = 64;
   int num_sms = 132;
   cublasLtHandle_t lt = nullptr;
@@ -128,7 +123,6 @@ struct dp_engine {
   std::vector<void*> allocs;
   bool weights_loaded = false;
 
-  ConvW stem;
   std::vector<Block> blocks;
   GNW head_gn;
   float* fc_w = nullptr; float* fc_b = nullptr;
@@ -140,7 +134,7 @@ struct dp_engine {
   // chunk's kernel tails / memory-bound GroupNorm passes overlap the other chunk's tensor-core convolutions.  Every
   // classifier pass is given the lane whose buffers, cuDNN handle and weight-gradient accumulators it uses.
   struct Lane {
-    void* net_in = nullptr;          // [chunk,H,H,Cp]
+    void* net_in = nullptr;          // [chunk,H,H,stem.in_ch]
     void* act = nullptr;             // scratch activation (stem out / GN outputs)
     void* act2 = nullptr;            // scratch (subsampled shortcut input)
     void* x0 = nullptr;              // pooled stem output (saved)
@@ -278,7 +272,7 @@ struct dp_engine {
   // DORPATCH_K1_WHOLE_MB (default 4096; 0 = one launch per chunk as in round 1).
   void* net_in_all = nullptr;
   size_t net_in_all_cap = 0, k1_whole_max = (size_t)4096 << 20;
-  size_t sample_in_bytes() const { return (size_t)H * H * Cp * es; }
+  size_t sample_in_bytes() const { return (size_t)H * H * stem.in_ch * es; }
   const void* whole_slice(int n0) const { return (const char*)net_in_all + (size_t)n0 * sample_in_bytes(); }
   bool k1_whole_ok(int n) const { return k1_whole_max > 0 && n > chunk && (size_t)n * sample_in_bytes() <= k1_whole_max; }
   bool ensure_net_in_all(int n) {
@@ -315,7 +309,7 @@ struct dp_engine {
       m = std::max(m, (size_t)b.hin * b.hin * std::max(b.cin, b.mid));
       m = std::max(m, (size_t)b.hout * b.hout * b.cout);
     }
-    m = std::max(m, (size_t)H * H * std::max(Cp, Cpd));
+    m = std::max(m, (size_t)H * H * std::max(stem.in_ch, stem.dx_ch));
     return m;
   }
 
@@ -359,8 +353,7 @@ struct dp_engine {
 
   void allocate() {
     const size_t n = (size_t)chunk;
-    make_conv(stem, 3, STEM_CH, 7, 2, 3, Cpd);
-    if (own_stem) stem_w_kn = dmalloc((size_t)160 * 64 * 2);
+    stem.allocate();
     for (auto& b : blocks) {
       make_gn(b.n1, b.cin); make_gn(b.n2, b.mid); make_gn(b.n3, b.mid);
       if (b.has_ds) make_conv(b.ds, b.cin, b.cout, 1, b.stride, 0, b.cin);
@@ -390,7 +383,7 @@ struct dp_engine {
         L.saved.push_back(Lane::Saved{dmalloc(n * b.hin * b.hin * b.mid * es), dmalloc(n * b.hout * b.hout * b.mid * es),
                                       dmalloc(n * b.hout * b.hout * b.cout * es), (float*)dmalloc(n * dp::GN_GROUPS * 2 * 4),
                                       (float*)dmalloc(n * dp::GN_GROUPS * 2 * 4), (float*)dmalloc(n * dp::GN_GROUPS * 2 * 4)});
-      L.net_in = dmalloc(n * H * H * Cp * es);
+      L.net_in = dmalloc(n * H * H * stem.in_ch * es);
       L.act = dmalloc(n * ma * es);
       L.act2 = dmalloc(n * ma * es / 4 + 256);
       L.x0 = dmalloc(n * Hp() * Hp() * STEM_CH * es);
@@ -457,7 +450,7 @@ struct dp_engine {
     add_wparam(pre + ".bias", W_BETA, nullptr, &g, g.C, 0, g.C);
   }
   void build_wparams() {
-    add_conv_param("stem.conv.weight", stem);
+    add_conv_param("stem.conv.weight", stem.conv);
     int s = 0, bi = 0;
     for (auto& b : blocks) {
       char pre[64];
@@ -489,7 +482,7 @@ struct dp_engine {
     part = std::max(part, (size_t)chunk * 2 * 2048);
     size_t half = 0;
     for (auto& b : blocks) half = std::max(half, (size_t)b.c2.cout * 9 * b.c2.cin_pad);
-    half = std::max(half, (size_t)STEM_CH * 49 * stem.cin_pad);
+    half = std::max(half, (size_t)STEM_CH * 49 * stem.conv.cin_pad);
     for (auto& L : lanes) {
       L.wacc = (float*)dmalloc(wacc_floats * 4);
       L.wg_partial = (float*)dmalloc(part * 4);
@@ -512,112 +505,73 @@ struct dp_engine {
   float* acc_of(const Lane& L, int pid) const { return L.wacc + wparams[pid].off; }
 
   // ---- weights -------------------------------------------------------------------------
-  void upload_conv(ConvW& c, const float* host, int64_t numel, cudaStream_t st) {
-    const int64_t want = (int64_t)c.cout * c.cin * c.k * c.k;
-    if (numel != want) fail("conv weight numel %lld != expected %lld", (long long)numel, (long long)want);
-    CUDA_OK(cudaMemcpyAsync(c.raw, host, (size_t)numel * 4, cudaMemcpyHostToDevice, st));
-    dp::launch_weight_standardize(c.raw, c.w, c.cout, c.cin, c.k, c.k, c.cin_pad, bf16, true, st);
-    KERNEL_OK();
-    CUDA_OK(cudaStreamSynchronize(st));
+  void standardize(const ConvW& c, cudaStream_t st) {
+    dp::launch_weight_standardize(c.raw, c.w, c.cout, c.cin, c.k, c.k, c.cin_pad, bf16, true, st); KERNEL_OK();
   }
-  void upload_vec(float* dst, const float* host, int64_t numel, int64_t want) {
-    if (numel != want) fail("vector numel %lld != expected %lld", (long long)numel, (long long)want);
-    CUDA_OK(cudaMemcpy(dst, host, (size_t)numel * 4, cudaMemcpyHostToDevice));
+  // One timm tensor from `src` (kind: H2D or D2D, on st), then what that kind needs: a convolution is re-standardised
+  // and its packed copies rebuilt (the stem's tile, or the fused GEMM's), a GroupNorm's "every gamma > 0" flag (the
+  // packed bf16 ReLU gate) is recomputed from the new values.
+  void load_param(const WParam& w, const float* src, cudaMemcpyKind kind, cudaStream_t st) {
+    const size_t bytes = (size_t)w.numel * 4;
+    switch (w.kind) {
+      case W_CONV: {
+        const ConvW& c = *w.conv;
+        CUDA_OK(cudaMemcpyAsync(c.raw, src, bytes, kind, st));
+        if (&c == &stem.conv) { stem.load(st); break; }
+        standardize(c, st);
+        if (fused_gemm)
+          for (auto& b : blocks) {
+            if (&c == &b.c1) { dp::launch_gn_gemm_pack(b.c1.w, b.c1p, b.mid, b.cin, st); KERNEL_OK(); }
+            if (&c == &b.c3) { dp::launch_gn_gemm_pack(b.c3.w, b.c3p, b.cout, b.mid, st); KERNEL_OK(); }
+          }
+        break;
+      }
+      case W_GAMMA: {
+        GNW& g_ = *w.gn;
+        CUDA_OK(cudaMemcpyAsync(g_.gamma, src, bytes, kind, st));
+        std::vector<float> h(g_.C);
+        CUDA_OK(cudaMemcpyAsync(h.data(), g_.gamma, bytes, cudaMemcpyDeviceToHost, st));   // pageable: returns when done
+        g_.pos = std::all_of(h.begin(), h.end(), [](float v) { return v > 0.f; });
+        break;
+      }
+      case W_BETA: CUDA_OK(cudaMemcpyAsync(w.gn->beta, src, bytes, kind, st)); break;
+      case W_FCW: CUDA_OK(cudaMemcpyAsync(fc_w, src, bytes, kind, st)); break;
+      default: CUDA_OK(cudaMemcpyAsync(fc_b, src, bytes, kind, st)); break;
+    }
   }
-  void upload_gamma(GNW& g_, const float* host, int64_t numel) {
-    upload_vec(g_.gamma, host, numel, g_.C);
-    g_.pos = true;
-    for (int64_t i = 0; i < numel; ++i) g_.pos = g_.pos && (host[i] > 0.f);
-  }
+  // The full set from host memory, on the default stream: every name of the table is required, other names are ignored.
   void load_weights(int n, const char* const* names, const float* const* ptrs, const int64_t* numels) {
     std::map<std::string, int> idx;
     for (int i = 0; i < n; ++i) idx[names[i]] = i;
-    auto get = [&](const std::string& k) -> int {
-      auto it = idx.find(k);
-      if (it == idx.end()) fail("missing weight tensor '%s'", k.c_str());
-      return it->second;
-    };
-    cudaStream_t st = 0;
-    {
-      int i = get("stem.conv.weight");
-      upload_conv(stem, ptrs[i], numels[i], st);
-      if (own_stem) { dp::launch_stem_pack(stem.w, stem_w_kn, stem.cin_pad, st); KERNEL_OK(); CUDA_OK(cudaStreamSynchronize(st)); }
-      int s = 0, bi = 0;
-      for (auto& b : blocks) {
-        char pre[64];
-        snprintf(pre, sizeof(pre), "stages.%d.blocks.%d.", s, bi);
-        auto P = [&](const char* suffix) { return std::string(pre) + suffix; };
-        if (b.has_ds) { i = get(P("downsample.conv.weight")); upload_conv(b.ds, ptrs[i], numels[i], st); }
-        i = get(P("conv1.weight")); upload_conv(b.c1, ptrs[i], numels[i], st);
-        i = get(P("conv2.weight")); upload_conv(b.c2, ptrs[i], numels[i], st);
-        i = get(P("conv3.weight")); upload_conv(b.c3, ptrs[i], numels[i], st);
-        if (fused_gemm) {
-          dp::launch_gn_gemm_pack(b.c1.w, b.c1p, b.mid, b.cin, st); KERNEL_OK();
-          dp::launch_gn_gemm_pack(b.c3.w, b.c3p, b.cout, b.mid, st); KERNEL_OK();
-          CUDA_OK(cudaStreamSynchronize(st));
-        }
-        i = get(P("norm1.weight")); upload_gamma(b.n1, ptrs[i], numels[i]);
-        i = get(P("norm1.bias")); upload_vec(b.n1.beta, ptrs[i], numels[i], b.cin);
-        i = get(P("norm2.weight")); upload_gamma(b.n2, ptrs[i], numels[i]);
-        i = get(P("norm2.bias")); upload_vec(b.n2.beta, ptrs[i], numels[i], b.mid);
-        i = get(P("norm3.weight")); upload_gamma(b.n3, ptrs[i], numels[i]);
-        i = get(P("norm3.bias")); upload_vec(b.n3.beta, ptrs[i], numels[i], b.mid);
-        if (++bi == DEPTHS[s]) { bi = 0; ++s; }
-      }
-      i = get("norm.weight"); upload_gamma(head_gn, ptrs[i], numels[i]);
-      i = get("norm.bias"); upload_vec(head_gn.beta, ptrs[i], numels[i], WIDTHS[3]);
-      i = get("head.fc.weight"); upload_vec(fc_w, ptrs[i], numels[i], (int64_t)K * WIDTHS[3]);
-      i = get("head.fc.bias"); upload_vec(fc_b, ptrs[i], numels[i], K);
+    for (const WParam& w : wparams) {
+      auto it = idx.find(w.name);
+      if (it == idx.end()) fail("missing weight tensor '%s'", w.name.c_str());
+      const int i = it->second;
+      if (numels[i] != w.numel) fail("weight tensor '%s' has %lld elements, expected %lld", names[i], (long long)numels[i], (long long)w.numel);
+      load_param(w, ptrs[i], cudaMemcpyHostToDevice, 0);
     }
+    CUDA_OK(cudaStreamSynchronize(0));
     weights_loaded = true;
     forward_clobbered();
   }
 
-  // Reload named tensors from fp32 device buffers (after an optimizer step): no host copy of the weights; the convs are
-  // re-standardised on the stream and re-packed for the own stem / fused GEMM; each reloaded GroupNorm's gamma > 0
-  // flag (the packed bf16 ReLU gate) is recomputed from the new values.
+  // Reload named tensors from fp32 device buffers (after an optimizer step), on the caller's stream: no host copy of
+  // the weights.  Any subset; everything is checked before anything changes.
   void load_weights_dev(int n, const char* const* names, const float* const* ptrs, const int64_t* numels, cudaStream_t st) {
     if (!weights_loaded) fail("dp_engine_load_weights_dev: load the full set with dp_engine_load_weights first");
     if (n < 0 || (n > 0 && (!names || !ptrs || !numels))) fail("dp_engine_load_weights_dev: null argument");
-    for (int i = 0; i < n; ++i) {                        // check everything before anything changes
+    std::vector<char> seen(wparams.size(), 0);
+    for (int i = 0; i < n; ++i) {
       if (!names[i]) fail("dp_engine_load_weights_dev: null name at position %d", i);
       const WParam& w = wparam(names[i]);
+      if (seen[&w - wparams.data()]++) fail("dp_engine_load_weights_dev: '%s' is named twice", names[i]);
       if (!ptrs[i]) fail("dp_engine_load_weights_dev: null pointer for '%s'", names[i]);
       if (numels[i] != w.numel) fail("dp_engine_load_weights_dev: '%s' has %lld elements, expected %lld", names[i], (long long)numels[i], (long long)w.numel);
     }
     drop_graphs();
     forward_clobbered();
-    std::vector<GNW*> gammas;
-    for (int i = 0; i < n; ++i) {
-      const WParam& w = wparam(names[i]);
-      const size_t bytes = (size_t)w.numel * 4;
-      switch (w.kind) {
-        case W_CONV: {
-          ConvW& c = *w.conv;
-          CUDA_OK(cudaMemcpyAsync(c.raw, ptrs[i], bytes, cudaMemcpyDeviceToDevice, st));
-          dp::launch_weight_standardize(c.raw, c.w, c.cout, c.cin, c.k, c.k, c.cin_pad, bf16, true, st); KERNEL_OK();
-          if (&c == &stem && own_stem) { dp::launch_stem_pack(stem.w, stem_w_kn, stem.cin_pad, st); KERNEL_OK(); }
-          if (fused_gemm)
-            for (auto& b : blocks) {
-              if (&c == &b.c1) { dp::launch_gn_gemm_pack(b.c1.w, b.c1p, b.mid, b.cin, st); KERNEL_OK(); }
-              if (&c == &b.c3) { dp::launch_gn_gemm_pack(b.c3.w, b.c3p, b.cout, b.mid, st); KERNEL_OK(); }
-            }
-          break;
-        }
-        case W_GAMMA: CUDA_OK(cudaMemcpyAsync(w.gn->gamma, ptrs[i], bytes, cudaMemcpyDeviceToDevice, st)); gammas.push_back(w.gn); break;
-        case W_BETA: CUDA_OK(cudaMemcpyAsync(w.gn->beta, ptrs[i], bytes, cudaMemcpyDeviceToDevice, st)); break;
-        case W_FCW: CUDA_OK(cudaMemcpyAsync(fc_w, ptrs[i], bytes, cudaMemcpyDeviceToDevice, st)); break;
-        default: CUDA_OK(cudaMemcpyAsync(fc_b, ptrs[i], bytes, cudaMemcpyDeviceToDevice, st)); break;
-      }
-    }
+    for (int i = 0; i < n; ++i) load_param(wparam(names[i]), ptrs[i], cudaMemcpyDeviceToDevice, st);
     CUDA_OK(cudaStreamSynchronize(st));
-    std::vector<float> h;
-    for (GNW* g_ : gammas) {
-      h.resize(g_->C);
-      CUDA_OK(cudaMemcpy(h.data(), g_->gamma, (size_t)g_->C * 4, cudaMemcpyDeviceToHost));
-      g_->pos = true;
-      for (float v : h) g_->pos = g_->pos && (v > 0.f);
-    }
   }
 
   // ---- cuDNN convolution -------------------------------------------------------------
@@ -844,27 +798,131 @@ struct dp_engine {
     KERNEL_OK(); ++launches;
   }
 
+  // FusedReduce: the stem dgrad fused with the masked EOT reduce (K1^T) of samples [n0, n0 + N) into G.
+  // Wgrad: the weight-gradient pass of one chunk (dp_eot_backward_params): accumulates d/d(parameter) of the requested
+  // parameters (`want`) into the lane's accumulators.  input: the chunk's network input.  need_dx: the input gradient
+  // is wanted too (else the backward stops at block `lo`, the lowest block whose gradients are wanted).
+  struct FusedReduce { const int16_t* rects; float* G; int B, S, n0; };
+  struct Wgrad { const void* input; bool need_dx; int lo; };
+  struct EotIn;
+
+  // ---- the stem: timm's stem.conv (7x7/2, 3 -> 64), ConstantPad2d(1, 0), MaxPool2d(3, 2) -------------------------
+  // Every choice about the stem is made here, once at create: the network-input layout, the forward, how the backward
+  // ends and the weight gradient.  A variant is an enum value plus its launches in forward / backward.
+  struct Stem {
+    enum Fwd { FWD_OWN, FWD_CUDNN };   // own: bf16 mma.sync kernel on the tight C = 3 input
+    // the backward ends in the library dgrad (K1^T separate), the dgrad fused with K1^T, or that plus the max-pool adjoint
+    enum BwdEnd { END_CUDNN, END_FUSED_REDUCE, END_FUSED_POOL_REDUCE };
+    enum WgradImpl { WG_OWN, WG_CUDNN };   // own: bf16 mma.sync kernel on the tight input
+    static constexpr int SUB = 128;      // samples per cuDNN stem call
+    dp_engine* e = nullptr;
+    ConvW conv;
+    void* w_kn = nullptr;   // FWD_OWN: the standardised weights as the kernel's packed tile
+    int in_ch = 4;          // channels per pixel of the network input (3 = tight, FWD_OWN)
+    int dx_ch = 4;          // channels per pixel of d(input) from the library dgrad, and of the stem filter (4 / 8)
+    Fwd fwd = FWD_CUDNN; BwdEnd bwd = END_CUDNN; WgradImpl wgrad = WG_CUDNN;
+
+    void configure(dp_engine* eng) {
+      e = eng;
+      auto is = [](const char* var, const char* val) { const char* s = getenv(var); return s && strcmp(s, val) == 0; };
+      dx_ch = e->bf16 ? 8 : 4;
+      if (const char* s = getenv("DORPATCH_CPAD")) dx_ch = atoi(s);
+      if (dx_ch != 4 && dx_ch != 8) fail("DORPATCH_CPAD must be 4 or 8");
+      const bool own = e->bf16 && !is("DORPATCH_STEM", "cudnn");
+      fwd = own ? FWD_OWN : FWD_CUDNN;
+      wgrad = own ? WG_OWN : WG_CUDNN;
+      in_ch = own ? 3 : dx_ch;
+      // measured: rebuilding the d_stem patch in shared memory costs more than the saved HBM round trip
+      // (2.25 ms vs 1.33 + 0.71 ms per 512-sample step) -> off unless DORPATCH_POOL_BWD=fused
+      if (!own || is("DORPATCH_STEM_BWD", "cudnn")) bwd = END_CUDNN;
+      else bwd = is("DORPATCH_POOL_BWD", "fused") ? END_FUSED_POOL_REDUCE : END_FUSED_REDUCE;
+    }
+    void allocate() {
+      e->make_conv(conv, 3, STEM_CH, 7, 2, 3, dx_ch);
+      if (fwd == FWD_OWN) w_kn = e->dmalloc((size_t)160 * 64 * 2);
+    }
+    void load(cudaStream_t st) {   // after new raw weights
+      e->standardize(conv, st);
+      if (fwd == FWD_OWN) { dp::launch_stem_pack(conv.w, w_kn, conv.cin_pad, st); KERNEL_OK(); }
+    }
+    // Does the backward of a chunk expanded from `in` end in the fused K1^T (backward() given a FusedReduce)?  The fused
+    // kernels have no affine (warped) variant.
+    bool folds_k1t(const EotIn& in) const { return !in.xf && bwd != END_CUDNN; }
+    // cuDNN's stem kernels degrade badly beyond ~128 samples of 224x224: the library forward, dgrad and filter gradient
+    // run in slices of SUB samples.  f(n, x, y): a slice of x ([N,H,H,x_ch], input side) and of y ([N,H/2,H/2,64]).
+    template <class F>
+    void cudnn_slices(int N, const void* x, int x_ch, const void* y, F f) const {
+      const int H = e->H, hs = e->Hs();
+      for (int n0 = 0; n0 < N; n0 += SUB)
+        f(std::min(SUB, N - n0), (char*)x + (size_t)n0 * H * H * x_ch * e->es, (char*)y + (size_t)n0 * hs * hs * STEM_CH * e->es);
+    }
+    // the own kernels, also behind the op-level test hooks
+    void own_wgrad(const void* input, const void* dY, float* partial, float* acc, int N, int cin_pad, cudaStream_t st) const {
+      dp::launch_stem_wgrad(input, dY, partial, acc, N, e->H, e->H, cin_pad, st); KERNEL_OK(); e->launches += 2;
+    }
+    void fused_reduce(const void* dY, const FusedReduce& fr, int N, cudaStream_t st) const {
+      dp::launch_stem_bwd_reduce(dY, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st); KERNEL_OK(); ++e->launches;
+    }
+    // input [N,H,H,in_ch] -> conv -> max-pool into L.x0 (train: keep the argmax for the backward)
+    void forward(const Lane& L, int N, const void* input, bool train, cudaStream_t st) const {
+      const int H = e->H, hs = e->Hs(), hp = e->Hp();
+      if (fwd == FWD_OWN) {
+        PROF(e, "stem_conv_fwd", ((double)N * H * H * 3 + (double)N * hs * hs * STEM_CH) * e->es, 2.0 * N * hs * hs * STEM_CH * 147, st,
+             dp::launch_stem_forward(input, w_kn, L.act, N, H, H, st));
+        KERNEL_OK(); ++e->launches;
+      } else {
+        cudnn_slices(N, input, in_ch, L.act, [&](int n, char* x, char* y) { e->conv_fwd(L, 0, conv, n, H, hs, x, y, st); });
+      }
+      PROF(e, "maxpool_fwd", (double)N * (hs * hs + hp * hp) * STEM_CH * e->es, 0, st,
+           dp::launch_maxpool_forward(L.act, L.x0, train ? L.pool_amax : nullptr, N, hs, hs, STEM_CH, e->bf16, st)); KERNEL_OK(); ++e->launches;
+    }
+    // d_x0: the gradient at the max-pool output.  Max-pool backward, the stem's weight gradient when wg wants it, then
+    // the dgrad, or the fused reduce when fr is given.  Returns d/d(input) ([N,H,H,dx_ch] in L.g[2]), or null when
+    // nothing of it was produced.
+    void* backward(const Lane& L, int N, const void* d_x0, const FusedReduce* fr, const Wgrad* wg, cudaStream_t st) const {
+      const int H = e->H, hs = e->Hs();
+      void *const GB = L.g[1], *const GC = L.g[2];
+      const bool want_w = wg && e->want_conv(conv);
+      if (wg && !wg->need_dx && !want_w) return nullptr;
+      if (fr && bwd == END_FUSED_POOL_REDUCE && !wg) {
+        // max-pool backward + stem dgrad + masked EOT reduce in one kernel: neither d_stem nor d/d(input) is written
+        PROF(e, "stem_bwd_reduce", (double)N * (hs / 2) * (hs / 2) * STEM_CH * (e->es + 1) + 3.0 * H * H * 4 * (double)N / fr->S,
+             2.0 * N * hs * hs * STEM_CH * 147, st,
+             dp::launch_stem_bwd_pool_reduce(d_x0, L.pool_amax, conv.w, conv.cin_pad, fr->rects, fr->G, fr->B, fr->S, fr->n0, N, H, H, st));
+        KERNEL_OK(); ++e->launches;
+        return nullptr;
+      }
+      PROF(e, "maxpool_bwd", (double)N * (hs * hs + (hs / 2) * (hs / 2)) * STEM_CH * e->es, 0, st,
+           dp::launch_maxpool_backward(d_x0, L.pool_amax, GB, N, hs, hs, STEM_CH, e->bf16, st)); KERNEL_OK(); ++e->launches;
+      if (want_w) {                                                                // dY = the max-pool adjoint (GB)
+        float* const acc = e->acc_of(L, conv.pid);
+        if (wgrad == WG_OWN)
+          PROF(e, "stem_wgrad", (double)N * (H * H * 3 + hs * hs * STEM_CH) * e->es, 2.0 * N * hs * hs * STEM_CH * 147, st,
+               own_wgrad(wg->input, GB, L.wg_partial, acc, N, conv.cin_pad, st));
+        else
+          cudnn_slices(N, wg->input, in_ch, GB, [&](int n, char* x, char* y) { e->conv_wgrad(L, 0, conv, n, H, hs, x, y, acc, st); });
+        if (!wg->need_dx) return nullptr;
+      }
+      if (fr) {
+        PROF(e, "stem_bwd_reduce", (double)N * hs * hs * STEM_CH * e->es + 3.0 * H * H * 4 * (double)N / fr->S,
+             2.0 * N * hs * hs * STEM_CH * 147, st, fused_reduce(GB, *fr, N, st));
+        return nullptr;
+      }
+      cudnn_slices(N, GC, dx_ch, GB, [&](int n, char* x, char* y) { e->conv_bwd(L, 0, conv, n, H, hs, y, x, st); });
+      return GC;
+    }
+  };
+  Stem stem;
+
   // ---- classifier forward ------------------------------------------------------------------
-  // input: [N,H,H,Cp] T.  train: keep what backward needs.  Leaves logits in L.logits.
+  // input: [N,H,H,stem.in_ch] T.  train: keep what backward needs.  Leaves logits in L.logits.
   void forward(const Lane& L, int N, const void* input, bool train, cudaStream_t st) {
     NvtxRange nvtx_("dorpatch.classifier_forward");
     if (!weights_loaded) fail("dp_engine_load_weights has not been called");
     if (N > chunk) fail("forward: N=%d exceeds chunk=%d", N, chunk);
     CUDNN_OK(cudnnSetStream(L.cudnn, st));
     void* const act = L.act;
-    const int hs = Hs(), hp = Hp();
-    if (own_stem) {
-      PROF(this, "stem_conv_fwd", ((double)N * H * H * 3 + (double)N * hs * hs * STEM_CH) * es, 2.0 * N * hs * hs * STEM_CH * 147, st,
-           dp::launch_stem_forward(input, stem_w_kn, act, N, H, H, st));
-      KERNEL_OK(); ++launches;
-    } else {
-      for (int n0 = 0; n0 < N; n0 += STEM_SUB) {   // cuDNN's stem kernels degrade badly beyond ~128 samples of 224x224
-        const int n = std::min(STEM_SUB, N - n0);
-        conv_fwd(L, 0, stem, n, H, hs, (const char*)input + (size_t)n0 * H * H * Cp * es, (char*)act + (size_t)n0 * hs * hs * STEM_CH * es, st);
-      }
-    }
-    PROF(this, "maxpool_fwd", (double)N * (hs * hs + hp * hp) * STEM_CH * es, 0, st,
-         dp::launch_maxpool_forward(act, L.x0, train ? L.pool_amax : nullptr, N, hs, hs, STEM_CH, bf16, st)); KERNEL_OK(); ++launches;
+    stem.forward(L, N, input, train, st);
     const void* cur = L.x0;
     for (size_t bi = 0; bi < blocks.size(); ++bi) {
       const Block& b = blocks[bi];
@@ -926,17 +984,9 @@ struct dp_engine {
   }
 
   // ---- classifier backward (to the input) -----------------------------------------------------
-  // dlog: [N,K] fp32 dev.  Returns d/d(input) ([N,H,H,Cpd] T, in one of the lane's gradient buffers), or null when
-  // nothing of it was produced.
-  // `fused`: non-null -> finish with the fused stem-dgrad + masked EOT reduce into fused->G instead of
-  // producing d/d(input) (bf16 own-stem path; the per-sample input gradient is never materialised).
-  struct FusedReduce { const int16_t* rects; float* G; int B, S, n0; };
-  bool fused_stem_bwd = false;     // set at create: own_stem && DORPATCH_STEM_BWD != "cudnn"
-  bool fused_pool_bwd = false;     // ... && DORPATCH_POOL_BWD == "fused": max-pool backward fused in as well (slower, off)
-  // Weight-gradient pass of one chunk (dp_eot_backward_params): accumulates d/d(parameter) of the requested
-  // parameters (`want`) into the lane's accumulators.  input: the chunk's network input.  need_dx: the
-  // input gradient is wanted too (else the backward stops at block `lo`, the lowest block whose gradients are wanted).
-  struct Wgrad { const void* input; bool need_dx; int lo; };
+  // dlog: [N,K] fp32 dev.  Returns d/d(input) ([N,H,H,stem.dx_ch] T, in one of the lane's gradient buffers), or null
+  // when nothing of it was produced.
+  // `fused`: non-null -> finish with the stem's fused K1^T into fused->G instead (only where stem.folds_k1t).
   void* backward(const Lane& L, int N, const float* dlog, cudaStream_t st, const FusedReduce* fused = nullptr, const Wgrad* wg = nullptr) {
     NvtxRange nvtx_("dorpatch.classifier_backward");
     CUDNN_OK(cudnnSetStream(L.cudnn, st));
@@ -1014,45 +1064,8 @@ struct dp_engine {
       if (W && want_gn(b.n1)) gn_wgrad(L, b.n1, GB, xin, s.st1, N, pin_, st);
       std::swap(GA, GD);
     }
-    const int hs = Hs();
     if (W && lo > 0) return nullptr;                                             // nothing below block lo is wanted
-    if (W && !wg->need_dx && !want_conv(stem)) return nullptr;
-    if (fused != nullptr && fused_pool_bwd && !W) {
-      // max-pool backward + stem dgrad + masked EOT reduce in one kernel: neither d_stem nor d/d(input) is written
-      PROF(this, "stem_bwd_reduce", (double)N * (hs / 2) * (hs / 2) * STEM_CH * (es + 1) + 3.0 * H * H * 4 * (double)N / fused->S,
-           2.0 * N * hs * hs * STEM_CH * 147, st,
-           dp::launch_stem_bwd_pool_reduce(GA, L.pool_amax, stem.w, stem.cin_pad, fused->rects, fused->G, fused->B, fused->S, fused->n0, N, H, H, st));
-      KERNEL_OK(); ++launches;
-      return nullptr;
-    }
-    PROF(this, "maxpool_bwd", (double)N * (hs * hs + (hs / 2) * (hs / 2)) * STEM_CH * es, 0, st,
-         dp::launch_maxpool_backward(GA, L.pool_amax, GB, N, hs, hs, STEM_CH, bf16, st)); KERNEL_OK(); ++launches;
-    if (W && want_conv(stem)) {                                                  // stem: dY = the max-pool adjoint (GB)
-      if (own_stem) {
-        PROF(this, "stem_wgrad", (double)N * (H * H * 3 + hs * hs * STEM_CH) * es, 2.0 * N * hs * hs * STEM_CH * 147, st,
-             dp::launch_stem_wgrad(wg->input, GB, L.wg_partial, acc_of(L, stem.pid), N, H, H, stem.cin_pad, st));
-        KERNEL_OK(); launches += 2;
-      } else {
-        for (int n0 = 0; n0 < N; n0 += STEM_SUB) {
-          const int n = std::min(STEM_SUB, N - n0);
-          conv_wgrad(L, 0, stem, n, H, hs, (const char*)wg->input + (size_t)n0 * H * H * Cp * es, (const char*)GB + (size_t)n0 * hs * hs * STEM_CH * es,
-                     acc_of(L, stem.pid), st);
-        }
-      }
-      if (!wg->need_dx) return nullptr;
-    }
-    if (fused != nullptr) {
-      PROF(this, "stem_bwd_reduce", (double)N * hs * hs * STEM_CH * es + 3.0 * H * H * 4 * (double)N / fused->S,
-           2.0 * N * hs * hs * STEM_CH * 147, st,
-           dp::launch_stem_bwd_reduce(GB, stem.w, stem.cin_pad, fused->rects, fused->G, fused->B, fused->S, fused->n0, N, H, H, st));
-      KERNEL_OK(); ++launches;
-      return nullptr;
-    }
-    for (int n0 = 0; n0 < N; n0 += STEM_SUB) {
-      const int n = std::min(STEM_SUB, N - n0);
-      conv_bwd(L, 0, stem, n, H, hs, (const char*)GB + (size_t)n0 * hs * hs * STEM_CH * es, (char*)GC + (size_t)n0 * H * H * Cpd * es, st);
-    }
-    return GC;
+    return stem.backward(L, N, GA, fused, wg, st);
   }
 
   // ---- EOT input: K1 and its adjoint K1^T for the chunk loops and the dp_expand* entry points ------------------------
@@ -1078,10 +1091,10 @@ struct dp_engine {
     const bool fused = in.x != nullptr;
     const double bytes = (double)n * H * H * 3 * es + (fused ? 7.0 : 3.0) * H * H * 4 * (double)n / in.S;
     if (in.xf)
-      PROF(this, "expand_affine", bytes, 0, st, dp::launch_expand_affine(in.img, in.xf, in.rects, dst, in.S, n0, n, H, H, Cp, bf16, st));
+      PROF(this, "expand_affine", bytes, 0, st, dp::launch_expand_affine(in.img, in.xf, in.rects, dst, in.S, n0, n, H, H, stem.in_ch, bf16, st));
     else
       PROF(this, "expand_k1", bytes, 0, st,
-           dp::launch_expand(in.img, in.x, in.mask, in.pattern, in.scale, in.rects, dst, in.B, in.S, n0, n, H, H, Cp, bf16, fused, num_sms, st));
+           dp::launch_expand(in.img, in.x, in.mask, in.pattern, in.scale, in.rects, dst, in.B, in.S, n0, n, H, H, stem.in_ch, bf16, fused, num_sms, st));
     KERNEL_OK(); ++launches;
   }
   // The network input of samples [n0, n0 + n): their slice of net_in_all when K1 ran once for the whole call, otherwise
@@ -1095,15 +1108,15 @@ struct dp_engine {
   // input is not warped, otherwise the library stem dgrad and then reduce_affine (warped) or reduce.  G null: no input
   // gradient (weight gradients only).
   void backward_reduce(const Lane& L, const EotIn& in, int n0, int n, float* G, cudaStream_t st, const Wgrad* wg = nullptr) {
-    const bool fuse = G && !in.xf && fused_stem_bwd;
+    const bool fuse = G && stem.folds_k1t(in);
     const FusedReduce fr{in.rects, G, in.B, in.S, n0};
     const void* dx = backward(L, n, L.dlogits, st, fuse ? &fr : nullptr, wg);
     if (!G || fuse) return;
     const double bytes = (double)n * H * H * 3 * es + 3.0 * H * H * 4 * (double)n / in.S;
     if (in.xf)
-      PROF(this, "reduce_affine", bytes, 0, st, dp::launch_reduce_affine(dx, in.img, in.xf, in.rects, G, in.S, n0, n, H, H, Cpd, bf16, st));
+      PROF(this, "reduce_affine", bytes, 0, st, dp::launch_reduce_affine(dx, in.img, in.xf, in.rects, G, in.S, n0, n, H, H, stem.dx_ch, bf16, st));
     else
-      PROF(this, "reduce_k1t", bytes, 0, st, dp::launch_reduce(dx, in.rects, G, in.B, in.S, n0, n, H, H, Cpd, bf16, st));
+      PROF(this, "reduce_k1t", bytes, 0, st, dp::launch_reduce(dx, in.rects, G, in.B, in.S, n0, n, H, H, stem.dx_ch, bf16, st));
     KERNEL_OK(); ++launches;
   }
 
@@ -1200,22 +1213,11 @@ int32_t dp_engine_create(const dp_config* cfg, dp_engine** out) {
     e->num_sms = prop.multiProcessorCount;
     e->bf16 = (cfg->precision == DP_PREC_BF16);
     e->es = e->bf16 ? 2 : 4;
-    e->Cpd = e->bf16 ? 8 : 4;
-    if (const char* s = getenv("DORPATCH_CPAD")) e->Cpd = atoi(s);
-    if (e->Cpd != 4 && e->Cpd != 8) fail("DORPATCH_CPAD must be 4 or 8");
-    const char* stem_env = getenv("DORPATCH_STEM");
-    e->own_stem = e->bf16 && !(stem_env && strcmp(stem_env, "cudnn") == 0);
-    e->Cp = e->own_stem ? 3 : e->Cpd;
-    const char* sb_env = getenv("DORPATCH_STEM_BWD");
-    e->fused_stem_bwd = e->own_stem && !(sb_env && strcmp(sb_env, "cudnn") == 0);
+    e->stem.configure(e);
     const char* fg_env = getenv("DORPATCH_FUSED_GEMM");
     e->fused_gemm = e->bf16 && fg_env && atoi(fg_env) != 0;   // validated (tests/test_gpu_ops.py, test_gpu_fused_gemm.py) but slower than cublasLt + GroupNorm: off unless asked for
     if (const char* g_env = getenv("DORPATCH_GRAPH")) e->graphs_on = atoi(g_env) != 0;
     if (const char* k_env = getenv("DORPATCH_K1_WHOLE_MB")) e->k1_whole_max = (size_t)std::max(0, atoi(k_env)) << 20;
-    const char* pb_env = getenv("DORPATCH_POOL_BWD");
-    // measured: rebuilding the d_stem patch in shared memory costs more than the saved HBM round trip
-    // (2.25 ms vs 1.33 + 0.71 ms per 512-sample step) -> off unless DORPATCH_POOL_BWD=fused
-    e->fused_pool_bwd = e->fused_stem_bwd && (pb_env && strcmp(pb_env, "fused") == 0);
     e->H = cfg->img; e->K = cfg->n_classes; e->chunk = cfg->chunk;
     e->cudnn_dt = e->bf16 ? CUDNN_DATA_BFLOAT16 : CUDNN_DATA_FLOAT;
     e->cuda_dt = e->bf16 ? CUDA_R_16BF : CUDA_R_32F;
@@ -1255,7 +1257,7 @@ void dp_engine_destroy(dp_engine* e) {
     if (c.wdesc) cudnnDestroyFilterDescriptor(c.wdesc);
     if (c.cdesc) cudnnDestroyConvolutionDescriptor(c.cdesc);
   };
-  kill(e->stem);
+  kill(e->stem.conv);
   for (auto& b : e->blocks) { kill(b.ds); kill(b.c1); kill(b.c2); kill(b.c3); }
   e->drop_graphs();
   for (auto& r : e->prof_recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
@@ -1327,7 +1329,7 @@ int32_t dp_engine_profile_read(dp_engine* e, int32_t max_n, char* names, int32_t
 int32_t dp_input_layout(const dp_engine* e, int32_t* c_pad, int32_t* elem_bytes) {
   DP_TRY
   if (!e) fail("null engine");
-  if (c_pad) *c_pad = e->Cp;
+  if (c_pad) *c_pad = e->stem.in_ch;
   if (elem_bytes) *elem_bytes = (int32_t)e->es;
   DP_CATCH
 }
@@ -1715,7 +1717,7 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
       const auto sp = e->wspan(i);
       lo_off = std::min(lo_off, sp.first); hi_off = std::max(hi_off, sp.second);
     }
-    if (want[e->stem.pid]) wg.lo = 0;
+    if (want[e->stem.conv.pid]) wg.lo = 0;
     for (int bi = (int)e->blocks.size() - 1; bi >= 0; --bi) {
       const Block& b = e->blocks[bi];
       if (e->want_conv(b.c1) || e->want_conv(b.c2) || e->want_conv(b.c3) || (b.has_ds && e->want_conv(b.ds)) ||
@@ -1831,13 +1833,13 @@ int32_t dp_net_forward_backward(dp_engine* e, const float* z, int32_t N, float* 
   if (N < 1 || N > e->chunk) fail("N=%d outside [1, chunk=%d]", N, e->chunk);
   e->forward_clobbered();
   const dp_engine::Lane& L = e->lanes[0];
-  dp::launch_pack_nchw(z, L.net_in, N, e->H, e->H, e->Cp, e->bf16, st); KERNEL_OK(); ++e->launches;
+  dp::launch_pack_nchw(z, L.net_in, N, e->H, e->H, e->stem.in_ch, e->bf16, st); KERNEL_OK(); ++e->launches;
   e->forward(L, N, L.net_in, dlogits_dev != nullptr, st);
   if (logits_dev) CUDA_OK(cudaMemcpyAsync(logits_dev, L.logits, (size_t)N * e->K * 4, cudaMemcpyDeviceToDevice, st));
   if (dlogits_dev) {
     if (!dz_dev) fail("dz_dev is required when dlogits_dev is given");
     const void* dx = e->backward(L, N, dlogits_dev, st);
-    dp::launch_unpack_nhwc(dx, dz_dev, N, e->H, e->H, e->Cpd, e->bf16, st); KERNEL_OK(); ++e->launches;
+    dp::launch_unpack_nhwc(dx, dz_dev, N, e->H, e->H, e->stem.dx_ch, e->bf16, st); KERNEL_OK(); ++e->launches;
   }
   DP_CATCH
 }
@@ -1937,14 +1939,13 @@ int32_t dp_debug_stem_bwd_reduce(dp_engine* e, const void* dY, const int16_t* re
                                  void* stream) {
   DP_TRY
   if (!e) fail("null engine");
-  if (!e->own_stem) fail("dp_debug_stem_bwd_reduce: the fused stem backward exists for the bf16 engine only");
+  if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_bwd_reduce: the fused stem backward exists for the bf16 engine only");
   CUDA_OK(cudaSetDevice(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   const int N = B * S;
   e->h2d_samples(rects_host, N, st);
   CUDA_OK(cudaMemsetAsync(G, 0, (size_t)B * 3 * e->H * e->H * 4, st));
-  dp::launch_stem_bwd_reduce(dY, e->stem.w, e->stem.cin_pad, rects_host ? e->rects_d : nullptr, G, B, S, 0, N, e->H, e->H, st);
-  KERNEL_OK(); ++e->launches;
+  e->stem.fused_reduce(dY, dp_engine::FusedReduce{rects_host ? e->rects_d : nullptr, G, B, S, 0}, N, st);
   DP_CATCH
 }
 
@@ -1956,8 +1957,7 @@ int32_t dp_debug_stem_wgrad(dp_engine* e, const void* in, const void* dY, int32_
   cudaStream_t st = (cudaStream_t)stream;
   e->ensure_wgrad_buffers();
   CUDA_OK(cudaMemsetAsync(dW, 0, (size_t)STEM_CH * 49 * 3 * 4, st));
-  dp::launch_stem_wgrad(in, dY, e->lanes[0].wg_partial, dW, N, e->H, e->H, 3, st);
-  KERNEL_OK(); e->launches += 2;
+  e->stem.own_wgrad(in, dY, e->lanes[0].wg_partial, dW, N, 3, st);
   DP_CATCH
 }
 

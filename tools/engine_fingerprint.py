@@ -10,6 +10,9 @@ the DORPATCH_* variants that change which launches those loops issue.  Two shape
 chunk: two lanes everywhere) and B = 2 x S = 5 (images straddle chunks: one lane for dp_attack_grad and
 dp_eot_backward).  Per call it records the launch-count delta, the graph-replay counter and the SHA-256 of every
 output; a second pass with the engine profiler on (one lane by design) records category -> count, bytes and flops.
+The last call reloads a few weights from the device (dp_engine_load_weights_dev: re-standardised convolutions, re-packed
+own-stem and fused-GEMM tiles, a GroupNorm whose gamma > 0 flag flips), runs predict / eot_forward / a full parameter
+backward on them, and restores the original weights.
 Gradients summed with fp32 atomics (the affine / colour EOT adjoint) are not bit-reproducible: they are saved
 next to the JSON and compared within the relative L2 bound of tests/test_gpu_eot_xform.py.
 """
@@ -39,7 +42,18 @@ VARIANTS = [  # (name, environment, precisions)
     ("k1whole0", {"DORPATCH_K1_WHOLE_MB": "0"}, ("fp32", "tf32", "bf16")),
     ("stembwd_cudnn", {"DORPATCH_STEM_BWD": "cudnn"}, ("bf16",)),   # the fused stem backward exists at bf16 only
     ("fused_gemm", {"DORPATCH_FUSED_GEMM": "1"}, ("bf16",)),       # bf16 only
+    ("stem_cudnn", {"DORPATCH_STEM": "cudnn"}, ("bf16",)),          # the library stem at bf16 (padded input)
+    ("pool_bwd_fused", {"DORPATCH_POOL_BWD": "fused"}, ("bf16",)),
+    ("cpad4", {"DORPATCH_CPAD": "4"}, ("bf16",)),
+    ("cpad8", {"DORPATCH_CPAD": "8"}, ("fp32", "tf32")),
 ]
+RELOAD = {  # the "reload" call's changes: name -> new tensor from the original
+    "stem.conv.weight": lambda t: t * 1.01,
+    "stages.0.blocks.1.conv1.weight": lambda t: t * 1.01,   # no downsample branch: the fused GEMM's operand
+    "stages.2.blocks.1.conv2.weight": lambda t: t * 1.01,
+    "stages.1.blocks.0.norm2.weight": lambda t: t * t.new_tensor([-1.0] + [1.0] * (t.numel() - 1)),   # gamma > 0 flag flips
+    "head.fc.bias": lambda t: t + t.new_tensor(np.linspace(-0.1, 0.1, t.numel(), dtype=np.float32)),
+}
 
 
 def _sha(t):
@@ -52,7 +66,7 @@ def _sha(t):
     return hashlib.sha256(np.ascontiguousarray(t).tobytes()).hexdigest()
 
 
-def _calls(e, B, S):
+def _calls(e, B, S, weights):
     """[(name, fn)]: fn() returns {output name: tensor / array}; names ending in '~' are compared within a tolerance."""
     import torch
     from dorpatch_b200 import eot as PE, masks as PM
@@ -109,6 +123,16 @@ def _calls(e, B, S):
         assert rc == 0, e.lib.dp_last_error()
         return {"out": out_in.clone()}
 
+    def reload():
+        e.load_state_dict_dev({n: f(weights[n].clone()).cuda() for n, f in RELOAD.items()})
+        try:
+            out = dict(zip(("preds", "logits"), e.predict(img, S, rects, return_logits=True)))
+            out["eot_logits"] = eot_fwd()["logits"]
+            out.update(params(list(shapes), True))
+        finally:
+            e.load_state_dict_dev({n: weights[n].cuda() for n in RELOAD})
+        return out
+
     calls = [("predict", lambda: dict(zip(("preds", "logits"), e.predict(img, S, rects, return_logits=True))))]
     for stage in (0, 1):
         calls += [("attack_s%d_%d" % (stage, i), lambda stage=stage: attack(stage)) for i in range(4)]
@@ -128,6 +152,7 @@ def _calls(e, B, S):
         ("params_head_img", lambda: params(HEAD, True)),
         ("params_head", lambda: params(HEAD, None)),
         ("net_forward_backward", lambda: dict(zip(("logits", "dz"), e.net_forward_backward(z, dz_logits)))),
+        ("reload", reload),
     ]
     return calls
 
@@ -158,7 +183,7 @@ def run(lib_path, out_path):
                 for prof in (False, True):
                     key = "%s/%s/B%dS%d%s" % (vname, prec, B, S, "/prof" if prof else "")
                     rec = result[key] = {}
-                    for name, fn in _calls(e, B, S):
+                    for name, fn in _calls(e, B, S, params):
                         if prof:
                             e.profile(True, reset=True)
                         l0 = e.launch_count
