@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "kernels.h"
+
 namespace dp {
 
 // ----------------------------------------------------------------------------
@@ -70,5 +72,72 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
 }
 
 __device__ __forceinline__ float sgn(float v) { return (float)(v > 0.f) - (float)(v < 0.f); }  // sgn(NaN) = 0, as torch.sign
+
+// ----------------------------------------------------------------------------
+// EOT samples are image-major: sample s belongs to image s / S.  A launch over samples [n0, n0 + n) touches
+// images_touched() images; its i-th image is b, whose samples in the launch are [lo, hi).  first: lo is b's first
+// sample, so the launch writes b's result rather than adding to it.
+// ----------------------------------------------------------------------------
+__host__ __device__ __forceinline__ int images_touched(int S, int n0, int n) {
+  const int first = n0 / S, last = (n0 + n - 1) / S;
+  return last - first + 1;
+}
+struct ImageSpan {
+  int b, lo, hi;
+  bool first;
+};
+__device__ __forceinline__ ImageSpan image_span(int S, int n0, int n, int i) {
+  const int b = n0 / S + i;
+  const int lo = max(n0, b * S), hi = min(n0 + n, (b + 1) * S);
+  return ImageSpan{b, lo, hi, lo == b * S};
+}
+
+// ----------------------------------------------------------------------------
+// Occlusion table: the only place its format is decoded.  A sample's row is RECT_SHORTS int16, four rectangles
+// {r0, r1, c0, c1}: rectangle k occludes rows [r0, r1) x columns [c0, c1) (half-open), and is empty when r1 <= r0 or
+// c1 <= c0 (unused slots are all zero).  A pixel is occluded when any rectangle covers it.  A row is 32 bytes: two
+// 16-byte words.
+// ----------------------------------------------------------------------------
+namespace occl {
+struct Words { int4 q0, q1; };   // one sample's row as read
+// sample n's row as two 16-byte words (also for a block-wide copy into shared memory)
+__device__ __forceinline__ const int4* row(const int16_t* rects, int n) {
+  return reinterpret_cast<const int4*>(rects + (size_t)n * RECT_SHORTS);
+}
+// from the table in global memory (the same address in every lane of a warp is a broadcast)
+__device__ __forceinline__ Words load(const int16_t* rects, int n) {
+  const int4* p = row(rects, n);
+  return Words{__ldg(p), __ldg(p + 1)};
+}
+// from a copy of row() in shared memory
+__device__ __forceinline__ Words load_shared(const int4* s) { return Words{s[0], s[1]}; }
+// r: one sample's row, in registers or shared memory
+__device__ __forceinline__ bool hit(const short* r, int row, int col) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (row >= r[4 * k] && row < r[4 * k + 1] && col >= r[4 * k + 2] && col < r[4 * k + 3]) return true;
+  return false;
+}
+}  // namespace occl
+
+// one sample's rectangles in registers
+struct Occlusion {
+  short r[RECT_SHORTS];
+  Occlusion() = default;
+  __device__ __forceinline__ explicit Occlusion(occl::Words w) { set(w); }
+  __device__ __forceinline__ void set(occl::Words w) {
+    *reinterpret_cast<int4*>(r) = w.q0;
+    *reinterpret_cast<int4*>(r + 8) = w.q1;
+  }
+  __device__ __forceinline__ bool hit(int row, int col) const { return occl::hit(r, row, col); }
+  // Rectangle k as the rows [rlo, rhi) it covers and, in a row of `cp` elements per pixel, the elements [elo, ehi).
+  // A rectangle with no columns covers no row (rlo = rhi = 0); one with no rows has rhi <= rlo.
+  __device__ __forceinline__ void span(int k, int cp, int& rlo, int& rhi, int& elo, int& ehi) const {
+    const int* w = reinterpret_cast<const int*>(r);   // {r0, r1} and {c0, c1}, each one 32-bit word (r0, c0 low)
+    rlo = (short)(w[2 * k] & 0xffff); rhi = (short)(w[2 * k] >> 16);
+    elo = (short)(w[2 * k + 1] & 0xffff) * cp; ehi = (short)(w[2 * k + 1] >> 16) * cp;
+    if (ehi <= elo) { rlo = 0; rhi = 0; }
+  }
+};
 
 }  // namespace dp

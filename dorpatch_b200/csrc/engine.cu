@@ -292,7 +292,7 @@ struct dp_engine {
     drop_graphs();                       // captured launches hold the old per-sample buffers
     // (old buffers stay in `allocs` and are released at destroy)
     cap_samples = std::max(n, cap_samples * 2);
-    rects_d = (int16_t*)dmalloc((size_t)cap_samples * 16 * sizeof(int16_t));
+    rects_d = (int16_t*)dmalloc((size_t)cap_samples * dp::RECT_SHORTS * sizeof(int16_t));
     y_d = (int32_t*)dmalloc((size_t)cap_samples * sizeof(int32_t));
     tg_d = (uint8_t*)dmalloc((size_t)cap_samples);
     loss_d = (float*)dmalloc((size_t)cap_samples * sizeof(float));
@@ -1137,7 +1137,7 @@ struct dp_engine {
   }
   void h2d_samples(const int16_t* rects_host, int N, cudaStream_t st) {
     ensure_samples(N);                   // every per-sample buffer holds N rows: rects_d does not grow on its own
-    if (rects_host != nullptr) stage(rects_d, cap_samples, rects_host, N, 16 * sizeof(int16_t), st);
+    if (rects_host != nullptr) stage(rects_d, cap_samples, rects_host, N, dp::RECT_SHORTS * sizeof(int16_t), st);
   }
   void check_B(int B) const {
     if (B < 1 || B > cfg.max_images) fail("B=%d outside [1, max_images=%d]", B, cfg.max_images);
@@ -1504,7 +1504,7 @@ static void attack_grad_impl(dp_engine* e, const dp_attack_args* a, cudaStream_t
   // per-sample labels / criterion flags / rectangles -> pinned staging.  Layout:
   // [H2D region: ys | tg | rects | xforms][D2H region: results]; the regions never overlap.
   GradLayout L_;
-  L_.rect_bytes = a->rects_host ? (size_t)N * 16 * sizeof(int16_t) : 0;
+  L_.rect_bytes = a->rects_host ? (size_t)N * dp::RECT_SHORTS * sizeof(int16_t) : 0;
   L_.xf_bytes = a->xform_host ? (size_t)N * 8 * sizeof(float) : 0;
   const size_t h2d_bytes = (((size_t)N * 5 + 15) / 16) * 16 + L_.rect_bytes + L_.xf_bytes;
   L_.d2h_off = (h2d_bytes + 255) / 256 * 256;
@@ -1651,7 +1651,7 @@ static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const
              (double)xf_host[i], (int)(i % 8));
   e->forward_clobbered();
   e->eot = dp_engine::EotSig{};
-  if (rects_host) e->stage(e->eot_rects_d, e->eot_rects_cap, rects_host, N, 16 * sizeof(int16_t), st);
+  if (rects_host) e->stage(e->eot_rects_d, e->eot_rects_cap, rects_host, N, dp::RECT_SHORTS * sizeof(int16_t), st);
   if (xf_host) e->stage(e->eot_xf_d, e->eot_xf_cap, xf_host, N, 8 * sizeof(float), st);
   const dp_engine::EotIn in = dp_engine::EotIn::image(img, xf_host ? e->eot_xf_d : nullptr, rects_host ? e->eot_rects_d : nullptr, B, S);
   const bool whole = !xf_host && e->ensure_net_in_all(N);

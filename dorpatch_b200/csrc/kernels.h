@@ -12,6 +12,8 @@ constexpr int GN_MAX_SPLITS = 16;
 // per-sample backward means, the work / done / ready counters; also covers the two-pass kernels' split partials)
 constexpr int GN_WS_FLOATS_PER_SAMPLE = 8192;
 constexpr int GN_WS_FLOATS_EXTRA = 4096;
+// int16 per sample of an occlusion table `rects` [N][RECT_SHORTS]: four rectangles {r0, r1, c0, c1} (common.cuh decodes them)
+constexpr int RECT_SHORTS = 16;
 
 // ---- classifier-side kernels (kernels_net.cu) --------------------------------------
 // timm StdConv2d standardisation of OIHW fp32 weights -> KRSC (NHWC filter), channel-padded.

@@ -10,6 +10,7 @@
 //   update   K3: attack.py:332-342                          chain rule through clip + sign step + clip
 // (file:line into the reference).  Images are NCHW fp32; network input is NHWC(Cp) T.
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -109,13 +110,6 @@ constexpr int EXP_WARPS = EXP_THREADS / 32;
 constexpr int EXP_HDR = 512 + 2048;   // mbarrier + per-item rectangle cache (64 samples x 32 B)
 constexpr int EXP_RCACHE = 64;
 
-__device__ __forceinline__ bool rect_hit(const short* r, int row, int col) {
-#pragma unroll
-  for (int k = 0; k < 4; ++k)
-    if (row >= r[4 * k] && row < r[4 * k + 1] && col >= r[4 * k + 2] && col < r[4 * k + 3]) return true;
-  return false;
-}
-
 struct ExpandParams {
   const float* img; const float* x; const float* mask; const float* pattern; const float* scale;
   const int16_t* rects; void* out;
@@ -151,16 +145,14 @@ __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(ExpandParams p) {
   if (threadIdx.x == 0) { ptx::mbar_init(bar, 1); ptx::fence_mbar_init(); ptx::fence_proxy_async(); }
   __syncthreads();
 
-  const int b_first = p.n0 / p.S, b_last = (p.n0 + p.n - 1) / p.S;
   const int tiles = H / EXP_R;
-  const int items = (b_last - b_first + 1) * tiles * p.sgroups;
+  const int items = images_touched(p.S, p.n0, p.n) * tiles * p.sgroups;
   uint32_t phase = 0;
 
   for (int item = blockIdx.x; item < items; item += gridDim.x) {
     const int sg = item % p.sgroups;
     const int tile = (item / p.sgroups) % tiles;
-    const int b = b_first + item / (p.sgroups * tiles);
-    const int lo = max(p.n0, b * p.S), hi = min(p.n0 + p.n, (b + 1) * p.S);
+    const auto [b, lo, hi, first] = image_span(p.S, p.n0, p.n, item / (p.sgroups * tiles));
     const int cnt = hi - lo;
     const int s_lo = lo + (int)(((long long)cnt * sg) / p.sgroups), s_hi = lo + (int)(((long long)cnt * (sg + 1)) / p.sgroups);
     if (s_lo >= s_hi) continue;   // uniform across the CTA
@@ -182,7 +174,7 @@ __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(ExpandParams p) {
     const bool cached = p.rects != nullptr && (s_hi - s_lo) <= EXP_RCACHE;
     if (cached)
       for (int i = threadIdx.x; i < 2 * (s_hi - s_lo); i += EXP_THREADS)
-        srect[i] = __ldg(reinterpret_cast<const int4*>(p.rects + (size_t)s_lo * 16) + i);
+        srect[i] = __ldg(occl::row(p.rects, s_lo) + i);
     ptx::mbar_wait(bar, phase);
     phase ^= 1u;
 
@@ -211,18 +203,10 @@ __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(ExpandParams p) {
       int rr0[4], rr1[4], el[4], eh[4];
       bool any = false;
       if (p.rects != nullptr) {
-        int4 q0, q1;
-        if (cached) { q0 = srect[2 * (n - s_lo)]; q1 = srect[2 * (n - s_lo) + 1]; }
-        else {
-          const int4* rp = reinterpret_cast<const int4*>(p.rects + (size_t)n * 16);
-          q0 = __ldg(rp); q1 = __ldg(rp + 1);                 // same address in every lane: broadcast
-        }
-        const int w[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
+        const Occlusion occ(cached ? occl::load_shared(srect + 2 * (n - s_lo)) : occl::load(p.rects, n));
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          rr0[k] = (short)(w[2 * k] & 0xffff); rr1[k] = (short)(w[2 * k] >> 16);
-          el[k] = (short)(w[2 * k + 1] & 0xffff) * CP; eh[k] = (short)(w[2 * k + 1] >> 16) * CP;
-          if (eh[k] <= el[k]) { rr0[k] = 0; rr1[k] = 0; }      // empty rectangle
+          occ.span(k, CP, rr0[k], rr1[k], el[k], eh[k]);
           any = any || (rr0[k] < r0 + EXP_R && rr1[k] > r0);
         }
       }
@@ -336,7 +320,7 @@ static void expand_launch(const ExpandParams& p, int num_sms, cudaStream_t st) {
     }
     return occ_cache[R];
   };
-  const int nb_img = (p.n0 + p.n - 1) / p.S - p.n0 / p.S + 1;
+  const int nb_img = images_touched(p.S, p.n0, p.n);
   auto usable = [&](int R) { return R >= 1 && R <= 32 && p.H % R == 0 && smem_of(R) <= 200 * 1024; };
   int best_R = 0, best_sg = 1;
   if (rows_env > 0 && usable(rows_env)) best_R = rows_env;
@@ -362,23 +346,27 @@ static void expand_launch(const ExpandParams& p, int num_sms, cudaStream_t st) {
   expand_kernel<T, CP, FUSED><<<best_grid, EXP_THREADS, smem, st>>>(q);
 }
 
+// f(T{}, integral_constant<int, CP>{}) for an activation type and channels per pixel, Cp in {3, 4, 8} (the engine
+// checks Cp when it is created)
+template <class F>
+static void dispatch_t_cp(bool bf16, int Cp, F&& f) {
+  auto by_cp = [&](auto t) {
+    if (Cp == 8) f(t, std::integral_constant<int, 8>{});
+    else if (Cp == 4) f(t, std::integral_constant<int, 4>{});
+    else f(t, std::integral_constant<int, 3>{});
+  };
+  if (bf16) by_cp(__nv_bfloat16{});
+  else by_cp(0.f);
+}
+
 void launch_expand(const float* img, const float* x, const float* mask, const float* pattern, const float* scale,
                    const int16_t* rects, void* out, int B, int S, int n0, int n, int H, int W, int Cp, bool bf16,
                    bool fused, int num_sms, cudaStream_t st) {
   ExpandParams p{img, x, mask, pattern, scale, rects, out, B, S, n0, n, H, W, 1, EXP_R_DEFAULT, 0};
-#define EXP_CASE(TT, CPV)                                                   \
-  if (fused) expand_launch<TT, CPV, true>(p, num_sms, st);                 \
-  else expand_launch<TT, CPV, false>(p, num_sms, st)
-  if (bf16) {
-    if (Cp == 8) { EXP_CASE(__nv_bfloat16, 8); }
-    else if (Cp == 4) { EXP_CASE(__nv_bfloat16, 4); }
-    else { EXP_CASE(__nv_bfloat16, 3); }
-  } else {
-    if (Cp == 4) { EXP_CASE(float, 4); }
-    else if (Cp == 8) { EXP_CASE(float, 8); }
-    else { EXP_CASE(float, 3); }
-  }
-#undef EXP_CASE
+  dispatch_t_cp(bf16, Cp, [&](auto t, auto cp) {
+    if (fused) expand_launch<decltype(t), cp, true>(p, num_sms, st);
+    else expand_launch<decltype(t), cp, false>(p, num_sms, st);
+  });
 }
 
 // =====================================================================================
@@ -416,13 +404,7 @@ __global__ void __launch_bounds__(256) expand_affine_kernel(const float* __restr
   const int h = px / W, w = px % W;
   const float* t = xf + (size_t)n * 8;
   const AffTap a = affine_taps(t, h, w, H, W);
-  bool occ = false;
-  if (rects != nullptr) {
-    short r[16];
-    const int4* rp = reinterpret_cast<const int4*>(rects + (size_t)n * 16);
-    *reinterpret_cast<int4*>(r) = __ldg(rp); *reinterpret_cast<int4*>(r + 8) = __ldg(rp + 1);
-    occ = rect_hit(r, h, w);
-  }
+  const bool occ = rects != nullptr && Occlusion(occl::load(rects, n)).hit(h, w);
   T* o = out + ((size_t)blockIdx.y * HW + px) * CP;
 #pragma unroll
   for (int c = 0; c < CP; ++c) {
@@ -446,12 +428,7 @@ __global__ void __launch_bounds__(256) reduce_affine_kernel(const T* __restrict_
   const int px = blockIdx.x * blockDim.x + threadIdx.x;
   if (px >= HW) return;
   const int h = px / W, w = px % W;
-  if (rects != nullptr) {
-    short r[16];
-    const int4* rp = reinterpret_cast<const int4*>(rects + (size_t)n * 16);
-    *reinterpret_cast<int4*>(r) = __ldg(rp); *reinterpret_cast<int4*>(r + 8) = __ldg(rp + 1);
-    if (rect_hit(r, h, w)) return;
-  }
+  if (rects != nullptr && Occlusion(occl::load(rects, n)).hit(h, w)) return;
   const float* t = xf + (size_t)n * 8;
   const AffTap a = affine_taps(t, h, w, H, W);
   const T* q = dz + ((size_t)blockIdx.y * HW + px) * CP;
@@ -473,18 +450,18 @@ __global__ void __launch_bounds__(256) reduce_affine_kernel(const T* __restrict_
 void launch_expand_affine(const float* adv, const float* xf, const int16_t* rects, void* out, int S, int n0, int n,
                           int H, int W, int Cp, bool bf16, cudaStream_t st) {
   dim3 grid((H * W + 255) / 256, n);
-#define EA(TT, CPV) expand_affine_kernel<TT, CPV><<<grid, 256, 0, st>>>(adv, xf, rects, (TT*)out, S, n0, H, W)
-  if (bf16) { if (Cp == 3) EA(__nv_bfloat16, 3); else if (Cp == 4) EA(__nv_bfloat16, 4); else EA(__nv_bfloat16, 8); }
-  else { if (Cp == 3) EA(float, 3); else if (Cp == 4) EA(float, 4); else EA(float, 8); }
-#undef EA
+  dispatch_t_cp(bf16, Cp, [&](auto t, auto cp) {
+    using T = decltype(t);
+    expand_affine_kernel<T, cp><<<grid, 256, 0, st>>>(adv, xf, rects, (T*)out, S, n0, H, W);
+  });
 }
 void launch_reduce_affine(const void* dz, const float* adv, const float* xf, const int16_t* rects, float* G, int S, int n0,
                           int n, int H, int W, int Cp, bool bf16, cudaStream_t st) {
   dim3 grid((H * W + 255) / 256, n);
-#define RA(TT, CPV) reduce_affine_kernel<TT, CPV><<<grid, 256, 0, st>>>((const TT*)dz, adv, xf, rects, G, S, n0, H, W)
-  if (bf16) { if (Cp == 4) RA(__nv_bfloat16, 4); else if (Cp == 3) RA(__nv_bfloat16, 3); else RA(__nv_bfloat16, 8); }
-  else { if (Cp == 4) RA(float, 4); else if (Cp == 3) RA(float, 3); else RA(float, 8); }
-#undef RA
+  dispatch_t_cp(bf16, Cp, [&](auto t, auto cp) {
+    using T = decltype(t);
+    reduce_affine_kernel<T, cp><<<grid, 256, 0, st>>>((const T*)dz, adv, xf, rects, G, S, n0, H, W);
+  });
 }
 
 // =====================================================================================
@@ -548,21 +525,21 @@ constexpr int RED_MAXS = 128;
 template <typename T, int CP>
 __global__ void __launch_bounds__(256) reduce_kernel(const T* __restrict__ dz, const int16_t* __restrict__ rects,
                                                      float* __restrict__ G, int S, int n0, int n, int H, int W) {
-  __shared__ __align__(16) short sr[RED_MAXS * 16];
+  __shared__ __align__(16) short sr[RED_MAXS * RECT_SHORTS];   // the rows of up to RED_MAXS samples
   const int HW = H * W;
-  const int b = n0 / S + blockIdx.y;
-  const int lo = max(n0, b * S), hi = min(n0 + n, (b + 1) * S);
+  const auto [b, lo, hi, first] = image_span(S, n0, n, blockIdx.y);
   const int px = blockIdx.x * blockDim.x + threadIdx.x;
   const int row = px / W, col = px % W;
   float acc[3] = {0.f, 0.f, 0.f};
   for (int base = lo; base < hi; base += RED_MAXS) {
     const int m = min(RED_MAXS, hi - base);
     __syncthreads();
-    for (int i = threadIdx.x; i < m * 16; i += blockDim.x) sr[i] = rects != nullptr ? rects[(size_t)base * 16 + i] : (short)0;
+    for (int i = threadIdx.x; i < m * RECT_SHORTS; i += blockDim.x)
+      sr[i] = rects != nullptr ? rects[(size_t)base * RECT_SHORTS + i] : (short)0;
     __syncthreads();
     if (px < HW) {
       for (int j = 0; j < m; ++j) {
-        if (rect_hit(sr + j * 16, row, col)) continue;
+        if (occl::hit(sr + j * RECT_SHORTS, row, col)) continue;
         const T* q = dz + ((size_t)(base + j - n0) * HW + px) * CP;
         if (CP * sizeof(T) == 16) {
           Vec<T> v; v.load(q);
@@ -575,7 +552,6 @@ __global__ void __launch_bounds__(256) reduce_kernel(const T* __restrict__ dz, c
     }
   }
   if (px < HW) {
-    const bool first = (lo == b * S);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       float* g = G + ((size_t)b * 3 + c) * HW + px;
@@ -586,12 +562,11 @@ __global__ void __launch_bounds__(256) reduce_kernel(const T* __restrict__ dz, c
 }
 void launch_reduce(const void* dz, const int16_t* rects, float* G, int B, int S, int n0, int n, int H, int W,
                    int Cp, bool bf16, cudaStream_t st) {
-  const int nb = (n0 + n - 1) / S - n0 / S + 1;
-  dim3 grid((H * W + 255) / 256, nb);
-#define RED_CASE(TT, CPV) reduce_kernel<TT, CPV><<<grid, 256, 0, st>>>((const TT*)dz, rects, G, S, n0, n, H, W)
-  if (bf16) { if (Cp == 8) RED_CASE(__nv_bfloat16, 8); else if (Cp == 4) RED_CASE(__nv_bfloat16, 4); else RED_CASE(__nv_bfloat16, 3); }
-  else { if (Cp == 4) RED_CASE(float, 4); else if (Cp == 8) RED_CASE(float, 8); else RED_CASE(float, 3); }
-#undef RED_CASE
+  const dim3 grid((H * W + 255) / 256, images_touched(S, n0, n));
+  dispatch_t_cp(bf16, Cp, [&](auto t, auto cp) {
+    using T = decltype(t);
+    reduce_kernel<T, cp><<<grid, 256, 0, st>>>((const T*)dz, rects, G, S, n0, n, H, W);
+  });
 }
 
 // =====================================================================================

@@ -11,6 +11,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "common.cuh"
 #include "kernels.h"
 
 namespace dp {
@@ -148,7 +149,6 @@ constexpr int THREADS = 256;
 constexpr int ALLTAPS = 49;                      // 9 + 12 + 12 + 16 taps of the four parity classes
 constexpr size_t W_BYTES = (size_t)ALLTAPS * 64 * 16;
 constexpr size_t PATCH_BYTES = (size_t)PR * PC * PIX;
-constexpr size_t SMEM = W_BYTES + 2 * PATCH_BYTES;
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   const uint32_t a = (uint32_t)__cvta_generic_to_shared(smem_dst);
@@ -160,33 +160,128 @@ __device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, co
   const uint32_t a = (uint32_t)__cvta_generic_to_shared(p);
   asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(a));
 }
-__device__ __forceinline__ bool rect_hit(const short* r, int row, int col) {
+
+// The CTA's tile: positions [i0, i0 + TI) x [j0, j0 + TJ) of the chunk whose first sample is n0.
+struct Tile { int i0, j0, n0, H, W; };
+
+// Where a sample's dY patch [PR][PC][PIX] comes from.  load(s, buf) starts the copy of sample s's data into staging
+// buffer buf (one cp.async group); once that group has landed, patch(buf) returns the sample's patch.  `stage` is the
+// shared memory after the weights, SMEM the kernel's dynamic shared memory.
+struct DyPatch {   // dY [n, H/2, W/2, 64]: the patch itself, double-buffered
+  const __nv_bfloat16* dY;
+  static constexpr size_t SMEM = W_BYTES + 2 * PATCH_BYTES;
+  __device__ __forceinline__ void load(unsigned char* stage, const Tile& t, int sample, int buf) const {
+    const int Ho = t.H / 2, Wo = t.W / 2;
+    const __nv_bfloat16* src = dY + (size_t)(sample - t.n0) * Ho * Wo * 64;
+    unsigned char* dst = stage + (size_t)buf * PATCH_BYTES;
+    for (int q = threadIdx.x; q < PR * PC * 8; q += THREADS) {
+      const int pix = q >> 3, ch = q & 7;
+      const int oy = t.i0 - 1 + pix / PC, ox = t.j0 - 1 + pix % PC;
+      unsigned char* d = dst + (size_t)pix * PIX + ch * 16;
+      if (oy >= 0 && oy < Ho && ox >= 0 && ox < Wo) cp_async16(d, src + ((size_t)oy * Wo + ox) * 64 + ch * 8);
+      else *reinterpret_cast<uint4*>(d) = make_uint4(0u, 0u, 0u, 0u);
+    }
+    cp_commit();
+  }
+  __device__ __forceinline__ const unsigned char* patch(unsigned char* stage, const Tile&, int buf) const {
+    return stage + (size_t)buf * PATCH_BYTES;
+  }
+};
+
+// PoolPatch also fuses the backward of ConstantPad2d(1,0)+MaxPool(3,2): it reads d_pool [n,Hp,Wp,64] + the int8 argmax
+// saved by the forward pass and rebuilds each sample's d_stem patch in shared memory (fp32 sum of the <= 4 windows that
+// selected a stem pixel, rounded once to bf16 -- bit-identical to maxpool_bwd_kernel's output), so the [N,112,112,64]
+// stem-output gradient is never written to HBM either.  The pooled-window region is double-buffered, the patch is not.
+constexpr int RR = 7, RC = 11;                                   // pooled-window region feeding one patch
+constexpr size_t REGION_BYTES = (size_t)RR * RC * (128 + 64);    // d_pool (bf16 x64) + argmax (int8 x64) per window
+struct PoolPatch {   // stage: [PR][PC][PIX] patch, then [2][RR*RC][128 + 64] region
+  const __nv_bfloat16* dpool;
+  const int8_t* amax;
+  static constexpr size_t SMEM = W_BYTES + PATCH_BYTES + 2 * REGION_BYTES;
+  __device__ __forceinline__ void load(unsigned char* stage, const Tile& t, int sample, int buf) const {
+    const int Hp = t.H / 4, Wp = t.W / 4;
+    const int wy0 = t.i0 / 2 - 1, wx0 = t.j0 / 2 - 1;             // first pooled window row / col of the region
+    const __nv_bfloat16* sp = dpool + (size_t)(sample - t.n0) * Hp * Wp * 64;
+    const int8_t* sa = amax + (size_t)(sample - t.n0) * Hp * Wp * 64;
+    unsigned char* dst = stage + PATCH_BYTES + (size_t)buf * REGION_BYTES;
+    for (int q = threadIdx.x; q < RR * RC * 12; q += THREADS) {   // 8 chunks of d_pool + 4 chunks of argmax per window
+      const int win = q / 12, ch = q % 12;
+      const int wy = wy0 + win / RC, wx = wx0 + win % RC;
+      unsigned char* d = dst + (size_t)win * 192 + ch * 16;
+      if (wy >= 0 && wy < Hp && wx >= 0 && wx < Wp) {
+        const size_t o = ((size_t)wy * Wp + wx) * 64;
+        if (ch < 8) cp_async16(d, sp + o + ch * 8);
+        else cp_async16(d, sa + o + (ch - 8) * 16);
+      } else {
+        *reinterpret_cast<uint4*>(d) = ch < 8 ? make_uint4(0u, 0u, 0u, 0u) : make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu);
+      }
+    }
+    cp_commit();
+  }
+  // max-pool backward of the region into the patch; ends in a block barrier
+  __device__ __forceinline__ const unsigned char* patch(unsigned char* stage, const Tile& t, int buf) const {
+    const int Ho = t.H / 2, Wo = t.W / 2, Hp = t.H / 4, Wp = t.W / 4;
+    const int wy0 = t.i0 / 2 - 1, wx0 = t.j0 / 2 - 1;
+    const unsigned char* rg = stage + PATCH_BYTES + (size_t)buf * REGION_BYTES;
+    for (int q = threadIdx.x; q < PR * PC * 8; q += THREADS) {
+      const int pix = q >> 3, ch = q & 7;
+      const int oy = t.i0 - 1 + pix / PC, ox = t.j0 - 1 + pix % PC;
+      float acc8[8];
 #pragma unroll
-  for (int k = 0; k < 4; ++k)
-    if (row >= r[4 * k] && row < r[4 * k + 1] && col >= r[4 * k + 2] && col < r[4 * k + 3]) return true;
-  return false;
-}
+      for (int k = 0; k < 8; ++k) acc8[k] = 0.f;
+      if (oy >= 0 && oy < Ho && ox >= 0 && ox < Wo) {
+        for (int wy = oy / 2; wy <= (oy + 1) / 2; ++wy) {
+          const int ky = oy - 2 * wy + 1;
+          if (wy >= Hp || ky < 0 || ky > 2) continue;
+          for (int wx = ox / 2; wx <= (ox + 1) / 2; ++wx) {
+            const int kx = ox - 2 * wx + 1;
+            if (wx >= Wp || kx < 0 || kx > 2) continue;
+            const unsigned char* wp = rg + (size_t)((wy - wy0) * RC + (wx - wx0)) * 192;
+            const uint4 dv = *reinterpret_cast<const uint4*>(wp + ch * 16);
+            const uint2 av = *reinterpret_cast<const uint2*>(wp + 128 + ch * 8);
+            const __nv_bfloat162* dh = reinterpret_cast<const __nv_bfloat162*>(&dv);
+            const uint32_t am[2] = {av.x, av.y};
+            const int want = ky * 3 + kx;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+              if ((int)((am[k >> 2] >> (8 * (k & 3))) & 0xffu) == want) {
+                const float2 f = __bfloat1622float2(dh[k >> 1]);
+                acc8[k] += (k & 1) ? f.y : f.x;
+              }
+            }
+          }
+        }
+      }
+      __nv_bfloat162 o[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) o[k] = __floats2bfloat162_rn(acc8[2 * k], acc8[2 * k + 1]);
+      *reinterpret_cast<uint4*>(stage + (size_t)pix * PIX + ch * 16) = *reinterpret_cast<const uint4*>(o);
+    }
+    __syncthreads();
+    return stage;
+  }
+};
 }  // namespace stemb
 
-// dY: [n, Ho, Wo, 64] bf16 for the chunk's samples (sample index relative to n0); w_krsc: [64][7][7][cin_pad] bf16.
-// One CTA = one 8x16 tile of positions (i,j) of one image = a 16x32 block of input pixels; all four parity
-// classes share the dY patch (loaded once per sample).
-__global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dY,
-                                                                             const __nv_bfloat16* __restrict__ w_krsc,
+// `in` (a stemb::DyPatch or stemb::PoolPatch) gives each sample's dY [.., H/2, W/2, 64] patch; w_krsc: [64][7][7][cin_pad]
+// bf16.  One CTA = one 8x16 tile of positions (i,j) of one image = a 16x32 block of input pixels; all four parity
+// classes share the dY patch (one per sample).
+template <class Src>
+__global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_reduce_kernel(Src in, const __nv_bfloat16* __restrict__ w_krsc,
                                                                              int cin_pad, const int16_t* __restrict__ rects,
                                                                              float* __restrict__ G, int S, int n0, int n,
                                                                              int H, int W) {
   using namespace stemb;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned char* Ws = smem_raw;                                   // [49 taps, class-major][k][8] bf16, 16 B per (tap, k)
-  unsigned char* patch = smem_raw + W_BYTES;                      // [2][PR][PC][PIX]
-  const int Ho = H / 2, Wo = W / 2, Hc = H / 2, Wc = W / 2;       // positions per parity class
+  unsigned char* stage = smem_raw + W_BYTES;
+  const int Hc = H / 2, Wc = W / 2;                               // positions per parity class
   const int tiles_j = (Wc + TJ - 1) / TJ;
   const int ti = blockIdx.x / tiles_j, tj = blockIdx.x % tiles_j;
-  const int b = n0 / S + blockIdx.y;
-  const int lo = max(n0, b * S), hi = min(n0 + n, (b + 1) * S);
+  const auto [b, lo, hi, first] = image_span(S, n0, n, blockIdx.y);
   if (lo >= hi) return;
   const int i0 = ti * TI, j0 = tj * TJ;
+  const Tile tile{i0, j0, n0, H, W};
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // weights, class-major: class cls = py*2+px owns taps [tap0(cls), tap0(cls) + nky*nkx): 9, 12, 12, 16 taps
@@ -203,37 +298,20 @@ __global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_reduce_kernel(cons
     *reinterpret_cast<uint4*>(Ws + (size_t)q * 16) = *reinterpret_cast<const uint4*>(v);
   }
 
-  auto load_patch = [&](int sample, int buf) {
-    const __nv_bfloat16* src = dY + (size_t)(sample - n0) * Ho * Wo * 64;
-    unsigned char* dst = patch + (size_t)buf * PATCH_BYTES;
-    for (int q = threadIdx.x; q < PR * PC * 8; q += THREADS) {
-      const int pix = q >> 3, ch = q & 7;
-      const int oy = i0 - 1 + pix / PC, ox = j0 - 1 + pix % PC;
-      unsigned char* d = dst + (size_t)pix * PIX + ch * 16;
-      if (oy >= 0 && oy < Ho && ox >= 0 && ox < Wo) cp_async16(d, src + ((size_t)oy * Wo + ox) * 64 + ch * 8);
-      else *reinterpret_cast<uint4*>(d) = make_uint4(0u, 0u, 0u, 0u);
-    }
-    cp_commit();
-  };
-
   float tot[4][4];
 #pragma unroll
   for (int c = 0; c < 4; ++c) { tot[c][0] = tot[c][1] = tot[c][2] = tot[c][3] = 0.f; }
   const int g = lane >> 2, t4 = lane & 3;
   const int irow = i0 + warp;                                      // this warp's position row
 
-  load_patch(lo, 0);
+  in.load(stage, tile, lo, 0);
   for (int s = lo; s < hi; ++s) {
     const int buf = (s - lo) & 1;
-    if (s + 1 < hi) { load_patch(s + 1, buf ^ 1); cp_wait<1>(); } else { cp_wait<0>(); }
+    if (s + 1 < hi) { in.load(stage, tile, s + 1, buf ^ 1); cp_wait<1>(); } else { cp_wait<0>(); }
     __syncthreads();
-    const unsigned char* pb = patch + (size_t)buf * PATCH_BYTES;
-    short r[16];
-    if (rects != nullptr) {
-      const int4* rp = reinterpret_cast<const int4*>(rects + (size_t)s * 16);
-      *reinterpret_cast<int4*>(r) = __ldg(rp);
-      *reinterpret_cast<int4*>(r + 8) = __ldg(rp + 1);
-    }
+    const unsigned char* pb = in.patch(stage, tile, buf);
+    Occlusion occ;
+    if (rects != nullptr) occ.set(occl::load(rects, s));
     // The 49 taps use only 16 distinct patch shifts (di, dj) in {-1..2}^2: load each A fragment once and feed
     // every parity class that has a tap at this shift (shared-memory bandwidth is the limit: N is only 8).
     float acc[4][4];
@@ -265,15 +343,14 @@ __global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_reduce_kernel(cons
     for (int cls = 0; cls < 4; ++cls) {
       const int py = cls >> 1, px = cls & 1;
       const int y = 2 * irow + py, xA = 2 * (j0 + g) + px, xB = 2 * (j0 + g + 8) + px;
-      const bool keepA = rects == nullptr || !rect_hit(r, y, xA);
-      const bool keepB = rects == nullptr || !rect_hit(r, y, xB);
+      const bool keepA = rects == nullptr || !occ.hit(y, xA);
+      const bool keepB = rects == nullptr || !occ.hit(y, xB);
       if (keepA) { tot[cls][0] += acc[cls][0]; tot[cls][1] += acc[cls][1]; }
       if (keepB) { tot[cls][2] += acc[cls][2]; tot[cls][3] += acc[cls][3]; }
     }
-    __syncthreads();                                               // patch[buf] may be refilled two iterations on
+    __syncthreads();                                               // the staging buffers may be refilled
   }
   // C fragment: (row g: cols 2*t4, 2*t4+1), (row g+8: same cols); channels 0..2 are real
-  const bool first = (lo == b * S);
   if (irow < Hc && t4 < 2) {
 #pragma unroll
     for (int cls = 0; cls < 4; ++cls) {
@@ -296,201 +373,23 @@ __global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_reduce_kernel(cons
   }
 }
 
-// Variant that also fuses the backward of ConstantPad2d(1,0)+MaxPool(3,2): reads d_pool [n,Hp,Wp,64] + the int8
-// argmax saved by the forward pass and rebuilds each sample's d_stem patch in shared memory (fp32 sum of the <= 4
-// windows that selected a stem pixel, rounded once to bf16 -- bit-identical to maxpool_bwd_kernel's output), so the
-// [N,112,112,64] stem-output gradient is never written to HBM either.
-namespace stemb {
-constexpr int RR = 7, RC = 11;                                   // pooled-window region feeding one patch
-constexpr size_t REGION_BYTES = (size_t)RR * RC * (128 + 64);    // d_pool (bf16 x64) + argmax (int8 x64) per window
-constexpr size_t SMEM_POOL = W_BYTES + PATCH_BYTES + 2 * REGION_BYTES;
-}  // namespace stemb
-
-__global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_pool_reduce_kernel(const __nv_bfloat16* __restrict__ dpool,
-                                                                                  const int8_t* __restrict__ amax,
-                                                                                  const __nv_bfloat16* __restrict__ w_krsc,
-                                                                                  int cin_pad, const int16_t* __restrict__ rects,
-                                                                                  float* __restrict__ G, int S, int n0, int n,
-                                                                                  int H, int W) {
-  using namespace stemb;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  unsigned char* Ws = smem_raw;
-  unsigned char* patch = smem_raw + W_BYTES;                      // [PR][PC][PIX]
-  unsigned char* region = patch + PATCH_BYTES;                    // [2][RR*RC][128 + 64]
-  const int Ho = H / 2, Wo = W / 2, Hp = H / 4, Wp = W / 4, Hc = H / 2, Wc = W / 2;
-  const int tiles_j = (Wc + TJ - 1) / TJ;
-  const int ti = blockIdx.x / tiles_j, tj = blockIdx.x % tiles_j;
-  const int b = n0 / S + blockIdx.y;
-  const int lo = max(n0, b * S), hi = min(n0 + n, (b + 1) * S);
-  if (lo >= hi) return;
-  const int i0 = ti * TI, j0 = tj * TJ;
-  const int wy0 = i0 / 2 - 1, wx0 = j0 / 2 - 1;                   // first pooled window row / col of the region
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  for (int q = threadIdx.x; q < 49 * 64; q += THREADS) {
-    const int t = q >> 6, k = q & 63;
-    int cls = 0, tl = t;
-    if (tl >= 9) { cls = 1; tl -= 9; if (tl >= 12) { cls = 2; tl -= 12; if (tl >= 12) { cls = 3; tl -= 12; } } }
-    const int py = cls >> 1, px = cls & 1, nkx = px ? 4 : 3;
-    const int ky = (py ? 0 : 1) + 2 * (tl / nkx), kx = (px ? 0 : 1) + 2 * (tl % nkx);
-    const __nv_bfloat16* src = w_krsc + ((size_t)(k * 7 + ky) * 7 + kx) * cin_pad;
-    __nv_bfloat16 v[8];
-#pragma unroll
-    for (int c = 0; c < 8; ++c) v[c] = (c < 3) ? src[c] : __float2bfloat16(0.f);
-    *reinterpret_cast<uint4*>(Ws + (size_t)q * 16) = *reinterpret_cast<const uint4*>(v);
-  }
-
-  auto load_region = [&](int sample, int buf) {
-    const __nv_bfloat16* sp = dpool + (size_t)(sample - n0) * Hp * Wp * 64;
-    const int8_t* sa = amax + (size_t)(sample - n0) * Hp * Wp * 64;
-    unsigned char* dst = region + (size_t)buf * REGION_BYTES;
-    for (int q = threadIdx.x; q < RR * RC * 12; q += THREADS) {   // 8 chunks of d_pool + 4 chunks of argmax per window
-      const int win = q / 12, ch = q % 12;
-      const int wy = wy0 + win / RC, wx = wx0 + win % RC;
-      unsigned char* d = dst + (size_t)win * 192 + ch * 16;
-      if (wy >= 0 && wy < Hp && wx >= 0 && wx < Wp) {
-        const size_t o = ((size_t)wy * Wp + wx) * 64;
-        if (ch < 8) cp_async16(d, sp + o + ch * 8);
-        else cp_async16(d, sa + o + (ch - 8) * 16);
-      } else {
-        *reinterpret_cast<uint4*>(d) = ch < 8 ? make_uint4(0u, 0u, 0u, 0u) : make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu);
-      }
-    }
-    cp_commit();
-  };
-
-  float tot[4][4];
-#pragma unroll
-  for (int c = 0; c < 4; ++c) { tot[c][0] = tot[c][1] = tot[c][2] = tot[c][3] = 0.f; }
-  const int g = lane >> 2, t4 = lane & 3;
-  const int irow = i0 + warp;
-
-  load_region(lo, 0);
-  for (int s = lo; s < hi; ++s) {
-    const int buf = (s - lo) & 1;
-    if (s + 1 < hi) { load_region(s + 1, buf ^ 1); cp_wait<1>(); } else { cp_wait<0>(); }
-    __syncthreads();
-    // ---- rebuild the d_stem patch of this sample from the pooled windows (max-pool backward) ----
-    const unsigned char* rg = region + (size_t)buf * REGION_BYTES;
-    for (int q = threadIdx.x; q < PR * PC * 8; q += THREADS) {
-      const int pix = q >> 3, ch = q & 7;
-      const int oy = i0 - 1 + pix / PC, ox = j0 - 1 + pix % PC;
-      float acc8[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) acc8[k] = 0.f;
-      if (oy >= 0 && oy < Ho && ox >= 0 && ox < Wo) {
-        for (int wy = oy / 2; wy <= (oy + 1) / 2; ++wy) {
-          const int ky = oy - 2 * wy + 1;
-          if (wy >= Hp || ky < 0 || ky > 2) continue;
-          for (int wx = ox / 2; wx <= (ox + 1) / 2; ++wx) {
-            const int kx = ox - 2 * wx + 1;
-            if (wx >= Wp || kx < 0 || kx > 2) continue;
-            const unsigned char* wp = rg + (size_t)((wy - wy0) * RC + (wx - wx0)) * 192;
-            const uint4 dv = *reinterpret_cast<const uint4*>(wp + ch * 16);
-            const uint2 av = *reinterpret_cast<const uint2*>(wp + 128 + ch * 8);
-            const __nv_bfloat162* dh = reinterpret_cast<const __nv_bfloat162*>(&dv);
-            const uint32_t am[2] = {av.x, av.y};
-            const int want = ky * 3 + kx;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              if ((int)((am[k >> 2] >> (8 * (k & 3))) & 0xffu) == want) {
-                const float2 f = __bfloat1622float2(dh[k >> 1]);
-                acc8[k] += (k & 1) ? f.y : f.x;
-              }
-            }
-          }
-        }
-      }
-      __nv_bfloat162 o[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) o[k] = __floats2bfloat162_rn(acc8[2 * k], acc8[2 * k + 1]);
-      *reinterpret_cast<uint4*>(patch + (size_t)pix * PIX + ch * 16) = *reinterpret_cast<const uint4*>(o);
-    }
-    __syncthreads();
-    const unsigned char* pb = patch;
-    short r[16];
-    if (rects != nullptr) {
-      const int4* rp = reinterpret_cast<const int4*>(rects + (size_t)s * 16);
-      *reinterpret_cast<int4*>(r) = __ldg(rp);
-      *reinterpret_cast<int4*>(r + 8) = __ldg(rp + 1);
-    }
-    float acc[4][4];
-#pragma unroll
-    for (int c = 0; c < 4; ++c) { acc[c][0] = acc[c][1] = acc[c][2] = acc[c][3] = 0.f; }
-#pragma unroll
-    for (int di = -1; di <= 2; ++di) {
-#pragma unroll
-      for (int dj = -1; dj <= 2; ++dj) {
-        const unsigned char* arow = pb + ((size_t)(warp + di + 1) * PC + (lane & 15) + dj + 1) * PIX + (lane >> 4) * 16;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          uint32_t a0, a1, a2, a3;
-          stem::ldmatrix_x4(a0, a1, a2, a3, arow + kk * 32);
-#pragma unroll
-          for (int cls = 0; cls < 4; ++cls) {
-            const int py = cls >> 1, px = cls & 1, nkx = px ? 4 : 3;
-            if ((di == 2 && !py) || (dj == 2 && !px)) continue;
-            const int t = ((py ? 2 : 1) - di) * nkx + ((px ? 2 : 1) - dj);
-            const int tap0 = cls == 0 ? 0 : (cls == 1 ? 9 : (cls == 2 ? 21 : 33));
-            uint32_t b0, b1;
-            ldmatrix_x2_trans(b0, b1, Ws + ((size_t)(tap0 + t) * 64 + kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * 16);
-            stem::mma_bf16(acc[cls], a0, a1, a2, a3, b0, b1);
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int cls = 0; cls < 4; ++cls) {
-      const int py = cls >> 1, px = cls & 1;
-      const int y = 2 * irow + py, xA = 2 * (j0 + g) + px, xB = 2 * (j0 + g + 8) + px;
-      const bool keepA = rects == nullptr || !rect_hit(r, y, xA);
-      const bool keepB = rects == nullptr || !rect_hit(r, y, xB);
-      if (keepA) { tot[cls][0] += acc[cls][0]; tot[cls][1] += acc[cls][1]; }
-      if (keepB) { tot[cls][2] += acc[cls][2]; tot[cls][3] += acc[cls][3]; }
-    }
-    __syncthreads();                                               // patch / region[buf] free for the next samples
-  }
-  const bool first = (lo == b * S);
-  if (irow < Hc && t4 < 2) {
-#pragma unroll
-    for (int cls = 0; cls < 4; ++cls) {
-      const int py = cls >> 1, px = cls & 1;
-      const int y = 2 * irow + py;
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        const int x = 2 * (j0 + g + half * 8) + px;
-        if (x >= W) continue;
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int c = 2 * t4 + e;
-          if (c >= 3) continue;
-          float* gp = G + ((size_t)b * 3 + c) * H * W + (size_t)y * W + x;
-          const float v = 2.0f * tot[cls][half * 2 + e];
-          *gp = first ? v : (*gp + v);
-        }
-      }
-    }
-  }
-}
-
-void launch_stem_bwd_pool_reduce(const void* dpool, const int8_t* amax, const void* w_krsc, int cin_pad, const int16_t* rects,
-                                 float* G, int B, int S, int n0, int n, int H, int W, cudaStream_t st) {
-  (void)B;
-  cudaFuncSetAttribute(stem_bwd_pool_reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)stemb::SMEM_POOL);
-  const int nb = (n0 + n - 1) / S - n0 / S + 1;
+template <class Src>
+static void launch_stem_bwd(Src in, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int S, int n0, int n,
+                            int H, int W, cudaStream_t st) {
+  cudaFuncSetAttribute(stem_bwd_reduce_kernel<Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Src::SMEM);
   const int tiles = ((H / 2 + stemb::TI - 1) / stemb::TI) * ((W / 2 + stemb::TJ - 1) / stemb::TJ);
-  stem_bwd_pool_reduce_kernel<<<dim3(tiles, nb), stemb::THREADS, stemb::SMEM_POOL, st>>>(
-      (const __nv_bfloat16*)dpool, amax, (const __nv_bfloat16*)w_krsc, cin_pad, rects, G, S, n0, n, H, W);
+  stem_bwd_reduce_kernel<Src><<<dim3(tiles, images_touched(S, n0, n)), stemb::THREADS, Src::SMEM, st>>>(
+      in, (const __nv_bfloat16*)w_krsc, cin_pad, rects, G, S, n0, n, H, W);
 }
-
 void launch_stem_bwd_reduce(const void* dY, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int B, int S,
                             int n0, int n, int H, int W, cudaStream_t st) {
   (void)B;
-  cudaFuncSetAttribute(stem_bwd_reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)stemb::SMEM);
-  const int nb = (n0 + n - 1) / S - n0 / S + 1;
-  const int tiles = ((H / 2 + stemb::TI - 1) / stemb::TI) * ((W / 2 + stemb::TJ - 1) / stemb::TJ);
-  stem_bwd_reduce_kernel<<<dim3(tiles, nb), stemb::THREADS, stemb::SMEM, st>>>(
-      (const __nv_bfloat16*)dY, (const __nv_bfloat16*)w_krsc, cin_pad, rects, G, S, n0, n, H, W);
+  launch_stem_bwd(stemb::DyPatch{(const __nv_bfloat16*)dY}, w_krsc, cin_pad, rects, G, S, n0, n, H, W, st);
+}
+void launch_stem_bwd_pool_reduce(const void* dpool, const int8_t* amax, const void* w_krsc, int cin_pad, const int16_t* rects,
+                                 float* G, int B, int S, int n0, int n, int H, int W, cudaStream_t st) {
+  (void)B;
+  launch_stem_bwd(stemb::PoolPatch{(const __nv_bfloat16*)dpool, amax}, w_krsc, cin_pad, rects, G, S, n0, n, H, W, st);
 }
 
 }  // namespace dp

@@ -31,6 +31,14 @@ def _host(a, dtype):
     return a, C.c_void_p(a.ctypes.data)
 
 
+def _host_rects(rects, N):
+    """The occlusion table of N samples (four int16 rectangles {r0, r1, c0, c1} each) as a contiguous host array and
+    its pointer; (None, None) without occlusion."""
+    if rects is None:
+        return None, None
+    return _host(np.asarray(rects).reshape(N, 4, 4), np.int16)
+
+
 class Engine:
     """ResNetV2-50x1-BiT attack engine on one CUDA device."""
 
@@ -162,9 +170,7 @@ class Engine:
         N = B * S
         dt = torch.bfloat16 if self.elem_bytes == 2 else torch.float32
         out = torch.empty((N, self.img, self.img, self.c_pad), dtype=dt, device=img.device)
-        rp = None
-        if rects is not None:
-            rects, rp = _host(np.asarray(rects).reshape(N, 4, 4), np.int16)
+        rects, rp = _host_rects(rects, N)
         _lib.check(self.lib.dp_expand(self.handle, _dev_ptr(img), B, S, rp, C.c_void_p(out.data_ptr()),
                                       self._stream()))
         return out
@@ -175,9 +181,7 @@ class Engine:
         N = B * S
         preds = np.empty(N, np.int32)
         logits = np.empty((N, self.n_classes), np.float32) if return_logits else None
-        rp = None
-        if rects is not None:
-            rects, rp = _host(np.asarray(rects).reshape(N, 4, 4), np.int16)
+        rects, rp = _host_rects(rects, N)
         _lib.check(self.lib.dp_predict(self.handle, _dev_ptr(img), B, S, rp, C.c_void_p(preds.ctypes.data),
                                        C.c_void_p(logits.ctypes.data) if return_logits else None, self._stream()))
         return (preds, logits) if return_logits else preds
@@ -190,9 +194,7 @@ class Engine:
         B = img.shape[0]
         N = B * int(S)
         logits = torch.empty((N, self.n_classes), dtype=torch.float32, device=img.device)
-        rp = None
-        if rects is not None:
-            rects, rp = _host(np.asarray(rects).reshape(N, 4, 4), np.int16)
+        rects, rp = _host_rects(rects, N)
         if xforms is None:
             _lib.check(self.lib.dp_eot_forward(self.handle, _dev_ptr(img), B, int(S), rp, _dev_ptr(logits),
                                                self._stream()))
