@@ -8,8 +8,9 @@ namespace dp {
 
 constexpr int GN_GROUPS = 32;
 constexpr int GN_MAX_SPLITS = 16;
-// GroupNorm scratch (`partial`): N * GN_WS_FLOATS_PER_SAMPLE + GN_WS_FLOATS_EXTRA floats (v3: per-tile partial sums,
-// per-sample backward means, the work / done / ready counters; also covers the two-pass kernels' split partials)
+// GroupNorm scratch (`partial`): N * GN_WS_FLOATS_PER_SAMPLE + GN_WS_FLOATS_EXTRA floats.  Per sample it holds the
+// statistics pass's per-tile partial sums (64 floats per tile; a sample with more tiles than fit takes the two-pass
+// statistics) or the two-pass kernels' split partials (GN_MAX_SPLITS * 64 floats).
 constexpr int GN_WS_FLOATS_PER_SAMPLE = 8192;
 constexpr int GN_WS_FLOATS_EXTRA = 4096;
 // int16 per sample of an occlusion table `rects` [N][RECT_SHORTS]: four rectangles {r0, r1, c0, c1} (common.cuh decodes them)
@@ -23,7 +24,6 @@ void launch_weight_standardize(const float* w_oihw, void* w_krsc, int O, int I, 
 void launch_pack_nchw(const float* z, void* out, int N, int H, int W, int Cp, bool bf16, cudaStream_t st);
 void launch_unpack_nhwc(const void* in, float* dz, int N, int H, int W, int Cp, bool bf16, cudaStream_t st);
 
-int gn_splits(int P, int C, bool bf16);
 // GroupNorm(32)+ReLU forward: stats partials -> apply.  `stats` [N][32][2] receives (mean, rstd).
 void launch_gn_relu_forward(const void* x, void* y, const float* gamma, const float* beta, float* partial,
                             float* stats, int N, int P, int C, bool bf16, cudaStream_t st);

@@ -1,5 +1,6 @@
 """Op-level GPU parity of the hand-written kernels that the network-level tests only see through the whole net:
-GroupNorm(32)+ReLU v2 forward / backward (fp32 and bf16, every ResNetV2-50 shape class), the bf16 engine's fused
+GroupNorm(32)+ReLU forward / backward (fp32 and bf16, every ResNetV2-50 shape class; the cluster kernels where their
+plan fits, the two-pass kernels at fp32 C = 2048 and at slabs too large for a cluster), the bf16 engine's fused
 stem-dgrad + masked EOT reduce (K1^T as the bench runs it), and the wgmma GroupNorm-prologue GEMM -- each against
 a PyTorch fp32/fp64 CPU restatement of the same operator on the same (bf16-rounded) operands, through the C ABI's
 dp_debug_* hooks.  Restated operators: timm GroupNormAct = F.group_norm(32, eps 1e-5) + ReLU and its autograd
@@ -41,7 +42,8 @@ def engines(oracle_params):
         e.close()
 
 
-GN_SHAPES = [(3136, 64), (3136, 256), (784, 128), (784, 512), (196, 1024), (196, 256), (49, 2048), (49, 512)]
+# (7056, 256): the first stage's 256-channel norms at 336 px; no cluster plan fits, so both dtypes run the two-pass kernels
+GN_SHAPES = [(3136, 64), (3136, 256), (784, 128), (784, 512), (196, 1024), (196, 256), (49, 2048), (49, 512), (7056, 256)]
 
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
