@@ -76,6 +76,9 @@ SIGNATURES = {
     "dp_failed_set_update": (c_i32, [c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_f32, c_vp, c_vp]),
     "dp_failed_set_read": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_vp, c_vp]),
     "dp_debug_stem_bwd_reduce": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp]),
+    "dp_debug_stem_bwd_pool_reduce": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp]),
+    "dp_debug_stem_forward": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),
+    "dp_debug_maxpool": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp]),
     "dp_debug_gn_gemm": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_vp]),
     "dp_debug_gn": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp]),
 }

@@ -856,25 +856,38 @@ struct dp_engine {
       for (int n0 = 0; n0 < N; n0 += SUB)
         f(std::min(SUB, N - n0), (char*)x + (size_t)n0 * H * H * x_ch * e->es, (char*)y + (size_t)n0 * hs * hs * STEM_CH * e->es);
     }
-    // the own kernels, also behind the op-level test hooks
+    // the own kernels and the max-pool, also behind the op-level test hooks
+    void own_forward(const void* input, void* out, int N, cudaStream_t st) const {
+      dp::launch_stem_forward(input, w_kn, out, N, e->H, e->H, st); KERNEL_OK(); ++e->launches;
+    }
+    // ConstantPad2d(1, 0) + MaxPool2d(3, 2) of x [N,hs,hs,C] into y [N,hs/2,hs/2,C] (argmax: null or [N,hs/2,hs/2,C])
+    void pool_forward(const void* x, void* y, int8_t* amax, int N, int hs, int C, cudaStream_t st) const {
+      dp::launch_maxpool_forward(x, y, amax, N, hs, hs, C, e->bf16, st); KERNEL_OK(); ++e->launches;
+    }
+    void pool_backward(const void* dy, const int8_t* amax, void* dx, int N, int hs, int C, cudaStream_t st) const {
+      dp::launch_maxpool_backward(dy, amax, dx, N, hs, hs, C, e->bf16, st); KERNEL_OK(); ++e->launches;
+    }
     void own_wgrad(const void* input, const void* dY, float* partial, float* acc, int N, int cin_pad, cudaStream_t st) const {
       dp::launch_stem_wgrad(input, dY, partial, acc, N, e->H, e->H, cin_pad, st); KERNEL_OK(); e->launches += 2;
     }
     void fused_reduce(const void* dY, const FusedReduce& fr, int N, cudaStream_t st) const {
       dp::launch_stem_bwd_reduce(dY, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st); KERNEL_OK(); ++e->launches;
     }
+    void fused_pool_reduce(const void* dpool, const int8_t* amax, const FusedReduce& fr, int N, cudaStream_t st) const {
+      dp::launch_stem_bwd_pool_reduce(dpool, amax, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st);
+      KERNEL_OK(); ++e->launches;
+    }
     // input [N,H,H,in_ch] -> conv -> max-pool into L.x0 (train: keep the argmax for the backward)
     void forward(const Lane& L, int N, const void* input, bool train, cudaStream_t st) const {
       const int H = e->H, hs = e->Hs(), hp = e->Hp();
       if (fwd == FWD_OWN) {
         PROF(e, "stem_conv_fwd", ((double)N * H * H * 3 + (double)N * hs * hs * STEM_CH) * e->es, 2.0 * N * hs * hs * STEM_CH * 147, st,
-             dp::launch_stem_forward(input, w_kn, L.act, N, H, H, st));
-        KERNEL_OK(); ++e->launches;
+             own_forward(input, L.act, N, st));
       } else {
         cudnn_slices(N, input, in_ch, L.act, [&](int n, char* x, char* y) { e->conv_fwd(L, 0, conv, n, H, hs, x, y, st); });
       }
       PROF(e, "maxpool_fwd", (double)N * (hs * hs + hp * hp) * STEM_CH * e->es, 0, st,
-           dp::launch_maxpool_forward(L.act, L.x0, train ? L.pool_amax : nullptr, N, hs, hs, STEM_CH, e->bf16, st)); KERNEL_OK(); ++e->launches;
+           pool_forward(L.act, L.x0, train ? L.pool_amax : nullptr, N, hs, STEM_CH, st));
     }
     // d_x0: the gradient at the max-pool output.  Max-pool backward, the stem's weight gradient when wg wants it, then
     // the dgrad, or the fused reduce when fr is given.  Returns d/d(input) ([N,H,H,dx_ch] in L.g[2]), or null when
@@ -887,13 +900,11 @@ struct dp_engine {
       if (fr && bwd == END_FUSED_POOL_REDUCE && !wg) {
         // max-pool backward + stem dgrad + masked EOT reduce in one kernel: neither d_stem nor d/d(input) is written
         PROF(e, "stem_bwd_reduce", (double)N * (hs / 2) * (hs / 2) * STEM_CH * (e->es + 1) + 3.0 * H * H * 4 * (double)N / fr->S,
-             2.0 * N * hs * hs * STEM_CH * 147, st,
-             dp::launch_stem_bwd_pool_reduce(d_x0, L.pool_amax, conv.w, conv.cin_pad, fr->rects, fr->G, fr->B, fr->S, fr->n0, N, H, H, st));
-        KERNEL_OK(); ++e->launches;
+             2.0 * N * hs * hs * STEM_CH * 147, st, fused_pool_reduce(d_x0, L.pool_amax, *fr, N, st));
         return nullptr;
       }
       PROF(e, "maxpool_bwd", (double)N * (hs * hs + (hs / 2) * (hs / 2)) * STEM_CH * e->es, 0, st,
-           dp::launch_maxpool_backward(d_x0, L.pool_amax, GB, N, hs, hs, STEM_CH, e->bf16, st)); KERNEL_OK(); ++e->launches;
+           pool_backward(d_x0, L.pool_amax, GB, N, hs, STEM_CH, st));
       if (want_w) {                                                                // dY = the max-pool adjoint (GB)
         float* const acc = e->acc_of(L, conv.pid);
         if (wgrad == WG_OWN)
@@ -1934,18 +1945,59 @@ int32_t dp_failed_set_read(dp_engine* e, int32_t b, int32_t* idx_host_out, int32
   DP_CATCH
 }
 
-/* ---- op-level test hooks (tests/test_gpu_ops.py) ------------------------------------------------------ */
+/* ---- op-level test hooks (tests/test_gpu_ops.py, tests/test_gpu_stem_ops.py) --------------------------- */
+// G is left to the kernel (no memset), which writes every element of every image: a gap would show as the caller's fill.
 int32_t dp_debug_stem_bwd_reduce(dp_engine* e, const void* dY, const int16_t* rects_host, int32_t B, int32_t S, float* G,
                                  void* stream) {
   DP_TRY
   if (!e) fail("null engine");
   if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_bwd_reduce: the fused stem backward exists for the bf16 engine only");
+  if (!dY || !G || B < 1 || S < 1) fail("dp_debug_stem_bwd_reduce: bad arguments");
   CUDA_OK(cudaSetDevice(e->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   const int N = B * S;
   e->h2d_samples(rects_host, N, st);
-  CUDA_OK(cudaMemsetAsync(G, 0, (size_t)B * 3 * e->H * e->H * 4, st));
   e->stem.fused_reduce(dY, dp_engine::FusedReduce{rects_host ? e->rects_d : nullptr, G, B, S, 0}, N, st);
+  DP_CATCH
+}
+
+int32_t dp_debug_stem_bwd_pool_reduce(dp_engine* e, const void* dpool, const int8_t* amax, const int16_t* rects_host, int32_t B,
+                                      int32_t S, float* G, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_bwd_pool_reduce: the fused stem backward exists for the bf16 engine only");
+  if (!dpool || !amax || !G || B < 1 || S < 1) fail("dp_debug_stem_bwd_pool_reduce: bad arguments");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int N = B * S;
+  e->h2d_samples(rects_host, N, st);
+  e->stem.fused_pool_reduce(dpool, amax, dp_engine::FusedReduce{rects_host ? e->rects_d : nullptr, G, B, S, 0}, N, st);
+  DP_CATCH
+}
+
+int32_t dp_debug_stem_forward(dp_engine* e, const void* in, void* out, void* w_out, int32_t N, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_forward: this engine's stem is not the own bf16 kernel");
+  if (!in || !out || N < 1 || N > 65535) fail("dp_debug_stem_forward: bad arguments");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const ConvW& c = e->stem.conv;
+  if (w_out) CUDA_OK(cudaMemcpyAsync(w_out, c.w, (size_t)c.cout * c.k * c.k * c.cin_pad * 2, cudaMemcpyDeviceToDevice, st));
+  e->stem.own_forward(in, out, N, st);
+  DP_CATCH
+}
+
+int32_t dp_debug_maxpool(dp_engine* e, const void* x, void* y, int8_t* amax, const void* dy, void* dx, int32_t N, int32_t Hs,
+                         int32_t C, void* stream) {
+  DP_TRY
+  if (!e) fail("null engine");
+  if (!x || !y || N < 1 || Hs < 2 || Hs % 2 != 0 || C < 1 || C % (e->bf16 ? 8 : 4) != 0 || (dy && (!amax || !dx)))
+    fail("dp_debug_maxpool: bad arguments");
+  CUDA_OK(cudaSetDevice(e->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  e->stem.pool_forward(x, y, amax, N, Hs, C, st);
+  if (dy) e->stem.pool_backward(dy, amax, dx, N, Hs, C, st);
   DP_CATCH
 }
 

@@ -26,6 +26,14 @@ def _dev_ptr(t, dtype=torch.float32):
     return C.c_void_p(t.data_ptr())
 
 
+def _version(t):
+    """t's in-place version counter, or None for an inference-mode tensor, which keeps none."""
+    try:
+        return t._version
+    except RuntimeError:
+        return None
+
+
 def _host(a, dtype):
     a = np.ascontiguousarray(a, dtype=dtype)
     return a, C.c_void_p(a.ctypes.data)
@@ -206,11 +214,27 @@ class Engine:
                                                      self._stream()))
         self.eot_forwards += 1
         self._eot_shape = tuple(img.shape)
+        # The backward reads img again for the chunks whose activations the engine no longer holds: keep the tensor
+        # alive (a caller's temporary would otherwise be freed and its memory handed to the next allocation, such as
+        # the gradient itself) and remember its version to refuse a backward after an in-place change.
+        self._eot_img, self._eot_img_version = img, _version(img)
         return logits
 
+    def _check_eot_img(self, fn, out):
+        img = getattr(self, "_eot_img", None)
+        if img is None:
+            return
+        if _version(img) != self._eot_img_version:
+            raise RuntimeError("%s: the image of the last eot_forward was modified in place since; run the forward "
+                               "again" % fn)
+        if out is not None and out.untyped_storage().data_ptr() == img.untyped_storage().data_ptr():
+            raise ValueError("%s: the gradient buffer shares memory with the image of the last eot_forward" % fn)
+
     def eot_backward(self, dlogits, out=None):
-        """d<dlogits, logits>/d img of the last eot_forward, [B,3,H,W] (weight gradients: eot_backward_params)."""
+        """d<dlogits, logits>/d img of the last eot_forward, [B,3,H,W] (weight gradients: eot_backward_params).
+        The image given to eot_forward must be unchanged (checked through its version counter)."""
         out = torch.empty(self._eot_shape, dtype=torch.float32, device=dlogits.device) if out is None else out
+        self._check_eot_img("eot_backward", out)
         _lib.check(self.lib.dp_eot_backward(self.handle, _dev_ptr(dlogits), _dev_ptr(out), self._stream()))
         return out
 
@@ -237,6 +261,7 @@ class Engine:
             if g.numel() != want:
                 raise ValueError("eot_backward_params: the gradient buffer of %s has %d elements, %s has %d"
                                  % (k, g.numel(), k, want))
+        self._check_eot_img("eot_backward_params", out)
         c_names = (C.c_char_p * n)(*[k.encode() for k in names])
         c_ptrs = (C.c_void_p * n)(*[_dev_ptr(g).value for g in grads])
         _lib.check(self.lib.dp_eot_backward_params(self.handle, _dev_ptr(dlogits), _dev_ptr(out), n, c_names, c_ptrs,

@@ -263,6 +263,21 @@ int32_t dp_failed_set_read(dp_engine* e, int32_t b, int32_t* idx_host_out, int32
  *   kernel in front of the wgmma GEMM and the classifier head). */
 int32_t dp_debug_stem_bwd_reduce(dp_engine* e, const void* dY, const int16_t* rects_host, int32_t B, int32_t S, float* G,
                                  void* stream);
+/* The bf16 engine's stem on caller-supplied tensors (tests/test_gpu_stem_ops.py), through the launches the engine runs.
+ * G is written by the kernels alone: every element of every image, nothing is zeroed first.
+ * dp_debug_stem_bwd_pool_reduce: dp_debug_stem_bwd_reduce with the max-pool backward fused in (DORPATCH_POOL_BWD=fused):
+ *   dpool [B*S, H/4, H/4, 64] bf16 and its argmax amax [B*S, H/4, H/4, 64] int8 (ky*3+kx, from dp_debug_maxpool).
+ * dp_debug_stem_forward: the own stem convolution, in [N,H,H,3] bf16 -> out [N,H/2,H/2,64] bf16.  w_out (optional)
+ *   receives the standardised weights the kernel reads, [64,7,7,cin_pad] bf16 (cin_pad 8, or DORPATCH_CPAD).
+ *   Refused by an engine whose stem is not the own kernel.
+ * dp_debug_maxpool: ConstantPad2d(1, 0) + MaxPool2d(3, 2) in the engine's activation dtype: x [N,Hs,Hs,C] -> y
+ *   [N,Hs/2,Hs/2,C] and (amax not null) the int8 argmax ky*3+kx of each window; with dy [N,Hs/2,Hs/2,C] also the
+ *   backward dx [N,Hs,Hs,C] from dy and amax.  Hs even, C a multiple of 8 (bf16) or 4 (fp32). */
+int32_t dp_debug_stem_bwd_pool_reduce(dp_engine* e, const void* dpool, const int8_t* amax, const int16_t* rects_host, int32_t B,
+                                      int32_t S, float* G, void* stream);
+int32_t dp_debug_stem_forward(dp_engine* e, const void* in, void* out, void* w_out, int32_t N, void* stream);
+int32_t dp_debug_maxpool(dp_engine* e, const void* x, void* y, int8_t* amax, const void* dy, void* dx, int32_t N, int32_t Hs,
+                         int32_t C, void* stream);
 /* bf16 stem weight-gradient kernel of dp_eot_backward_params on caller-supplied operands (tests/test_gpu_param_grad.py):
  * dW [64,7,7,3] fp32 dev (overwritten) = sum over samples and output pixels of dY [N,H/2,H/2,64] x im2col(in [N,H,H,3]),
  * both bf16 dev (the tight network input of the bf16 engine). */
