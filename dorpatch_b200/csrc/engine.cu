@@ -23,6 +23,7 @@
 #include <stdexcept>
 #include <string>
 #include <tuple>
+#include <utility>
 #include <vector>
 
 #include <nvtx3/nvToolsExt.h>   // header-only NVTX v3: no-ops unless a profiler injects itself (ncu --nvtx, nsys)
@@ -58,10 +59,6 @@ thread_local std::string g_last_error;
     cublasStatus_t _s = (expr);                                                                    \
     if (_s != CUBLAS_STATUS_SUCCESS) fail("cuBLASLt error %d at %s:%d [%s]", (int)_s, __FILE__, __LINE__, #expr); \
   } while (0)
-#define KERNEL_OK() CUDA_OK(cudaGetLastError())
-// PROF(engine, "category", algorithmic bytes, flops, stream, statement)
-#define PROF(E, NAME, BYTES, FLOPS, ST, ...) \
-  do { (E)->prof_begin(NAME, (double)(BYTES), (double)(FLOPS), ST); __VA_ARGS__; (E)->prof_end(ST); } while (0)
 
 constexpr int DEPTHS[4] = {3, 4, 6, 3};
 constexpr int WIDTHS[4] = {256, 512, 1024, 2048};
@@ -229,6 +226,20 @@ struct dp_engine {
     }
     prof_recs.clear();
   }
+  // Every launch of the engine: f() enqueues on st and returns the number of kernels it enqueued (a dp::launch_*'s
+  // return value; 1 for a cuDNN / cublasLt call, whatever the library enqueues inside it).  The sum is `launches`
+  // (dp_engine_launch_count); cuDNN Find* and cublasLt autotune trials run outside run() and are not counted.
+  // cat: the profiler region's category and its algorithmic bytes / flops; run(st, f) is a launch outside the profile.
+  template <class F>
+  void run(const char* cat, double bytes, double flops, cudaStream_t st, F&& f) {
+    if (cat) prof_begin(cat, bytes, flops, st);
+    const int n = f();
+    if (cat) prof_end(st);
+    CUDA_OK(cudaGetLastError());
+    launches += n;
+  }
+  template <class F>
+  void run(cudaStream_t st, F&& f) { run(nullptr, 0, 0, st, std::forward<F>(f)); }
 
   // ---- whole-step CUDA graphs (SURVEY 8f N4): dp_attack_grad's launch sequence (staging copies, paste, regularisers,
   // every chunk's K1 -> forward -> CW -> backward -> K1^T on both lanes, result copies) captured once per call
@@ -504,9 +515,9 @@ struct dp_engine {
   }
   float* acc_of(const Lane& L, int pid) const { return L.wacc + wparams[pid].off; }
 
-  // ---- weights -------------------------------------------------------------------------
+  // ---- weights (their launches are counted, not profiled) --------------------------------------------------------
   void standardize(const ConvW& c, cudaStream_t st) {
-    dp::launch_weight_standardize(c.raw, c.w, c.cout, c.cin, c.k, c.k, c.cin_pad, bf16, true, st); KERNEL_OK();
+    run(st, [&] { return dp::launch_weight_standardize(c.raw, c.w, c.cout, c.cin, c.k, c.k, c.cin_pad, bf16, true, st); });
   }
   // One timm tensor from `src` (kind: H2D or D2D, on st), then what that kind needs: a convolution is re-standardised
   // and its packed copies rebuilt (the stem's tile, or the fused GEMM's), a GroupNorm's "every gamma > 0" flag (the
@@ -521,8 +532,8 @@ struct dp_engine {
         standardize(c, st);
         if (fused_gemm)
           for (auto& b : blocks) {
-            if (&c == &b.c1) { dp::launch_gn_gemm_pack(b.c1.w, b.c1p, b.mid, b.cin, st); KERNEL_OK(); }
-            if (&c == &b.c3) { dp::launch_gn_gemm_pack(b.c3.w, b.c3p, b.cout, b.mid, st); KERNEL_OK(); }
+            if (&c == &b.c1) run(st, [&] { return dp::launch_gn_gemm_pack(b.c1.w, b.c1p, b.mid, b.cin, st); });
+            if (&c == &b.c3) run(st, [&] { return dp::launch_gn_gemm_pack(b.c3.w, b.c3p, b.cout, b.mid, st); });
           }
         break;
       }
@@ -638,9 +649,10 @@ struct dp_engine {
     const float one = 1.f, zero = 0.f;
     const double fl = 2.0 * N * hout * hout * c.cout * c.k * c.k * c.cin;
     const double by = ((double)N * hin * hin * c.cin_pad + (double)N * hout * hout * c.cout + (double)c.cout * c.k * c.k * c.cin_pad) * es;
-    PROF(this, c.k == 7 ? "stem_conv_fwd" : "conv3x3_fwd", by, fl, st,
-         CUDNN_OK(cudnnConvolutionForward(L.cudnn, &one, p.xdesc, x, c.wdesc, c.w, c.cdesc, p.fwd_algo, L.lib_ws, lib_ws_bytes, &zero, p.ydesc, y)));
-    ++launches;
+    run(c.k == 7 ? "stem_conv_fwd" : "conv3x3_fwd", by, fl, st, [&] {
+      CUDNN_OK(cudnnConvolutionForward(L.cudnn, &one, p.xdesc, x, c.wdesc, c.w, c.cdesc, p.fwd_algo, L.lib_ws, lib_ws_bytes, &zero, p.ydesc, y));
+      return 1;
+    });
   }
   void conv_bwd(const Lane& L, int layer_id, const ConvW& c, int N, int hin, int hout, const void* dy, void* dx, cudaStream_t st) {
     CudnnPlan& p = conv_plan(layer_id, c, N, hin, hout);
@@ -649,9 +661,10 @@ struct dp_engine {
     const float one = 1.f, zero = 0.f;
     const double fl = 2.0 * N * hout * hout * c.cout * c.k * c.k * c.cin;
     const double by = ((double)N * hin * hin * c.cin_pad + (double)N * hout * hout * c.cout + (double)c.cout * c.k * c.k * c.cin_pad) * es;
-    PROF(this, c.k == 7 ? "stem_conv_bwd" : "conv3x3_bwd", by, fl, st,
-         CUDNN_OK(cudnnConvolutionBackwardData(L.cudnn, &one, c.wdesc, c.w, p.ydesc, dy, c.cdesc, p.bwd_algo, L.lib_ws, lib_ws_bytes, &zero, p.xdesc, dx)));
-    ++launches;
+    run(c.k == 7 ? "stem_conv_bwd" : "conv3x3_bwd", by, fl, st, [&] {
+      CUDNN_OK(cudnnConvolutionBackwardData(L.cudnn, &one, c.wdesc, c.w, p.ydesc, dy, c.cdesc, p.bwd_algo, L.lib_ws, lib_ws_bytes, &zero, p.xdesc, dx));
+      return 1;
+    });
   }
 
   // ---- cublasLt GEMM (1x1 convolutions, NHWC) ---------------------------------------------
@@ -719,9 +732,10 @@ struct dp_engine {
       p.tuned = true;
     }
     const double by = ((double)rows * k + (double)rows * nout * (beta != 0.f ? 2 : 1) + (double)nout * k) * (mode >= 2 ? 4 : es);
-    PROF(this, mode == 0 ? "gemm1x1_fwd" : (mode == 1 ? "gemm1x1_bwd" : (mode == 2 ? "fc_fwd" : "fc_bwd")), by, 2.0 * rows * nout * k, st,
-         CUBLAS_OK(cublasLtMatmul(lt, p.op, &one, W, p.a, X, p.b, &beta, Cres ? Cres : D, p.c, D, p.c, &p.algo, L.lib_ws, lib_ws_bytes, st)));
-    ++launches;
+    run(mode == 0 ? "gemm1x1_fwd" : (mode == 1 ? "gemm1x1_bwd" : (mode == 2 ? "fc_fwd" : "fc_bwd")), by, 2.0 * rows * nout * k, st, [&] {
+      CUBLAS_OK(cublasLtMatmul(lt, p.op, &one, W, p.a, X, p.b, &beta, Cres ? Cres : D, p.c, D, p.c, &p.algo, L.lib_ws, lib_ws_bytes, st));
+      return 1;
+    });
   }
 
   // ---- weight gradients ----------------------------------------------------------------------
@@ -746,11 +760,12 @@ struct dp_engine {
     const size_t wn = (size_t)c.cout * c.k * c.k * c.cin_pad;
     const double fl = 2.0 * N * hout * hout * c.cout * c.k * c.k * c.cin;
     const double by = ((double)N * hin * hin * c.cin_pad + (double)N * hout * hout * c.cout) * es + (double)wn * 8;
-    PROF(this, c.k == 7 ? "stem_wgrad" : "conv3x3_wgrad", by, fl, st,
-         CUDNN_OK(cudnnConvolutionBackwardFilter(L.cudnn, &one, p.xdesc, x, p.ydesc, dy, c.cdesc, p.wgd_algo, L.lib_ws, lib_ws_bytes,
-                                                 bf16 ? &zero : &one, c.wdesc, bf16 ? L.wg_half : (void*)acc)));
-    ++launches;
-    if (bf16) { dp::launch_add_bf16(L.wg_half, acc, wn, st); KERNEL_OK(); ++launches; }
+    run(c.k == 7 ? "stem_wgrad" : "conv3x3_wgrad", by, fl, st, [&] {
+      CUDNN_OK(cudnnConvolutionBackwardFilter(L.cudnn, &one, p.xdesc, x, p.ydesc, dy, c.cdesc, p.wgd_algo, L.lib_ws, lib_ws_bytes,
+                                              bf16 ? &zero : &one, c.wdesc, bf16 ? L.wg_half : (void*)acc));
+      return 1;
+    });
+    if (bf16) run(st, [&] { return dp::launch_add_bf16(L.wg_half, acc, wn, st); });
   }
   // 1x1 convolutions and the fc layer: D[cout][cin] (fp32) += dY^T X over `rows` pixels.  Column-major view:
   // D [cin x cout] = X [cin x rows] * (dY [cout x rows])^T.  head: fp32 operands and math (the fc layer is fp32).
@@ -782,20 +797,20 @@ struct dp_engine {
     GemmPlan& p = it->second;
     const float one = 1.f;
     const double by = ((double)rows * (cin + cout)) * (head ? 4 : es) + (double)cin * cout * 8;
-    PROF(this, head ? "fc_wgrad" : "gemm1x1_wgrad", by, 2.0 * rows * cout * cin, st,
-         CUBLAS_OK(cublasLtMatmul(lt, p.op, &one, X, p.a, dY, p.b, &one, D, p.c, D, p.c, &p.algo, L.lib_ws, lib_ws_bytes, st)));
-    ++launches;
+    run(head ? "fc_wgrad" : "gemm1x1_wgrad", by, 2.0 * rows * cout * cin, st, [&] {
+      CUBLAS_OK(cublasLtMatmul(lt, p.op, &one, X, p.a, dY, p.b, &one, D, p.c, D, p.c, &p.algo, L.lib_ws, lib_ws_bytes, st));
+      return 1;
+    });
   }
   // GroupNorm affine gradients of one norm: dy at its (ReLU) output, x its input, stats the forward's
   void gn_wgrad(const Lane& L, const GNW& g, const void* dy, const void* x, const float* stats, int N, int P, cudaStream_t st) {
-    PROF(this, "gn_affine_wgrad", 2.0 * N * P * g.C * es + (double)N * 2 * g.C * 8, 0, st, {
-      dp::launch_gn_affine_partial(dy, x, g.gamma, g.beta, stats, L.wg_partial, N, P, g.C, bf16, st);
-      dp::launch_colsum_add(L.wg_partial, acc_of(L, g.pid), N, 2 * g.C, st);
-    }); KERNEL_OK(); launches += 2;
+    run("gn_affine_wgrad", 2.0 * N * P * g.C * es + (double)N * 2 * g.C * 8, 0, st, [&] {
+      const int n = dp::launch_gn_affine_partial(dy, x, g.gamma, g.beta, stats, L.wg_partial, N, P, g.C, bf16, st);
+      return n + dp::launch_colsum_add(L.wg_partial, acc_of(L, g.pid), N, 2 * g.C, st);
+    });
   }
   void gn_apply(const GNW& g, const void* x, const float* stats, void* y, int N, int P, cudaStream_t st) {
-    PROF(this, "gn_apply_wgrad", 2.0 * N * P * g.C * es, 0, st, dp::launch_gn_apply(x, y, g.gamma, g.beta, stats, N, P, g.C, bf16, st));
-    KERNEL_OK(); ++launches;
+    run("gn_apply_wgrad", 2.0 * N * P * g.C * es, 0, st, [&] { return dp::launch_gn_apply(x, y, g.gamma, g.beta, stats, N, P, g.C, bf16, st); });
   }
 
   // FusedReduce: the stem dgrad fused with the masked EOT reduce (K1^T) of samples [n0, n0 + N) into G.
@@ -843,7 +858,7 @@ struct dp_engine {
     }
     void load(cudaStream_t st) {   // after new raw weights
       e->standardize(conv, st);
-      if (fwd == FWD_OWN) { dp::launch_stem_pack(conv.w, w_kn, conv.cin_pad, st); KERNEL_OK(); }
+      if (fwd == FWD_OWN) e->run(st, [&] { return dp::launch_stem_pack(conv.w, w_kn, conv.cin_pad, st); });
     }
     // Does the backward of a chunk expanded from `in` end in the fused K1^T (backward() given a FusedReduce)?  The fused
     // kernels have no affine (warped) variant.
@@ -856,38 +871,37 @@ struct dp_engine {
       for (int n0 = 0; n0 < N; n0 += SUB)
         f(std::min(SUB, N - n0), (char*)x + (size_t)n0 * H * H * x_ch * e->es, (char*)y + (size_t)n0 * hs * hs * STEM_CH * e->es);
     }
-    // the own kernels and the max-pool, also behind the op-level test hooks
-    void own_forward(const void* input, void* out, int N, cudaStream_t st) const {
-      dp::launch_stem_forward(input, w_kn, out, N, e->H, e->H, st); KERNEL_OK(); ++e->launches;
+    // the own kernels and the max-pool, also behind the op-level test hooks; each returns its launch count (run())
+    int own_forward(const void* input, void* out, int N, cudaStream_t st) const {
+      return dp::launch_stem_forward(input, w_kn, out, N, e->H, e->H, st);
     }
     // ConstantPad2d(1, 0) + MaxPool2d(3, 2) of x [N,hs,hs,C] into y [N,hs/2,hs/2,C] (argmax: null or [N,hs/2,hs/2,C])
-    void pool_forward(const void* x, void* y, int8_t* amax, int N, int hs, int C, cudaStream_t st) const {
-      dp::launch_maxpool_forward(x, y, amax, N, hs, hs, C, e->bf16, st); KERNEL_OK(); ++e->launches;
+    int pool_forward(const void* x, void* y, int8_t* amax, int N, int hs, int C, cudaStream_t st) const {
+      return dp::launch_maxpool_forward(x, y, amax, N, hs, hs, C, e->bf16, st);
     }
-    void pool_backward(const void* dy, const int8_t* amax, void* dx, int N, int hs, int C, cudaStream_t st) const {
-      dp::launch_maxpool_backward(dy, amax, dx, N, hs, hs, C, e->bf16, st); KERNEL_OK(); ++e->launches;
+    int pool_backward(const void* dy, const int8_t* amax, void* dx, int N, int hs, int C, cudaStream_t st) const {
+      return dp::launch_maxpool_backward(dy, amax, dx, N, hs, hs, C, e->bf16, st);
     }
-    void own_wgrad(const void* input, const void* dY, float* partial, float* acc, int N, int cin_pad, cudaStream_t st) const {
-      dp::launch_stem_wgrad(input, dY, partial, acc, N, e->H, e->H, cin_pad, st); KERNEL_OK(); e->launches += 2;
+    int own_wgrad(const void* input, const void* dY, float* partial, float* acc, int N, int cin_pad, cudaStream_t st) const {
+      return dp::launch_stem_wgrad(input, dY, partial, acc, N, e->H, e->H, cin_pad, st);
     }
-    void fused_reduce(const void* dY, const FusedReduce& fr, int N, cudaStream_t st) const {
-      dp::launch_stem_bwd_reduce(dY, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st); KERNEL_OK(); ++e->launches;
+    int fused_reduce(const void* dY, const FusedReduce& fr, int N, cudaStream_t st) const {
+      return dp::launch_stem_bwd_reduce(dY, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st);
     }
-    void fused_pool_reduce(const void* dpool, const int8_t* amax, const FusedReduce& fr, int N, cudaStream_t st) const {
-      dp::launch_stem_bwd_pool_reduce(dpool, amax, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st);
-      KERNEL_OK(); ++e->launches;
+    int fused_pool_reduce(const void* dpool, const int8_t* amax, const FusedReduce& fr, int N, cudaStream_t st) const {
+      return dp::launch_stem_bwd_pool_reduce(dpool, amax, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st);
     }
     // input [N,H,H,in_ch] -> conv -> max-pool into L.x0 (train: keep the argmax for the backward)
     void forward(const Lane& L, int N, const void* input, bool train, cudaStream_t st) const {
       const int H = e->H, hs = e->Hs(), hp = e->Hp();
       if (fwd == FWD_OWN) {
-        PROF(e, "stem_conv_fwd", ((double)N * H * H * 3 + (double)N * hs * hs * STEM_CH) * e->es, 2.0 * N * hs * hs * STEM_CH * 147, st,
-             own_forward(input, L.act, N, st));
+        e->run("stem_conv_fwd", ((double)N * H * H * 3 + (double)N * hs * hs * STEM_CH) * e->es, 2.0 * N * hs * hs * STEM_CH * 147, st,
+               [&] { return own_forward(input, L.act, N, st); });
       } else {
         cudnn_slices(N, input, in_ch, L.act, [&](int n, char* x, char* y) { e->conv_fwd(L, 0, conv, n, H, hs, x, y, st); });
       }
-      PROF(e, "maxpool_fwd", (double)N * (hs * hs + hp * hp) * STEM_CH * e->es, 0, st,
-           pool_forward(L.act, L.x0, train ? L.pool_amax : nullptr, N, hs, STEM_CH, st));
+      e->run("maxpool_fwd", (double)N * (hs * hs + hp * hp) * STEM_CH * e->es, 0, st,
+             [&] { return pool_forward(L.act, L.x0, train ? L.pool_amax : nullptr, N, hs, STEM_CH, st); });
     }
     // d_x0: the gradient at the max-pool output.  Max-pool backward, the stem's weight gradient when wg wants it, then
     // the dgrad, or the fused reduce when fr is given.  Returns d/d(input) ([N,H,H,dx_ch] in L.g[2]), or null when
@@ -899,24 +913,24 @@ struct dp_engine {
       if (wg && !wg->need_dx && !want_w) return nullptr;
       if (fr && bwd == END_FUSED_POOL_REDUCE && !wg) {
         // max-pool backward + stem dgrad + masked EOT reduce in one kernel: neither d_stem nor d/d(input) is written
-        PROF(e, "stem_bwd_reduce", (double)N * (hs / 2) * (hs / 2) * STEM_CH * (e->es + 1) + 3.0 * H * H * 4 * (double)N / fr->S,
-             2.0 * N * hs * hs * STEM_CH * 147, st, fused_pool_reduce(d_x0, L.pool_amax, *fr, N, st));
+        e->run("stem_bwd_reduce", (double)N * (hs / 2) * (hs / 2) * STEM_CH * (e->es + 1) + 3.0 * H * H * 4 * (double)N / fr->S,
+               2.0 * N * hs * hs * STEM_CH * 147, st, [&] { return fused_pool_reduce(d_x0, L.pool_amax, *fr, N, st); });
         return nullptr;
       }
-      PROF(e, "maxpool_bwd", (double)N * (hs * hs + (hs / 2) * (hs / 2)) * STEM_CH * e->es, 0, st,
-           pool_backward(d_x0, L.pool_amax, GB, N, hs, STEM_CH, st));
+      e->run("maxpool_bwd", (double)N * (hs * hs + (hs / 2) * (hs / 2)) * STEM_CH * e->es, 0, st,
+             [&] { return pool_backward(d_x0, L.pool_amax, GB, N, hs, STEM_CH, st); });
       if (want_w) {                                                                // dY = the max-pool adjoint (GB)
         float* const acc = e->acc_of(L, conv.pid);
         if (wgrad == WG_OWN)
-          PROF(e, "stem_wgrad", (double)N * (H * H * 3 + hs * hs * STEM_CH) * e->es, 2.0 * N * hs * hs * STEM_CH * 147, st,
-               own_wgrad(wg->input, GB, L.wg_partial, acc, N, conv.cin_pad, st));
+          e->run("stem_wgrad", (double)N * (H * H * 3 + hs * hs * STEM_CH) * e->es, 2.0 * N * hs * hs * STEM_CH * 147, st,
+                 [&] { return own_wgrad(wg->input, GB, L.wg_partial, acc, N, conv.cin_pad, st); });
         else
           cudnn_slices(N, wg->input, in_ch, GB, [&](int n, char* x, char* y) { e->conv_wgrad(L, 0, conv, n, H, hs, x, y, acc, st); });
         if (!wg->need_dx) return nullptr;
       }
       if (fr) {
-        PROF(e, "stem_bwd_reduce", (double)N * hs * hs * STEM_CH * e->es + 3.0 * H * H * 4 * (double)N / fr->S,
-             2.0 * N * hs * hs * STEM_CH * 147, st, fused_reduce(GB, *fr, N, st));
+        e->run("stem_bwd_reduce", (double)N * hs * hs * STEM_CH * e->es + 3.0 * H * H * 4 * (double)N / fr->S,
+               2.0 * N * hs * hs * STEM_CH * 147, st, [&] { return fused_reduce(GB, *fr, N, st); });
         return nullptr;
       }
       cudnn_slices(N, GC, dx_ch, GB, [&](int n, char* x, char* y) { e->conv_bwd(L, 0, conv, n, H, hs, y, x, st); });
@@ -945,52 +959,46 @@ struct dp_engine {
       const bool fuse1 = fused_gemm && !b.has_ds && dp::gn_gemm_supported(pin_, b.cin, b.mid);
       const bool fuse3 = fused_gemm && dp::gn_gemm_supported(pout, b.mid, b.cout);
       // xp = relu(gn1(cur))
-      if (fuse1) {
-        PROF(this, "gn_stats", 1.0 * N * pin_ * b.cin * es, 0, st, dp::launch_gn_stats(cur, L.gn_partial, s.st1, N, pin_, b.cin, bf16, st));
-        KERNEL_OK(); launches += 2;
-      } else {
-        PROF(this, "gn_relu_fwd", 2.0 * N * pin_ * b.cin * es, 0, st,
-             dp::launch_gn_relu_forward(cur, act, b.n1.gamma, b.n1.beta, L.gn_partial, s.st1, N, pin_, b.cin, bf16, st)); KERNEL_OK(); launches += 2;
-      }
+      if (fuse1)
+        run("gn_stats", 1.0 * N * pin_ * b.cin * es, 0, st, [&] { return dp::launch_gn_stats(cur, L.gn_partial, s.st1, N, pin_, b.cin, bf16, st); });
+      else
+        run("gn_relu_fwd", 2.0 * N * pin_ * b.cin * es, 0, st,
+            [&] { return dp::launch_gn_relu_forward(cur, act, b.n1.gamma, b.n1.beta, L.gn_partial, s.st1, N, pin_, b.cin, bf16, st); });
       const void* shortcut = cur;
       if (b.has_ds) {
         const void* src = act;
         if (b.stride == 2) {
-          PROF(this, "subsample", 2.0 * N * pout * b.cin * es, 0, st, dp::launch_subsample2(act, L.act2, N, b.hin, b.hin, b.cin, bf16, st));
-          KERNEL_OK(); ++launches; src = L.act2;
+          run("subsample", 2.0 * N * pout * b.cin * es, 0, st, [&] { return dp::launch_subsample2(act, L.act2, N, b.hin, b.hin, b.cin, bf16, st); });
+          src = L.act2;
         }
         gemm(L, N * pout, b.cout, b.cin, 0, b.ds.w, src, nullptr, 0.f, s.out, st);
         shortcut = s.out;
       }
-      if (fuse1) {
-        PROF(this, "gn_gemm1x1_fwd", ((double)N * pin_ * (b.cin + b.mid) + (double)b.mid * b.cin) * es, 2.0 * N * pin_ * b.mid * b.cin, st,
-             dp::launch_gn_gemm_forward(cur, b.c1p, s.st1, b.n1.gamma, b.n1.beta, nullptr, s.h1, N, pin_, b.cin, b.mid, st));
-        KERNEL_OK(); ++launches;
-      } else {
+      if (fuse1)
+        run("gn_gemm1x1_fwd", ((double)N * pin_ * (b.cin + b.mid) + (double)b.mid * b.cin) * es, 2.0 * N * pin_ * b.mid * b.cin, st,
+            [&] { return dp::launch_gn_gemm_forward(cur, b.c1p, s.st1, b.n1.gamma, b.n1.beta, nullptr, s.h1, N, pin_, b.cin, b.mid, st); });
+      else
         gemm(L, N * pin_, b.mid, b.cin, 0, b.c1.w, act, nullptr, 0.f, s.h1, st);
-      }
-      PROF(this, "gn_relu_fwd", 2.0 * N * pin_ * b.mid * es, 0, st,
-           dp::launch_gn_relu_forward(s.h1, act, b.n2.gamma, b.n2.beta, L.gn_partial, s.st2, N, pin_, b.mid, bf16, st)); KERNEL_OK(); launches += 2;
+      run("gn_relu_fwd", 2.0 * N * pin_ * b.mid * es, 0, st,
+          [&] { return dp::launch_gn_relu_forward(s.h1, act, b.n2.gamma, b.n2.beta, L.gn_partial, s.st2, N, pin_, b.mid, bf16, st); });
       conv_fwd(L, lid, b.c2, N, b.hin, b.hout, act, s.h2, st);
       if (fuse3) {
-        PROF(this, "gn_stats", 1.0 * N * pout * b.mid * es, 0, st, dp::launch_gn_stats(s.h2, L.gn_partial, s.st3, N, pout, b.mid, bf16, st));
-        KERNEL_OK(); launches += 2;
-        PROF(this, "gn_gemm1x1_fwd", ((double)N * pout * (b.mid + 2.0 * b.cout) + (double)b.cout * b.mid) * es, 2.0 * N * pout * b.cout * b.mid, st,
-             dp::launch_gn_gemm_forward(s.h2, b.c3p, s.st3, b.n3.gamma, b.n3.beta, shortcut, s.out, N, pout, b.mid, b.cout, st));
-        KERNEL_OK(); ++launches;
+        run("gn_stats", 1.0 * N * pout * b.mid * es, 0, st, [&] { return dp::launch_gn_stats(s.h2, L.gn_partial, s.st3, N, pout, b.mid, bf16, st); });
+        run("gn_gemm1x1_fwd", ((double)N * pout * (b.mid + 2.0 * b.cout) + (double)b.cout * b.mid) * es, 2.0 * N * pout * b.cout * b.mid, st,
+            [&] { return dp::launch_gn_gemm_forward(s.h2, b.c3p, s.st3, b.n3.gamma, b.n3.beta, shortcut, s.out, N, pout, b.mid, b.cout, st); });
       } else {
-        PROF(this, "gn_relu_fwd", 2.0 * N * pout * b.mid * es, 0, st,
-             dp::launch_gn_relu_forward(s.h2, act, b.n3.gamma, b.n3.beta, L.gn_partial, s.st3, N, pout, b.mid, bf16, st)); KERNEL_OK(); launches += 2;
+        run("gn_relu_fwd", 2.0 * N * pout * b.mid * es, 0, st,
+            [&] { return dp::launch_gn_relu_forward(s.h2, act, b.n3.gamma, b.n3.beta, L.gn_partial, s.st3, N, pout, b.mid, bf16, st); });
         gemm(L, N * pout, b.cout, b.mid, 0, b.c3.w, act, shortcut, 1.f, s.out, st);   // + shortcut fused as C operand
       }
       cur = s.out;
     }
     const Block& last = blocks.back();
     const int pl = last.hout * last.hout;
-    PROF(this, "head_fwd", (double)N * pl * last.cout * es, 2.0 * N * last.cout * K, st, {
-      dp::launch_gn_stats(cur, L.gn_partial, L.head_stats, N, pl, last.cout, bf16, st);
-      dp::launch_head_pool(cur, head_gn.gamma, head_gn.beta, L.head_stats, L.pooled, N, pl, last.cout, bf16, st);
-    }); KERNEL_OK(); launches += 3;
+    run("head_fwd", (double)N * pl * last.cout * es, 2.0 * N * last.cout * K, st, [&] {
+      const int n = dp::launch_gn_stats(cur, L.gn_partial, L.head_stats, N, pl, last.cout, bf16, st);
+      return n + dp::launch_head_pool(cur, head_gn.gamma, head_gn.beta, L.head_stats, L.pooled, N, pl, last.cout, bf16, st);
+    });
     gemm(L, N, K, last.cout, 2, fc_w, L.pooled, nullptr, 0.f, L.logits, st);   // logits = pooled * Wfc^T + b (fp32)
   }
 
@@ -1011,17 +1019,14 @@ struct dp_engine {
     if (W) {                                                                     // fc: dW += dlogits^T pooled, db += sum dlogits
       const int fw = wparam_idx.at("head.fc.weight"), fb = wparam_idx.at("head.fc.bias");
       if (want[fw]) wgrad_gemm(L, N, K, last.cout, L.pooled, dlog, acc_of(L, fw), true, st);
-      if (want[fb]) {
-        PROF(this, "fc_wgrad", (double)N * K * 4, 0, st, dp::launch_colsum_add(dlog, acc_of(L, fb), N, K, st));
-        KERNEL_OK(); ++launches;
-      }
+      if (want[fb]) run("fc_wgrad", (double)N * K * 4, 0, st, [&] { return dp::launch_colsum_add(dlog, acc_of(L, fb), N, K, st); });
       if (!wg->need_dx && wg->lo >= (int)blocks.size() && !want_gn(head_gn)) return nullptr;
     }
     gemm(L, N, last.cout, K, 3, fc_w, dlog, nullptr, 0.f, L.dpooled, st);      // dpooled = dlogits * Wfc (fp32)
-    PROF(this, "head_bwd", 2.0 * N * pl * last.cout * es, 0, st, {
-      dp::launch_pool_grad_bcast(L.dpooled, GB, N, pl, last.cout, bf16, st);
-      dp::launch_gn_relu_backward(GB, last_out, nullptr, GA, head_gn.gamma, head_gn.beta, L.head_stats, gn_partial, N, pl, last.cout, bf16, st, head_gn.pos);
-    }); KERNEL_OK(); launches += 3;
+    run("head_bwd", 2.0 * N * pl * last.cout * es, 0, st, [&] {
+      const int n = dp::launch_pool_grad_bcast(L.dpooled, GB, N, pl, last.cout, bf16, st);
+      return n + dp::launch_gn_relu_backward(GB, last_out, nullptr, GA, head_gn.gamma, head_gn.beta, L.head_stats, gn_partial, N, pl, last.cout, bf16, st, head_gn.pos);
+    });
     if (W && want_gn(head_gn)) gn_wgrad(L, head_gn, GB, last_out, L.head_stats, N, pl, st);
     const int lo = W && !wg->need_dx ? wg->lo : 0;
     for (int bi = (int)blocks.size() - 1; bi >= lo; --bi) {
@@ -1037,24 +1042,24 @@ struct dp_engine {
       }
       // d_a3 = d_out * W3
       gemm(L, N * pout, b.mid, b.cout, 1, b.c3.w, GA, nullptr, 0.f, GB, st);
-      PROF(this, "gn_relu_bwd", 3.0 * N * pout * b.mid * es, 0, st,
-           dp::launch_gn_relu_backward(GB, s.h2, nullptr, GC, b.n3.gamma, b.n3.beta, s.st3, gn_partial, N, pout, b.mid, bf16, st, b.n3.pos)); KERNEL_OK(); launches += 2;
+      run("gn_relu_bwd", 3.0 * N * pout * b.mid * es, 0, st,
+          [&] { return dp::launch_gn_relu_backward(GB, s.h2, nullptr, GC, b.n3.gamma, b.n3.beta, s.st3, gn_partial, N, pout, b.mid, bf16, st, b.n3.pos); });
       if (W && want_gn(b.n3)) gn_wgrad(L, b.n3, GB, s.h2, s.st3, N, pout, st);
       if (W && want_conv(b.c2)) {                                                // conv2: dY = GC, X = relu(gn2(h1))
         gn_apply(b.n2, s.h1, s.st2, act, N, pin_, st);
         conv_wgrad(L, lid, b.c2, N, b.hin, b.hout, act, GC, acc_of(L, b.c2.pid), st);
       }
       conv_bwd(L, lid, b.c2, N, b.hin, b.hout, GC, GB, st);
-      PROF(this, "gn_relu_bwd", 3.0 * N * pin_ * b.mid * es, 0, st,
-           dp::launch_gn_relu_backward(GB, s.h1, nullptr, GC, b.n2.gamma, b.n2.beta, s.st2, gn_partial, N, pin_, b.mid, bf16, st, b.n2.pos)); KERNEL_OK(); launches += 2;
+      run("gn_relu_bwd", 3.0 * N * pin_ * b.mid * es, 0, st,
+          [&] { return dp::launch_gn_relu_backward(GB, s.h1, nullptr, GC, b.n2.gamma, b.n2.beta, s.st2, gn_partial, N, pin_, b.mid, bf16, st, b.n2.pos); });
       if (W && want_gn(b.n2)) gn_wgrad(L, b.n2, GB, s.h1, s.st2, N, pin_, st);
       if (W && (want_conv(b.c1) || (b.has_ds && want_conv(b.ds)))) gn_apply(b.n1, xin, s.st1, act, N, pin_, st);   // relu(gn1(xin))
       if (W && want_conv(b.c1)) wgrad_gemm(L, N * pin_, b.mid, b.cin, act, GC, acc_of(L, b.c1.pid), false, st);   // conv1: dY = GC
       if (W && b.has_ds && want_conv(b.ds)) {                                    // downsample: dY = GA, X = (subsampled) act
         const void* src = act;
         if (b.stride == 2) {
-          PROF(this, "subsample", 2.0 * N * pout * b.cin * es, 0, st, dp::launch_subsample2(act, L.act2, N, b.hin, b.hin, b.cin, bf16, st));
-          KERNEL_OK(); ++launches; src = L.act2;
+          run("subsample", 2.0 * N * pout * b.cin * es, 0, st, [&] { return dp::launch_subsample2(act, L.act2, N, b.hin, b.hin, b.cin, bf16, st); });
+          src = L.act2;
         }
         wgrad_gemm(L, N * pout, b.cout, b.cin, src, GA, acc_of(L, b.ds.pid), false, st);
       }
@@ -1062,15 +1067,15 @@ struct dp_engine {
       if (b.has_ds) {
         if (b.stride == 2) {
           gemm(L, N * pout, b.cin, b.cout, 1, b.ds.w, GA, nullptr, 0.f, GC, st);
-          PROF(this, "subsample", 3.0 * N * pout * b.cin * es, 0, st, dp::launch_subsample2_adjoint_add(GC, GB, N, b.hin, b.hin, b.cin, bf16, st)); KERNEL_OK(); ++launches;
+          run("subsample", 3.0 * N * pout * b.cin * es, 0, st, [&] { return dp::launch_subsample2_adjoint_add(GC, GB, N, b.hin, b.hin, b.cin, bf16, st); });
         } else {
           gemm(L, N * pout, b.cin, b.cout, 1, b.ds.w, GA, nullptr, 1.f, GB, st); // accumulate
         }
-        PROF(this, "gn_relu_bwd", 3.0 * N * pin_ * b.cin * es, 0, st,
-             dp::launch_gn_relu_backward(GB, xin, nullptr, GD, b.n1.gamma, b.n1.beta, s.st1, gn_partial, N, pin_, b.cin, bf16, st, b.n1.pos)); KERNEL_OK(); launches += 2;
+        run("gn_relu_bwd", 3.0 * N * pin_ * b.cin * es, 0, st,
+            [&] { return dp::launch_gn_relu_backward(GB, xin, nullptr, GD, b.n1.gamma, b.n1.beta, s.st1, gn_partial, N, pin_, b.cin, bf16, st, b.n1.pos); });
       } else {
-        PROF(this, "gn_relu_bwd", 4.0 * N * pin_ * b.cin * es, 0, st,
-             dp::launch_gn_relu_backward(GB, xin, GA, GD, b.n1.gamma, b.n1.beta, s.st1, gn_partial, N, pin_, b.cin, bf16, st, b.n1.pos)); KERNEL_OK(); launches += 2;
+        run("gn_relu_bwd", 4.0 * N * pin_ * b.cin * es, 0, st,
+            [&] { return dp::launch_gn_relu_backward(GB, xin, GA, GD, b.n1.gamma, b.n1.beta, s.st1, gn_partial, N, pin_, b.cin, bf16, st, b.n1.pos); });
       }
       if (W && want_gn(b.n1)) gn_wgrad(L, b.n1, GB, xin, s.st1, N, pin_, st);
       std::swap(GA, GD);
@@ -1102,11 +1107,11 @@ struct dp_engine {
     const bool fused = in.x != nullptr;
     const double bytes = (double)n * H * H * 3 * es + (fused ? 7.0 : 3.0) * H * H * 4 * (double)n / in.S;
     if (in.xf)
-      PROF(this, "expand_affine", bytes, 0, st, dp::launch_expand_affine(in.img, in.xf, in.rects, dst, in.S, n0, n, H, H, stem.in_ch, bf16, st));
+      run("expand_affine", bytes, 0, st, [&] { return dp::launch_expand_affine(in.img, in.xf, in.rects, dst, in.S, n0, n, H, H, stem.in_ch, bf16, st); });
     else
-      PROF(this, "expand_k1", bytes, 0, st,
-           dp::launch_expand(in.img, in.x, in.mask, in.pattern, in.scale, in.rects, dst, in.B, in.S, n0, n, H, H, stem.in_ch, bf16, fused, num_sms, st));
-    KERNEL_OK(); ++launches;
+      run("expand_k1", bytes, 0, st, [&] {
+        return dp::launch_expand(in.img, in.x, in.mask, in.pattern, in.scale, in.rects, dst, in.B, in.S, n0, n, H, H, stem.in_ch, bf16, fused, num_sms, st);
+      });
   }
   // The network input of samples [n0, n0 + n): their slice of net_in_all when K1 ran once for the whole call, otherwise
   // K1 into the lane's net_in.
@@ -1125,10 +1130,9 @@ struct dp_engine {
     if (!G || fuse) return;
     const double bytes = (double)n * H * H * 3 * es + 3.0 * H * H * 4 * (double)n / in.S;
     if (in.xf)
-      PROF(this, "reduce_affine", bytes, 0, st, dp::launch_reduce_affine(dx, in.img, in.xf, in.rects, G, in.S, n0, n, H, H, stem.dx_ch, bf16, st));
+      run("reduce_affine", bytes, 0, st, [&] { return dp::launch_reduce_affine(dx, in.img, in.xf, in.rects, G, in.S, n0, n, H, H, stem.dx_ch, bf16, st); });
     else
-      PROF(this, "reduce_k1t", bytes, 0, st, dp::launch_reduce(dx, in.rects, G, in.B, in.S, n0, n, H, H, stem.dx_ch, bf16, st));
-    KERNEL_OK(); ++launches;
+      run("reduce_k1t", bytes, 0, st, [&] { return dp::launch_reduce(dx, in.rects, G, in.B, in.S, n0, n, H, H, stem.dx_ch, bf16, st); });
   }
 
   // ---- helpers for the attack entry points --------------------------------------------------
@@ -1186,18 +1190,29 @@ struct LaneWalk {
 // =========================================================================================
 // C ABI
 // =========================================================================================
-#define DP_TRY try {
-#define DP_CATCH                                   \
-  }                                                \
-  catch (const std::exception& ex) {               \
-    g_last_error = ex.what();                      \
-    return 1;                                      \
-  }                                                \
-  catch (...) {                                    \
-    g_last_error = "unknown C++ exception";        \
-    return 1;                                      \
-  }                                                \
+// Every entry point returns 0, or 1 with the message of what f() threw in dp_last_error.
+template <class F>
+static int32_t guarded(F&& f) {
+  try {
+    f();
+  } catch (const std::exception& ex) {
+    g_last_error = ex.what();
+    return 1;
+  } catch (...) {
+    g_last_error = "unknown C++ exception";
+    return 1;
+  }
   return 0;
+}
+// The same for an entry point on engine e: e is not null and its device is current when f(stream) runs.
+template <class F>
+static int32_t on_engine(dp_engine* e, void* stream, F&& f) {
+  return guarded([&] {
+    if (!e) fail("null engine");
+    CUDA_OK(cudaSetDevice(e->cfg.device));
+    f((cudaStream_t)stream);
+  });
+}
 
 extern "C" {
 
@@ -1205,43 +1220,43 @@ int32_t dp_abi_version(void) { return DP_ABI_VERSION; }
 const char* dp_last_error(void) { return g_last_error.c_str(); }
 
 int32_t dp_engine_create(const dp_config* cfg, dp_engine** out) {
-  DP_TRY
-  if (!cfg || !out) fail("null argument");
-  if (cfg->img % 56 != 0 || cfg->img < 56) fail("img=%d must be a positive multiple of 56", cfg->img);
-  if (cfg->chunk < 1) fail("chunk must be >= 1");
-  if (cfg->max_images < 1) fail("max_images must be >= 1");
-  if (cfg->precision < 0 || cfg->precision > 2) fail("unknown precision %d", cfg->precision);
-  int ndev = 0;
-  CUDA_OK(cudaGetDeviceCount(&ndev));
-  if (cfg->device < 0 || cfg->device >= ndev) fail("device %d not present (%d CUDA devices)", cfg->device, ndev);
-  CUDA_OK(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop;
-  CUDA_OK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 9 || prop.minor != 0) fail("device %d is sm_%d%d; this engine is built for sm_90a (H100) only", cfg->device, prop.major, prop.minor);
-  dp_engine* e = new dp_engine();
-  try {
-    e->cfg = *cfg;
-    e->num_sms = prop.multiProcessorCount;
-    e->bf16 = (cfg->precision == DP_PREC_BF16);
-    e->es = e->bf16 ? 2 : 4;
-    e->stem.configure(e);
-    const char* fg_env = getenv("DORPATCH_FUSED_GEMM");
-    e->fused_gemm = e->bf16 && fg_env && atoi(fg_env) != 0;   // validated (tests/test_gpu_ops.py, test_gpu_fused_gemm.py) but slower than cublasLt + GroupNorm: off unless asked for
-    if (const char* g_env = getenv("DORPATCH_GRAPH")) e->graphs_on = atoi(g_env) != 0;
-    if (const char* k_env = getenv("DORPATCH_K1_WHOLE_MB")) e->k1_whole_max = (size_t)std::max(0, atoi(k_env)) << 20;
-    e->H = cfg->img; e->K = cfg->n_classes; e->chunk = cfg->chunk;
-    e->cudnn_dt = e->bf16 ? CUDNN_DATA_BFLOAT16 : CUDNN_DATA_FLOAT;
-    e->cuda_dt = e->bf16 ? CUDA_R_16BF : CUDA_R_32F;
-    e->lt_compute = (cfg->precision == DP_PREC_TF32) ? CUBLAS_COMPUTE_32F_FAST_TF32 : CUBLAS_COMPUTE_32F;
-    CUBLAS_OK(cublasLtCreate(&e->lt));
-    e->build_arch();
-    e->allocate();
-  } catch (...) {
-    dp_engine_destroy(e);
-    throw;
-  }
-  *out = e;
-  DP_CATCH
+  return guarded([&] {
+    if (!cfg || !out) fail("null argument");
+    if (cfg->img % 56 != 0 || cfg->img < 56) fail("img=%d must be a positive multiple of 56", cfg->img);
+    if (cfg->chunk < 1) fail("chunk must be >= 1");
+    if (cfg->max_images < 1) fail("max_images must be >= 1");
+    if (cfg->precision < 0 || cfg->precision > 2) fail("unknown precision %d", cfg->precision);
+    int ndev = 0;
+    CUDA_OK(cudaGetDeviceCount(&ndev));
+    if (cfg->device < 0 || cfg->device >= ndev) fail("device %d not present (%d CUDA devices)", cfg->device, ndev);
+    CUDA_OK(cudaSetDevice(cfg->device));
+    cudaDeviceProp prop;
+    CUDA_OK(cudaGetDeviceProperties(&prop, cfg->device));
+    if (prop.major != 9 || prop.minor != 0) fail("device %d is sm_%d%d; this engine is built for sm_90a (H100) only", cfg->device, prop.major, prop.minor);
+    dp_engine* e = new dp_engine();
+    try {
+      e->cfg = *cfg;
+      e->num_sms = prop.multiProcessorCount;
+      e->bf16 = (cfg->precision == DP_PREC_BF16);
+      e->es = e->bf16 ? 2 : 4;
+      e->stem.configure(e);
+      const char* fg_env = getenv("DORPATCH_FUSED_GEMM");
+      e->fused_gemm = e->bf16 && fg_env && atoi(fg_env) != 0;   // validated (tests/test_gpu_ops.py, test_gpu_fused_gemm.py) but slower than cublasLt + GroupNorm: off unless asked for
+      if (const char* g_env = getenv("DORPATCH_GRAPH")) e->graphs_on = atoi(g_env) != 0;
+      if (const char* k_env = getenv("DORPATCH_K1_WHOLE_MB")) e->k1_whole_max = (size_t)std::max(0, atoi(k_env)) << 20;
+      e->H = cfg->img; e->K = cfg->n_classes; e->chunk = cfg->chunk;
+      e->cudnn_dt = e->bf16 ? CUDNN_DATA_BFLOAT16 : CUDNN_DATA_FLOAT;
+      e->cuda_dt = e->bf16 ? CUDA_R_16BF : CUDA_R_32F;
+      e->lt_compute = (cfg->precision == DP_PREC_TF32) ? CUBLAS_COMPUTE_32F_FAST_TF32 : CUBLAS_COMPUTE_32F;
+      CUBLAS_OK(cublasLtCreate(&e->lt));
+      e->build_arch();
+      e->allocate();
+    } catch (...) {
+      dp_engine_destroy(e);
+      throw;
+    }
+    *out = e;
+  });
 }
 
 void dp_engine_destroy(dp_engine* e) {
@@ -1288,20 +1303,16 @@ void dp_engine_destroy(dp_engine* e) {
 }
 
 int32_t dp_engine_load_weights(dp_engine* e, int32_t n, const char* const* names, const float* const* ptrs, const int64_t* numels) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  e->load_weights(n, names, ptrs, numels);
-  DP_CATCH
+  return on_engine(e, nullptr, [&](cudaStream_t) {
+    e->load_weights(n, names, ptrs, numels);
+  });
 }
 
 int32_t dp_engine_load_weights_dev(dp_engine* e, int32_t n, const char* const* names, const float* const* dev_ptrs,
                                    const int64_t* numels, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  e->load_weights_dev(n, names, dev_ptrs, numels, (cudaStream_t)stream);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    e->load_weights_dev(n, names, dev_ptrs, numels, st);
+  });
 }
 
 int64_t dp_engine_device_bytes(const dp_engine* e) { return e ? e->device_bytes : 0; }
@@ -1310,107 +1321,88 @@ int64_t dp_engine_graph_replays(const dp_engine* e) { return e ? e->graph_replay
 const char* dp_engine_graph_status(const dp_engine* e) { return e ? e->graph_msg.c_str() : ""; }
 
 int32_t dp_engine_profile(dp_engine* e, int32_t enable) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  e->prof_collect();
-  e->prof_on = enable != 0;
-  if (enable == 2) {   // reset
-    for (size_t i = 0; i < e->prof_ms.size(); ++i) { e->prof_ms[i] = 0; e->prof_bytes[i] = 0; e->prof_flops[i] = 0; e->prof_count[i] = 0; }
-  }
-  DP_CATCH
+  return on_engine(e, nullptr, [&](cudaStream_t) {
+    e->prof_collect();
+    e->prof_on = enable != 0;
+    if (enable == 2) {   // reset
+      for (size_t i = 0; i < e->prof_ms.size(); ++i) { e->prof_ms[i] = 0; e->prof_bytes[i] = 0; e->prof_flops[i] = 0; e->prof_count[i] = 0; }
+    }
+  });
 }
 
 int32_t dp_engine_profile_read(dp_engine* e, int32_t max_n, char* names, int32_t name_stride, double* ms, double* bytes,
                                double* flops, int64_t* counts, int32_t* n_out) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  e->prof_collect();
-  int n = (int)e->prof_names.size();
-  if (n > max_n) n = max_n;
-  for (int i = 0; i < n; ++i) {
-    snprintf(names + (size_t)i * name_stride, name_stride, "%s", e->prof_names[i].c_str());
-    ms[i] = e->prof_ms[i]; bytes[i] = e->prof_bytes[i]; flops[i] = e->prof_flops[i]; counts[i] = e->prof_count[i];
-  }
-  *n_out = n;
-  DP_CATCH
+  return on_engine(e, nullptr, [&](cudaStream_t) {
+    e->prof_collect();
+    int n = (int)e->prof_names.size();
+    if (n > max_n) n = max_n;
+    for (int i = 0; i < n; ++i) {
+      snprintf(names + (size_t)i * name_stride, name_stride, "%s", e->prof_names[i].c_str());
+      ms[i] = e->prof_ms[i]; bytes[i] = e->prof_bytes[i]; flops[i] = e->prof_flops[i]; counts[i] = e->prof_count[i];
+    }
+    *n_out = n;
+  });
 }
 
 int32_t dp_input_layout(const dp_engine* e, int32_t* c_pad, int32_t* elem_bytes) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (c_pad) *c_pad = e->stem.in_ch;
-  if (elem_bytes) *elem_bytes = (int32_t)e->es;
-  DP_CATCH
+  return guarded([&] {
+    if (!e) fail("null engine");
+    if (c_pad) *c_pad = e->stem.in_ch;
+    if (elem_bytes) *elem_bytes = (int32_t)e->es;
+  });
 }
 
 int32_t dp_paste(dp_engine* e, const float* x, const float* mask, const float* pattern, int32_t B, float eps,
                  float* adv_x_out, float* l2_host, float* scale_host, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  e->check_B(B);
-  cudaStream_t st = (cudaStream_t)stream;
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  // with an output buffer this is the stand-alone helper (utils.clip, main.py:140): it must not disturb the per-step
-  // state (adv_x, clip scale) a dp_attack_grad left behind for dp_attack_update; without one it IS the step's paste
-  float* l2d = adv_x_out ? e->helper_l2 : e->l2;
-  float* scd = adv_x_out ? e->helper_scale : e->scale;
-  dp::launch_paste(x, mask, pattern, adv_x_out ? adv_x_out : e->adv_x, l2d, scd, B, e->H, e->H, eps, st); KERNEL_OK(); ++e->launches;
-  if (l2_host) CUDA_OK(cudaMemcpyAsync(l2_host, l2d, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-  if (scale_host) CUDA_OK(cudaMemcpyAsync(scale_host, scd, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-  if (l2_host || scale_host) CUDA_OK(cudaStreamSynchronize(st));
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    e->check_B(B);
+    // with an output buffer this is the stand-alone helper (utils.clip, main.py:140): it must not disturb the per-step
+    // state (adv_x, clip scale) a dp_attack_grad left behind for dp_attack_update; without one it IS the step's paste
+    float* l2d = adv_x_out ? e->helper_l2 : e->l2;
+    float* scd = adv_x_out ? e->helper_scale : e->scale;
+    e->run(st, [&] { return dp::launch_paste(x, mask, pattern, adv_x_out ? adv_x_out : e->adv_x, l2d, scd, B, e->H, e->H, eps, st); });
+    if (l2_host) CUDA_OK(cudaMemcpyAsync(l2_host, l2d, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    if (scale_host) CUDA_OK(cudaMemcpyAsync(scale_host, scd, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    if (l2_host || scale_host) CUDA_OK(cudaStreamSynchronize(st));
+  });
 }
 
 int32_t dp_window_sum(dp_engine* e, const float* t, int32_t B, int32_t k, int32_t square, float* out_host, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  e->check_B(B);
-  if (k < 1 || e->H % k != 0) fail("window %d does not divide img %d", k, e->H);
-  cudaStream_t st = (cudaStream_t)stream;
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  const size_t n = (size_t)B * (e->H / k) * (e->H / k);
-  float* tmp = e->helper_ws;   // own scratch (never the structural-loss gradient the sign step reads)
-  dp::launch_window_sum(t, tmp, B, e->H, e->H, k, square != 0, st); KERNEL_OK(); ++e->launches;
-  CUDA_OK(cudaMemcpyAsync(out_host, tmp, n * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    e->check_B(B);
+    if (k < 1 || e->H % k != 0) fail("window %d does not divide img %d", k, e->H);
+    const size_t n = (size_t)B * (e->H / k) * (e->H / k);
+    float* tmp = e->helper_ws;   // own scratch (never the structural-loss gradient the sign step reads)
+    e->run(st, [&] { return dp::launch_window_sum(t, tmp, B, e->H, e->H, k, square != 0, st); });
+    CUDA_OK(cudaMemcpyAsync(out_host, tmp, n * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+  });
 }
 
 int32_t dp_expand(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host, void* out, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  cudaStream_t st = (cudaStream_t)stream;
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  const int N = B * S;
-  if (out == nullptr && N > e->chunk) fail("dp_expand: B*S=%d exceeds chunk=%d and no output buffer was given", N, e->chunk);
-  e->h2d_samples(rects_host, N, st);
-  e->launch_k1(dp_engine::EotIn::image(img, nullptr, rects_host ? e->rects_d : nullptr, B, S), 0, N, out ? out : e->lanes[0].net_in, st);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    const int N = B * S;
+    if (out == nullptr && N > e->chunk) fail("dp_expand: B*S=%d exceeds chunk=%d and no output buffer was given", N, e->chunk);
+    e->h2d_samples(rects_host, N, st);
+    e->launch_k1(dp_engine::EotIn::image(img, nullptr, rects_host ? e->rects_d : nullptr, B, S), 0, N, out ? out : e->lanes[0].net_in, st);
+  });
 }
 
 int32_t dp_expand_dev(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_dev, void* out, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (!out) fail("dp_expand_dev needs an output buffer");
-  cudaStream_t st = (cudaStream_t)stream;
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  e->launch_k1(dp_engine::EotIn::image(img, nullptr, rects_dev, B, S), 0, B * S, out, st);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!out) fail("dp_expand_dev needs an output buffer");
+    e->launch_k1(dp_engine::EotIn::image(img, nullptr, rects_dev, B, S), 0, B * S, out, st);
+  });
 }
 
 int32_t dp_expand_step_dev(dp_engine* e, const float* x, const float* mask, const float* pattern, int32_t B, int32_t S,
                            const int16_t* rects_dev, int32_t n0, int32_t n, void* out, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (!out || !x || !mask || !pattern) fail("dp_expand_step_dev: null pointer");
-  if (n0 < 0 || n < 1 || n0 + n > B * S) fail("dp_expand_step_dev: samples [%d, %d) outside [0, %d)", n0, n0 + n, B * S);
-  e->check_B(B);
-  cudaStream_t st = (cudaStream_t)stream;
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  e->launch_k1(dp_engine::EotIn::paste(x, mask, pattern, e->scale, rects_dev, B, S), n0, n, out, st);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!out || !x || !mask || !pattern) fail("dp_expand_step_dev: null pointer");
+    if (n0 < 0 || n < 1 || n0 + n > B * S) fail("dp_expand_step_dev: samples [%d, %d) outside [0, %d)", n0, n0 + n, B * S);
+    e->check_B(B);
+    e->launch_k1(dp_engine::EotIn::paste(x, mask, pattern, e->scale, rects_dev, B, S), n0, n, out, st);
+  });
 }
 
 int32_t dp_k1_samples_per_launch(const dp_engine* e, int32_t n_samples) {
@@ -1420,30 +1412,27 @@ int32_t dp_k1_samples_per_launch(const dp_engine* e, int32_t n_samples) {
 
 int32_t dp_predict(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host, int32_t* preds_host,
                    float* logits_host, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  NvtxRange nvtx_("dorpatch.predict");
-  cudaStream_t st = (cudaStream_t)stream;
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  const int N = B * S;
-  if (N < 1) fail("dp_predict: empty batch");
-  e->forward_clobbered();
-  e->h2d_samples(rects_host, N, st);
-  const dp_engine::EotIn in = dp_engine::EotIn::image(img, nullptr, rects_host ? e->rects_d : nullptr, B, S);
-  // forward-only scan (collect_failure, PatchCleanser): chunks alternate between the two lanes like dp_attack_grad
-  LaneWalk walk(e, st, N > e->chunk);
-  for (int n0 = 0, c = 0; n0 < N; n0 += e->chunk, ++c) {
-    const int n = std::min(e->chunk, N - n0);
-    const dp_engine::Lane& L = e->lanes[walk.lane_of(c)];
-    cudaStream_t const ls = walk.stream(walk.lane_of(c));
-    e->forward(L, n, e->chunk_input(L, in, n0, n, false, ls), false, ls);
-    dp::launch_argmax(L.logits, e->preds_d + n0, n, e->K, ls); KERNEL_OK(); ++e->launches;
-    if (logits_host) CUDA_OK(cudaMemcpyAsync(logits_host + (size_t)n0 * e->K, L.logits, (size_t)n * e->K * 4, cudaMemcpyDeviceToHost, ls));
-  }
-  walk.join();
-  CUDA_OK(cudaMemcpyAsync(preds_host, e->preds_d, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    NvtxRange nvtx_("dorpatch.predict");
+    const int N = B * S;
+    if (N < 1) fail("dp_predict: empty batch");
+    e->forward_clobbered();
+    e->h2d_samples(rects_host, N, st);
+    const dp_engine::EotIn in = dp_engine::EotIn::image(img, nullptr, rects_host ? e->rects_d : nullptr, B, S);
+    // forward-only scan (collect_failure, PatchCleanser): chunks alternate between the two lanes like dp_attack_grad
+    LaneWalk walk(e, st, N > e->chunk);
+    for (int n0 = 0, c = 0; n0 < N; n0 += e->chunk, ++c) {
+      const int n = std::min(e->chunk, N - n0);
+      const dp_engine::Lane& L = e->lanes[walk.lane_of(c)];
+      cudaStream_t const ls = walk.stream(walk.lane_of(c));
+      e->forward(L, n, e->chunk_input(L, in, n0, n, false, ls), false, ls);
+      e->run(ls, [&] { return dp::launch_argmax(L.logits, e->preds_d + n0, n, e->K, ls); });
+      if (logits_host) CUDA_OK(cudaMemcpyAsync(logits_host + (size_t)n0 * e->K, L.logits, (size_t)n * e->K * 4, cudaMemcpyDeviceToHost, ls));
+    }
+    walk.join();
+    CUDA_OK(cudaMemcpyAsync(preds_host, e->preds_d, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+  });
 }
 
 // Everything dp_attack_grad puts on the stream: staging H2D copies, per-image kernels, the chunk loop on one or two
@@ -1462,11 +1451,11 @@ static void attack_grad_enqueue(dp_engine* e, const dp_attack_args* a, const Gra
   const int16_t* rects = rect_bytes ? e->rects_d : nullptr;
 
   const double img_bytes = (double)B * H * H * 4;
-  PROF(e, "paste", 10.0 * img_bytes, 0, st, dp::launch_paste(a->x, a->mask, a->pattern, e->adv_x, e->l2, e->scale, B, H, H, a->eps, st)); KERNEL_OK(); ++e->launches;
-  PROF(e, "struct", 9.0 * img_bytes, 0, st, dp::launch_struct(e->adv_x, a->x, e->loss_struc, e->dLs, B, H, H, st)); KERNEL_OK(); ++e->launches;
-  if (a->stage == 0) {
-    PROF(e, "maskreg", img_bytes, 0, st, dp::launch_maskreg(a->mask, e->loss_density, e->group_lasso, e->win_dev, e->grp_ss, B, H, H, e->unit, st)); KERNEL_OK(); ++e->launches;
-  }
+  e->run("paste", 10.0 * img_bytes, 0, st, [&] { return dp::launch_paste(a->x, a->mask, a->pattern, e->adv_x, e->l2, e->scale, B, H, H, a->eps, st); });
+  e->run("struct", 9.0 * img_bytes, 0, st, [&] { return dp::launch_struct(e->adv_x, a->x, e->loss_struc, e->dLs, B, H, H, st); });
+  if (a->stage == 0)
+    e->run("maskreg", img_bytes, 0, st,
+           [&] { return dp::launch_maskreg(a->mask, e->loss_density, e->group_lasso, e->win_dev, e->grp_ss, B, H, H, e->unit, st); });
   const float inv_s = 1.0f / (float)a->S_total;
   // with transforms each chunk's input is the pasted image adv_x warped; otherwise K1 pastes as it expands
   const dp_engine::EotIn in = xf_bytes ? dp_engine::EotIn::image(e->adv_x, e->xf_d, rects, B, S)
@@ -1481,9 +1470,9 @@ static void attack_grad_enqueue(dp_engine* e, const dp_attack_args* a, const Gra
     const dp_engine::Lane& L = e->lanes[walk.lane_of(c)];
     cudaStream_t const ls = walk.stream(walk.lane_of(c));
     e->forward(L, n, e->chunk_input(L, in, n0, n, k1_whole, ls), true, ls);
-    PROF(e, "cw_k4", 2.0 * n * e->K * 4, 0, ls,
-         dp::launch_cw(L.logits, e->y_d + n0, e->tg_d + n0, a->confidence, inv_s, e->loss_d + n0, e->preds_d + n0, L.dlogits, n, e->K, ls));
-    KERNEL_OK(); ++e->launches;
+    e->run("cw_k4", 2.0 * n * e->K * 4, 0, ls, [&] {
+      return dp::launch_cw(L.logits, e->y_d + n0, e->tg_d + n0, a->confidence, inv_s, e->loss_d + n0, e->preds_d + n0, L.dlogits, n, e->K, ls);
+    });
     e->backward_reduce(L, in, n0, n, a->grad_adv, ls);
   }
   walk.join();
@@ -1595,51 +1584,44 @@ static void attack_update_impl(dp_engine* e, const dp_update_args* u, cudaStream
   CUDA_OK(cudaMemcpyAsync(e->lr_d, h, (size_t)B * 4, cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaMemcpyAsync(e->structured_d, h + B, (size_t)B * 4, cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaMemcpyAsync(e->coeff_d, h + 2 * B, (size_t)B * 4, cudaMemcpyHostToDevice, st));
-  PROF(e, "update_k3", (double)B * e->H * e->H * 4 * (u->stage == 0 ? 15.0 : 13.0), 0, st,
-       dp::launch_update(u->x, u->mask, u->pattern, u->grad_adv, e->dLs, e->scale, e->win_dev, e->grp_ss, e->lr_d, e->structured_d,
-                         e->coeff_d, u->density, u->clip_min, u->clip_max, u->stage, u->grad_pattern_out, u->grad_mask_out, u->grad_pattern_bias, B, e->H, e->H, e->unit, st));
-  KERNEL_OK(); ++e->launches;
+  e->run("update_k3", (double)B * e->H * e->H * 4 * (u->stage == 0 ? 15.0 : 13.0), 0, st, [&] {
+    return dp::launch_update(u->x, u->mask, u->pattern, u->grad_adv, e->dLs, e->scale, e->win_dev, e->grp_ss, e->lr_d, e->structured_d,
+                             e->coeff_d, u->density, u->clip_min, u->clip_max, u->stage, u->grad_pattern_out, u->grad_mask_out, u->grad_pattern_bias, B, e->H, e->H, e->unit, st);
+  });
   CUDA_OK(cudaStreamSynchronize(st));   // `pin` may be reused by the next call
 }
 
 int32_t dp_attack_grad(dp_engine* e, const dp_attack_args* a, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  attack_grad_impl(e, a, (cudaStream_t)stream);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    attack_grad_impl(e, a, st);
+  });
 }
 
 int32_t dp_attack_update(dp_engine* e, const dp_update_args* u, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  attack_update_impl(e, u, (cudaStream_t)stream);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    attack_update_impl(e, u, st);
+  });
 }
 
 int32_t dp_attack_step_host(dp_engine* e, const dp_attack_args* g, const dp_update_args* u, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (!g || !u) fail("null args");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  e->check_B(g->B);
-  const size_t B = (size_t)g->B, HW = (size_t)e->H * e->H;
-  CUDA_OK(cudaMemcpyAsync(e->host_x, g->x, B * 3 * HW * 4, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemcpyAsync(e->host_mask, g->mask, B * HW * 4, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemcpyAsync(e->host_pattern, g->pattern, B * 3 * HW * 4, cudaMemcpyHostToDevice, st));
-  dp_attack_args ga = *g;
-  ga.x = e->host_x; ga.mask = e->host_mask; ga.pattern = e->host_pattern; ga.grad_adv = e->host_G;
-  attack_grad_impl(e, &ga, st);
-  dp_update_args ua = *u;
-  ua.x = e->host_x; ua.mask = e->host_mask; ua.pattern = e->host_pattern; ua.grad_adv = e->host_G;
-  ua.grad_pattern_out = nullptr; ua.grad_mask_out = nullptr; ua.grad_pattern_bias = nullptr;
-  attack_update_impl(e, &ua, st);
-  CUDA_OK(cudaMemcpyAsync(u->mask, e->host_mask, B * HW * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaMemcpyAsync(u->pattern, e->host_pattern, B * 3 * HW * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!g || !u) fail("null args");
+    e->check_B(g->B);
+    const size_t B = (size_t)g->B, HW = (size_t)e->H * e->H;
+    CUDA_OK(cudaMemcpyAsync(e->host_x, g->x, B * 3 * HW * 4, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(e->host_mask, g->mask, B * HW * 4, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(e->host_pattern, g->pattern, B * 3 * HW * 4, cudaMemcpyHostToDevice, st));
+    dp_attack_args ga = *g;
+    ga.x = e->host_x; ga.mask = e->host_mask; ga.pattern = e->host_pattern; ga.grad_adv = e->host_G;
+    attack_grad_impl(e, &ga, st);
+    dp_update_args ua = *u;
+    ua.x = e->host_x; ua.mask = e->host_mask; ua.pattern = e->host_pattern; ua.grad_adv = e->host_G;
+    ua.grad_pattern_out = nullptr; ua.grad_mask_out = nullptr; ua.grad_pattern_bias = nullptr;
+    attack_update_impl(e, &ua, st);
+    CUDA_OK(cudaMemcpyAsync(u->mask, e->host_mask, B * HW * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaMemcpyAsync(u->pattern, e->host_pattern, B * 3 * HW * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+  });
 }
 
 /* ---- differentiable classifier: model(occlude(img)) and its input gradient as two calls ------------------------- */
@@ -1788,257 +1770,215 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
       const float* b = nl > 1 ? e->lanes[1].wacc + w.off : nullptr;
       if (w.kind == dp_engine::W_CONV) {
         const ConvW& c = *w.conv;
-        PROF(e, "ws_wgrad", (double)w.numel * 8 + (double)c.cout * c.k * c.k * c.cin_pad * 4 * nl, 0, st,
-             dp::launch_ws_backward(c.raw, a, b, pc->grads[i], c.cout, c.cin, c.k, c.k, c.cin_pad, pc->accumulate != 0, st));
+        e->run("ws_wgrad", (double)w.numel * 8 + (double)c.cout * c.k * c.k * c.cin_pad * 4 * nl, 0, st,
+               [&] { return dp::launch_ws_backward(c.raw, a, b, pc->grads[i], c.cout, c.cin, c.k, c.k, c.cin_pad, pc->accumulate != 0, st); });
       } else {
-        PROF(e, "vec_wgrad", (double)w.numel * 4 * (nl + 2), 0, st,
-             dp::launch_vec_finish(a, b, pc->grads[i], (size_t)w.numel, pc->accumulate != 0, st));
+        e->run("vec_wgrad", (double)w.numel * 4 * (nl + 2), 0, st,
+               [&] { return dp::launch_vec_finish(a, b, pc->grads[i], (size_t)w.numel, pc->accumulate != 0, st); });
       }
-      KERNEL_OK(); ++e->launches;
     }
   }
 }
 
 int32_t dp_eot_forward(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host, float* logits_dev,
                        void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  eot_forward_impl(e, img, B, S, rects_host, nullptr, logits_dev, (cudaStream_t)stream);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    eot_forward_impl(e, img, B, S, rects_host, nullptr, logits_dev, st);
+  });
 }
 
 int32_t dp_eot_forward_xform(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host,
                              const float* xform_host, float* logits_dev, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  eot_forward_impl(e, img, B, S, rects_host, xform_host, logits_dev, (cudaStream_t)stream);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    eot_forward_impl(e, img, B, S, rects_host, xform_host, logits_dev, st);
+  });
 }
 
 int32_t dp_eot_backward(dp_engine* e, const float* dlogits_dev, float* grad_img_dev, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  eot_backward_impl(e, dlogits_dev, grad_img_dev, (cudaStream_t)stream);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    eot_backward_impl(e, dlogits_dev, grad_img_dev, st);
+  });
 }
 
 int32_t dp_eot_backward_params(dp_engine* e, const float* dlogits_dev, float* grad_img_dev, int32_t n, const char* const* names,
                                float* const* grad_dev_ptrs, int32_t accumulate, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  ParamCall pc{n, names, grad_dev_ptrs, accumulate};
-  eot_backward_impl(e, dlogits_dev, grad_img_dev, (cudaStream_t)stream, &pc);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    ParamCall pc{n, names, grad_dev_ptrs, accumulate};
+    eot_backward_impl(e, dlogits_dev, grad_img_dev, st, &pc);
+  });
 }
 
 int32_t dp_net_forward_backward(dp_engine* e, const float* z, int32_t N, float* logits_dev, const float* dlogits_dev,
                                 float* dz_dev, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  if (N < 1 || N > e->chunk) fail("N=%d outside [1, chunk=%d]", N, e->chunk);
-  e->forward_clobbered();
-  const dp_engine::Lane& L = e->lanes[0];
-  dp::launch_pack_nchw(z, L.net_in, N, e->H, e->H, e->stem.in_ch, e->bf16, st); KERNEL_OK(); ++e->launches;
-  e->forward(L, N, L.net_in, dlogits_dev != nullptr, st);
-  if (logits_dev) CUDA_OK(cudaMemcpyAsync(logits_dev, L.logits, (size_t)N * e->K * 4, cudaMemcpyDeviceToDevice, st));
-  if (dlogits_dev) {
-    if (!dz_dev) fail("dz_dev is required when dlogits_dev is given");
-    const void* dx = e->backward(L, N, dlogits_dev, st);
-    dp::launch_unpack_nhwc(dx, dz_dev, N, e->H, e->H, e->stem.dx_ch, e->bf16, st); KERNEL_OK(); ++e->launches;
-  }
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (N < 1 || N > e->chunk) fail("N=%d outside [1, chunk=%d]", N, e->chunk);
+    e->forward_clobbered();
+    const dp_engine::Lane& L = e->lanes[0];
+    e->run(st, [&] { return dp::launch_pack_nchw(z, L.net_in, N, e->H, e->H, e->stem.in_ch, e->bf16, st); });
+    e->forward(L, N, L.net_in, dlogits_dev != nullptr, st);
+    if (logits_dev) CUDA_OK(cudaMemcpyAsync(logits_dev, L.logits, (size_t)N * e->K * 4, cudaMemcpyDeviceToDevice, st));
+    if (dlogits_dev) {
+      if (!dz_dev) fail("dz_dev is required when dlogits_dev is given");
+      const void* dx = e->backward(L, N, dlogits_dev, st);
+      e->run(st, [&] { return dp::launch_unpack_nhwc(dx, dz_dev, N, e->H, e->H, e->stem.dx_ch, e->bf16, st); });
+    }
+  });
 }
 
 /* ---- failed-mask sets on the device (attack.py:96,187-190,259-267) ------------------------------------- */
 int32_t dp_failed_set_reset(dp_engine* e, int32_t n_mask, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (n_mask < 1) fail("dp_failed_set_reset: n_mask %d < 1", n_mask);
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int words = (int)(((int64_t)n_mask + 31) / 32);
-  const size_t B = (size_t)e->cfg.max_images;
-  if (words > e->failed_words_alloc) {                 // the old bitmaps stay in `allocs` until destroy
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (n_mask < 1) fail("dp_failed_set_reset: n_mask %d < 1", n_mask);
+    const int words = (int)(((int64_t)n_mask + 31) / 32);
+    const size_t B = (size_t)e->cfg.max_images;
+    if (words > e->failed_words_alloc) {                 // the old bitmaps stay in `allocs` until destroy
+      CUDA_OK(cudaStreamSynchronize(st));
+      e->failed_bits = (uint32_t*)e->dmalloc(B * words * 4);
+      e->failed_words_alloc = words;
+    }
+    e->failed_masks = n_mask;
+    e->failed_words = words;
+    CUDA_OK(cudaMemsetAsync(e->failed_bits, 0, B * words * 4, st));
     CUDA_OK(cudaStreamSynchronize(st));
-    e->failed_bits = (uint32_t*)e->dmalloc(B * words * 4);
-    e->failed_words_alloc = words;
-  }
-  e->failed_masks = n_mask;
-  e->failed_words = words;
-  CUDA_OK(cudaMemsetAsync(e->failed_bits, 0, B * words * 4, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  DP_CATCH
+  });
 }
 
 int32_t dp_failed_set_write(dp_engine* e, int32_t b, const int32_t* idx_host, int32_t n, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (b < 0 || b >= e->cfg.max_images) fail("image %d outside [0, max_images=%d)", b, e->cfg.max_images);
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  std::vector<uint32_t> w(e->failed_words, 0u);
-  for (int i = 0; i < n; ++i) {
-    if (idx_host[i] < 0 || idx_host[i] >= e->failed_masks) fail("mask index %d outside [0, %d)", idx_host[i], e->failed_masks);
-    w[idx_host[i] >> 5] |= 1u << (idx_host[i] & 31);
-  }
-  CUDA_OK(cudaMemcpyAsync(e->failed_bits + (size_t)b * e->failed_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (b < 0 || b >= e->cfg.max_images) fail("image %d outside [0, max_images=%d)", b, e->cfg.max_images);
+    std::vector<uint32_t> w(e->failed_words, 0u);
+    for (int i = 0; i < n; ++i) {
+      if (idx_host[i] < 0 || idx_host[i] >= e->failed_masks) fail("mask index %d outside [0, %d)", idx_host[i], e->failed_masks);
+      w[idx_host[i] >> 5] |= 1u << (idx_host[i] & 31);
+    }
+    CUDA_OK(cudaMemcpyAsync(e->failed_bits + (size_t)b * e->failed_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+  });
 }
 
 int32_t dp_failed_set_update(dp_engine* e, int32_t B, int32_t S, const int32_t* idx_host, const int32_t* nff_host, const uint8_t* active_host,
                              const float* loss_host, float thresh, int32_t* count_host, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  e->check_B(B);
-  if (S < 1 || !idx_host || !nff_host || !active_host || !count_host) fail("dp_failed_set_update: bad arguments");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int N = B * S;
-  if (N > e->failed_cap) {
-    e->failed_cap = std::max(N, e->failed_cap * 2);
-    e->failed_idx = (int32_t*)e->dmalloc((size_t)e->failed_cap * 4);
-    e->failed_loss = (float*)e->dmalloc((size_t)e->failed_cap * 4);
-  }
-  for (int i = 0; i < N; ++i)
-    if (idx_host[i] < 0 || idx_host[i] >= e->failed_masks) fail("mask index %d outside [0, %d)", idx_host[i], e->failed_masks);
-  CUDA_OK(cudaMemcpyAsync(e->failed_idx, idx_host, (size_t)N * 4, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemcpyAsync(e->failed_nff, nff_host, (size_t)B * 4, cudaMemcpyHostToDevice, st));
-  CUDA_OK(cudaMemcpyAsync(e->failed_active, active_host, (size_t)B, cudaMemcpyHostToDevice, st));
-  const float* loss = e->loss_d;                       // default: the per-sample CW losses the last dp_attack_grad left on the device
-  if (loss_host != nullptr) {                          // EOT-sharded runs pass the all-gathered losses
-    CUDA_OK(cudaMemcpyAsync(e->failed_loss, loss_host, (size_t)N * 4, cudaMemcpyHostToDevice, st));
-    loss = e->failed_loss;
-  } else if (N > e->cap_samples) fail("dp_failed_set_update: no device losses for %d samples", N);
-  dp::launch_failed_update(e->failed_bits, e->failed_words, e->failed_idx, loss, e->failed_nff, e->failed_active, B, S, thresh,
-                           e->failed_count, st);
-  KERNEL_OK(); ++e->launches;
-  CUDA_OK(cudaMemcpyAsync(count_host, e->failed_count, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    e->check_B(B);
+    if (S < 1 || !idx_host || !nff_host || !active_host || !count_host) fail("dp_failed_set_update: bad arguments");
+    const int N = B * S;
+    if (N > e->failed_cap) {
+      e->failed_cap = std::max(N, e->failed_cap * 2);
+      e->failed_idx = (int32_t*)e->dmalloc((size_t)e->failed_cap * 4);
+      e->failed_loss = (float*)e->dmalloc((size_t)e->failed_cap * 4);
+    }
+    for (int i = 0; i < N; ++i)
+      if (idx_host[i] < 0 || idx_host[i] >= e->failed_masks) fail("mask index %d outside [0, %d)", idx_host[i], e->failed_masks);
+    CUDA_OK(cudaMemcpyAsync(e->failed_idx, idx_host, (size_t)N * 4, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(e->failed_nff, nff_host, (size_t)B * 4, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(e->failed_active, active_host, (size_t)B, cudaMemcpyHostToDevice, st));
+    const float* loss = e->loss_d;                       // default: the per-sample CW losses the last dp_attack_grad left on the device
+    if (loss_host != nullptr) {                          // EOT-sharded runs pass the all-gathered losses
+      CUDA_OK(cudaMemcpyAsync(e->failed_loss, loss_host, (size_t)N * 4, cudaMemcpyHostToDevice, st));
+      loss = e->failed_loss;
+    } else if (N > e->cap_samples) fail("dp_failed_set_update: no device losses for %d samples", N);
+    e->run(st, [&] {
+      return dp::launch_failed_update(e->failed_bits, e->failed_words, e->failed_idx, loss, e->failed_nff, e->failed_active, B, S, thresh,
+                                      e->failed_count, st);
+    });
+    CUDA_OK(cudaMemcpyAsync(count_host, e->failed_count, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+  });
 }
 
 int32_t dp_failed_set_read(dp_engine* e, int32_t b, int32_t* idx_host_out, int32_t cap, int32_t* n_out, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (b < 0 || b >= e->cfg.max_images) fail("image %d outside [0, max_images=%d)", b, e->cfg.max_images);
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  std::vector<uint32_t> w(e->failed_words);
-  CUDA_OK(cudaMemcpyAsync(w.data(), e->failed_bits + (size_t)b * e->failed_words, w.size() * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  int n = 0;
-  for (int j = 0; j < e->failed_words; ++j)            // set bits only: the 90 720-mask universe is 2835 words
-    for (uint32_t v = w[j]; v; v &= v - 1) {
-      const int i = j * 32 + __builtin_ctz(v);
-      if (n < cap && idx_host_out) idx_host_out[n] = i;
-      ++n;
-    }
-  if (n_out) *n_out = n;
-  if (n > cap && idx_host_out) fail("dp_failed_set_read: %d indices, buffer holds %d", n, cap);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (b < 0 || b >= e->cfg.max_images) fail("image %d outside [0, max_images=%d)", b, e->cfg.max_images);
+    std::vector<uint32_t> w(e->failed_words);
+    CUDA_OK(cudaMemcpyAsync(w.data(), e->failed_bits + (size_t)b * e->failed_words, w.size() * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    int n = 0;
+    for (int j = 0; j < e->failed_words; ++j)            // set bits only: the 90 720-mask universe is 2835 words
+      for (uint32_t v = w[j]; v; v &= v - 1) {
+        const int i = j * 32 + __builtin_ctz(v);
+        if (n < cap && idx_host_out) idx_host_out[n] = i;
+        ++n;
+      }
+    if (n_out) *n_out = n;
+    if (n > cap && idx_host_out) fail("dp_failed_set_read: %d indices, buffer holds %d", n, cap);
+  });
 }
 
 /* ---- op-level test hooks (tests/test_gpu_ops.py, tests/test_gpu_stem_ops.py) --------------------------- */
 // G is left to the kernel (no memset), which writes every element of every image: a gap would show as the caller's fill.
 int32_t dp_debug_stem_bwd_reduce(dp_engine* e, const void* dY, const int16_t* rects_host, int32_t B, int32_t S, float* G,
                                  void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_bwd_reduce: the fused stem backward exists for the bf16 engine only");
-  if (!dY || !G || B < 1 || S < 1) fail("dp_debug_stem_bwd_reduce: bad arguments");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int N = B * S;
-  e->h2d_samples(rects_host, N, st);
-  e->stem.fused_reduce(dY, dp_engine::FusedReduce{rects_host ? e->rects_d : nullptr, G, B, S, 0}, N, st);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_bwd_reduce: the fused stem backward exists for the bf16 engine only");
+    if (!dY || !G || B < 1 || S < 1) fail("dp_debug_stem_bwd_reduce: bad arguments");
+    const int N = B * S;
+    e->h2d_samples(rects_host, N, st);
+    const dp_engine::FusedReduce fr{rects_host ? e->rects_d : nullptr, G, B, S, 0};
+    e->run(st, [&] { return e->stem.fused_reduce(dY, fr, N, st); });
+  });
 }
 
 int32_t dp_debug_stem_bwd_pool_reduce(dp_engine* e, const void* dpool, const int8_t* amax, const int16_t* rects_host, int32_t B,
                                       int32_t S, float* G, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_bwd_pool_reduce: the fused stem backward exists for the bf16 engine only");
-  if (!dpool || !amax || !G || B < 1 || S < 1) fail("dp_debug_stem_bwd_pool_reduce: bad arguments");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int N = B * S;
-  e->h2d_samples(rects_host, N, st);
-  e->stem.fused_pool_reduce(dpool, amax, dp_engine::FusedReduce{rects_host ? e->rects_d : nullptr, G, B, S, 0}, N, st);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_bwd_pool_reduce: the fused stem backward exists for the bf16 engine only");
+    if (!dpool || !amax || !G || B < 1 || S < 1) fail("dp_debug_stem_bwd_pool_reduce: bad arguments");
+    const int N = B * S;
+    e->h2d_samples(rects_host, N, st);
+    const dp_engine::FusedReduce fr{rects_host ? e->rects_d : nullptr, G, B, S, 0};
+    e->run(st, [&] { return e->stem.fused_pool_reduce(dpool, amax, fr, N, st); });
+  });
 }
 
 int32_t dp_debug_stem_forward(dp_engine* e, const void* in, void* out, void* w_out, int32_t N, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_forward: this engine's stem is not the own bf16 kernel");
-  if (!in || !out || N < 1 || N > 65535) fail("dp_debug_stem_forward: bad arguments");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const ConvW& c = e->stem.conv;
-  if (w_out) CUDA_OK(cudaMemcpyAsync(w_out, c.w, (size_t)c.cout * c.k * c.k * c.cin_pad * 2, cudaMemcpyDeviceToDevice, st));
-  e->stem.own_forward(in, out, N, st);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_forward: this engine's stem is not the own bf16 kernel");
+    if (!in || !out || N < 1 || N > 65535) fail("dp_debug_stem_forward: bad arguments");
+    const ConvW& c = e->stem.conv;
+    if (w_out) CUDA_OK(cudaMemcpyAsync(w_out, c.w, (size_t)c.cout * c.k * c.k * c.cin_pad * 2, cudaMemcpyDeviceToDevice, st));
+    e->run(st, [&] { return e->stem.own_forward(in, out, N, st); });
+  });
 }
 
 int32_t dp_debug_maxpool(dp_engine* e, const void* x, void* y, int8_t* amax, const void* dy, void* dx, int32_t N, int32_t Hs,
                          int32_t C, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (!x || !y || N < 1 || Hs < 2 || Hs % 2 != 0 || C < 1 || C % (e->bf16 ? 8 : 4) != 0 || (dy && (!amax || !dx)))
-    fail("dp_debug_maxpool: bad arguments");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  e->stem.pool_forward(x, y, amax, N, Hs, C, st);
-  if (dy) e->stem.pool_backward(dy, amax, dx, N, Hs, C, st);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!x || !y || N < 1 || Hs < 2 || Hs % 2 != 0 || C < 1 || C % (e->bf16 ? 8 : 4) != 0 || (dy && (!amax || !dx)))
+      fail("dp_debug_maxpool: bad arguments");
+    e->run(st, [&] { return e->stem.pool_forward(x, y, amax, N, Hs, C, st); });
+    if (dy) e->run(st, [&] { return e->stem.pool_backward(dy, amax, dx, N, Hs, C, st); });
+  });
 }
 
 int32_t dp_debug_stem_wgrad(dp_engine* e, const void* in, const void* dY, int32_t N, float* dW, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (!in || !dY || !dW || N < 1) fail("dp_debug_stem_wgrad: bad arguments");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  e->ensure_wgrad_buffers();
-  CUDA_OK(cudaMemsetAsync(dW, 0, (size_t)STEM_CH * 49 * 3 * 4, st));
-  e->stem.own_wgrad(in, dY, e->lanes[0].wg_partial, dW, N, 3, st);
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!in || !dY || !dW || N < 1) fail("dp_debug_stem_wgrad: bad arguments");
+    e->ensure_wgrad_buffers();
+    CUDA_OK(cudaMemsetAsync(dW, 0, (size_t)STEM_CH * 49 * 3 * 4, st));
+    e->run(st, [&] { return e->stem.own_wgrad(in, dY, e->lanes[0].wg_partial, dW, N, 3, st); });
+  });
 }
 
 int32_t dp_debug_gn_wgrad(dp_engine* e, const void* x, const void* dy, const float* gamma, const float* beta, const float* stats,
                           int32_t N, int32_t P, int32_t C, float* dgb, void* y, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (!x || !dy || !gamma || !beta || !stats || !dgb || N < 1 || N > e->chunk || P < 1 || C % dp::GN_GROUPS != 0 || C > 2048)
-    fail("dp_debug_gn_wgrad: bad arguments");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  e->ensure_wgrad_buffers();
-  CUDA_OK(cudaMemsetAsync(dgb, 0, (size_t)2 * C * 4, st));
-  dp::launch_gn_affine_partial(dy, x, gamma, beta, stats, e->lanes[0].wg_partial, N, P, C, e->bf16, st); KERNEL_OK();
-  dp::launch_colsum_add(e->lanes[0].wg_partial, dgb, N, 2 * C, st); KERNEL_OK();
-  if (y) { dp::launch_gn_apply(x, y, gamma, beta, stats, N, P, C, e->bf16, st); KERNEL_OK(); }
-  e->launches += y ? 3 : 2;
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!x || !dy || !gamma || !beta || !stats || !dgb || N < 1 || N > e->chunk || P < 1 || C % dp::GN_GROUPS != 0 || C > 2048)
+      fail("dp_debug_gn_wgrad: bad arguments");
+    e->ensure_wgrad_buffers();
+    CUDA_OK(cudaMemsetAsync(dgb, 0, (size_t)2 * C * 4, st));
+    float* const partial = e->lanes[0].wg_partial;
+    e->run(st, [&] { return dp::launch_gn_affine_partial(dy, x, gamma, beta, stats, partial, N, P, C, e->bf16, st); });
+    e->run(st, [&] { return dp::launch_colsum_add(partial, dgb, N, 2 * C, st); });
+    if (y) e->run(st, [&] { return dp::launch_gn_apply(x, y, gamma, beta, stats, N, P, C, e->bf16, st); });
+  });
 }
 
 int32_t dp_debug_ws_backward(dp_engine* e, const float* w_raw, const float* g_a, const float* g_b, int32_t O, int32_t I, int32_t k,
                              int32_t Ipad, float* out, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  if (!w_raw || !g_a || !out || O < 1 || I < 1 || k < 1 || Ipad < I) fail("dp_debug_ws_backward: bad arguments");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  dp::launch_ws_backward(w_raw, g_a, g_b, out, O, I, k, k, Ipad, false, (cudaStream_t)stream); KERNEL_OK();
-  ++e->launches;
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!w_raw || !g_a || !out || O < 1 || I < 1 || k < 1 || Ipad < I) fail("dp_debug_ws_backward: bad arguments");
+    e->run(st, [&] { return dp::launch_ws_backward(w_raw, g_a, g_b, out, O, I, k, k, Ipad, false, st); });
+  });
 }
 
 int32_t dp_debug_k1_tuning(int32_t rows, int32_t sg, int32_t mode) {
@@ -2055,39 +1995,40 @@ int32_t dp_debug_k1_last(int32_t* out4) {
 
 int32_t dp_debug_gn_gemm(dp_engine* e, const void* x, const void* w_nk, const float* stats, const float* gamma, const float* beta,
                          const void* shortcut, void* out, int32_t N, int32_t P, int32_t K, int32_t Nout, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  if (!dp::gn_gemm_supported(P, K, Nout)) fail("dp_debug_gn_gemm: shape P=%d K=%d Nout=%d not supported by the wgmma kernel", P, K, Nout);
-  void* packed = nullptr;
-  CUDA_OK(cudaMalloc(&packed, (size_t)Nout * K * 2));
-  dp::launch_gn_gemm_pack(w_nk, packed, Nout, K, st);
-  const bool ok = dp::launch_gn_gemm_forward(x, packed, stats, gamma, beta, shortcut, out, N, P, K, Nout, st);
-  cudaError_t err = cudaStreamSynchronize(st);
-  cudaFree(packed);
-  if (!ok) fail("dp_debug_gn_gemm: launch refused");
-  CUDA_OK(err);
-  KERNEL_OK(); e->launches += 2;
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!dp::gn_gemm_supported(P, K, Nout)) fail("dp_debug_gn_gemm: shape P=%d K=%d Nout=%d not supported by the wgmma kernel", P, K, Nout);
+    void* packed = nullptr;
+    CUDA_OK(cudaMalloc(&packed, (size_t)Nout * K * 2));
+    int fwd = 0;
+    try {
+      e->run(st, [&] {
+        const int n = dp::launch_gn_gemm_pack(w_nk, packed, Nout, K, st);
+        return n + (fwd = dp::launch_gn_gemm_forward(x, packed, stats, gamma, beta, shortcut, out, N, P, K, Nout, st));
+      });
+    } catch (...) {
+      cudaFree(packed);
+      throw;
+    }
+    const cudaError_t err = cudaStreamSynchronize(st);
+    cudaFree(packed);
+    if (!fwd) fail("dp_debug_gn_gemm: launch refused");
+    CUDA_OK(err);
+  });
 }
 
 int32_t dp_debug_gn(dp_engine* e, const void* x, const void* dy, const void* addend, const float* gamma, const float* beta,
                     int32_t gamma_positive, void* y, void* dx, float* stats, int32_t N, int32_t P, int32_t C, void* stream) {
-  DP_TRY
-  if (!e) fail("null engine");
-  CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  if (N > e->chunk) fail("dp_debug_gn: N=%d exceeds chunk=%d (statistics scratch)", N, e->chunk);
-  if (y == nullptr) {   // statistics only: the pass in front of the wgmma GEMM / the classifier head
-    dp::launch_gn_stats(x, e->lanes[0].gn_partial, stats, N, P, C, e->bf16, st); KERNEL_OK();
-    e->launches += 2;
-    return 0;
-  }
-  dp::launch_gn_relu_forward(x, y, gamma, beta, e->lanes[0].gn_partial, stats, N, P, C, e->bf16, st); KERNEL_OK();
-  if (dy != nullptr) { dp::launch_gn_relu_backward(dy, x, addend, dx, gamma, beta, stats, e->lanes[0].gn_partial, N, P, C, e->bf16, st, gamma_positive != 0); KERNEL_OK(); }
-  e->launches += 4;
-  DP_CATCH
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (N > e->chunk) fail("dp_debug_gn: N=%d exceeds chunk=%d (statistics scratch)", N, e->chunk);
+    float* const partial = e->lanes[0].gn_partial;
+    if (y == nullptr) {   // statistics only: the pass in front of the wgmma GEMM / the classifier head
+      e->run(st, [&] { return dp::launch_gn_stats(x, partial, stats, N, P, C, e->bf16, st); });
+      return;
+    }
+    e->run(st, [&] { return dp::launch_gn_relu_forward(x, y, gamma, beta, partial, stats, N, P, C, e->bf16, st); });
+    if (dy != nullptr)
+      e->run(st, [&] { return dp::launch_gn_relu_backward(dy, x, addend, dx, gamma, beta, stats, partial, N, P, C, e->bf16, st, gamma_positive != 0); });
+  });
 }
 
 }  // extern "C"

@@ -242,13 +242,14 @@ bool gn_gemm_supported(int P, int K, int Nout) {
          (tc::BM + P - 1) / P + 1 <= tc::MAX_TILE_SAMPLES;
 }
 
-void launch_gn_gemm_pack(const void* w, void* out, int Nout, int K, cudaStream_t st) {
+int launch_gn_gemm_pack(const void* w, void* out, int Nout, int K, cudaStream_t st) {
   tc::pack_w_kernel<<<256, 256, 0, st>>>((const __nv_bfloat16*)w, (__nv_bfloat16*)out, Nout, K, gn_gemm_tile_n(Nout));
+  return 1;
 }
 
-bool launch_gn_gemm_forward(const void* x, const void* w_packed, const float* stats, const float* gamma, const float* beta,
-                            const void* shortcut, void* out, int N, int P, int K, int Nout, cudaStream_t st) {
-  if (!gn_gemm_supported(P, K, Nout)) return false;
+int launch_gn_gemm_forward(const void* x, const void* w_packed, const float* stats, const float* gamma, const float* beta,
+                           const void* shortcut, void* out, int N, int P, int K, int Nout, cudaStream_t st) {
+  if (!gn_gemm_supported(P, K, Nout)) return 0;
   tc::GemmParams p{(const __nv_bfloat16*)x, (const __nv_bfloat16*)w_packed, stats, gamma, beta,
                    (const __nv_bfloat16*)shortcut, (__nv_bfloat16*)out, N * P, P, K, Nout, N};
   const int bn = gn_gemm_tile_n(Nout);
@@ -262,10 +263,10 @@ bool launch_gn_gemm_forward(const void* x, const void* w_packed, const float* st
   switch (bn) {
     GG_CASE(64)
     GG_CASE(128)
-    default: return false;
+    default: return 0;
   }
 #undef GG_CASE
-  return true;
+  return 1;
 }
 
 }  // namespace dp

@@ -49,9 +49,10 @@ __global__ void ws_kernel(const float* __restrict__ w, T* __restrict__ out, int 
   }
 }
 
-void launch_weight_standardize(const float* w, void* out, int O, int I, int kh, int kw, int Ipad, bool bf16,
-                               bool standardize, cudaStream_t st) {
+int launch_weight_standardize(const float* w, void* out, int O, int I, int kh, int kw, int Ipad, bool bf16,
+                              bool standardize, cudaStream_t st) {
   DISPATCH_T(bf16, (ws_kernel<T><<<O, 256, 0, st>>>(w, (T*)out, I, kh, kw, Ipad, standardize ? 1 : 0)));
+  return 1;
 }
 
 // ------------------------------------------------------------------------------------
@@ -74,13 +75,15 @@ __global__ void unpack_kernel(const T* __restrict__ in, float* __restrict__ dz, 
   const size_t n = i / HW, p = i % HW;
   for (int c = 0; c < 3; ++c) dz[(n * 3 + c) * HW + p] = to_float(in[i * Cp + c]);
 }
-void launch_pack_nchw(const float* z, void* out, int N, int H, int W, int Cp, bool bf16, cudaStream_t st) {
+int launch_pack_nchw(const float* z, void* out, int N, int H, int W, int Cp, bool bf16, cudaStream_t st) {
   size_t total = (size_t)N * H * W;
   DISPATCH_T(bf16, (pack_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(z, (T*)out, H * W, Cp, total)));
+  return 1;
 }
-void launch_unpack_nhwc(const void* in, float* dz, int N, int H, int W, int Cp, bool bf16, cudaStream_t st) {
+int launch_unpack_nhwc(const void* in, float* dz, int N, int H, int W, int Cp, bool bf16, cudaStream_t st) {
   size_t total = (size_t)N * H * W;
   DISPATCH_T(bf16, (unpack_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const T*)in, dz, H * W, Cp, total)));
+  return 1;
 }
 
 // ------------------------------------------------------------------------------------
@@ -240,18 +243,20 @@ static int apply_slabs(int P, int C, int V) {
   return s;
 }
 
-static void launch_gn_stats_2pass(const void* x, float* partial, float* stats, int N, int P, int C, bool bf16, cudaStream_t st) {
+static int launch_gn_stats_2pass(const void* x, float* partial, float* stats, int N, int P, int C, bool bf16, cudaStream_t st) {
   const int splits = gn_splits(P, C, bf16);
   DISPATCH_T(bf16, (gn_stats_kernel<T><<<dim3(splits, N), GN_THREADS, 0, st>>>((const T*)x, partial, P, C, splits)));
   DISPATCH_T(bf16, (gn_finalize_kernel<T><<<N, 32, 0, st>>>(partial, stats, P, C, splits)));
+  return 2;
 }
 
-static void launch_gn_relu_forward_2pass(const void* x, void* y, const float* gamma, const float* beta, float* partial,
-                                         float* stats, int N, int P, int C, bool bf16, cudaStream_t st) {
+static int launch_gn_relu_forward_2pass(const void* x, void* y, const float* gamma, const float* beta, float* partial,
+                                        float* stats, int N, int P, int C, bool bf16, cudaStream_t st) {
   const int splits = gn_splits(P, C, bf16);
   DISPATCH_T(bf16, (gn_stats_kernel<T><<<dim3(splits, N), GN_THREADS, 0, st>>>((const T*)x, partial, P, C, splits)));
   DISPATCH_T(bf16, (gn_apply_kernel<T><<<dim3(apply_slabs(P, C, Vec<T>::N), N), GN_THREADS, 0, st>>>(
                        (const T*)x, (T*)y, gamma, beta, partial, stats, P, C, splits)));
+  return 2;
 }
 
 // ---- backward -----------------------------------------------------------------------
@@ -347,14 +352,15 @@ __global__ void __launch_bounds__(GN_THREADS) gn_bwd_apply_kernel(const T* __res
   }
 }
 
-static void launch_gn_relu_backward_2pass(const void* dy, const void* x, const void* addend, void* dx, const float* gamma,
-                                          const float* beta, const float* stats, float* partial, int N, int P, int C,
-                                          bool bf16, cudaStream_t st) {
+static int launch_gn_relu_backward_2pass(const void* dy, const void* x, const void* addend, void* dx, const float* gamma,
+                                         const float* beta, const float* stats, float* partial, int N, int P, int C,
+                                         bool bf16, cudaStream_t st) {
   const int splits = gn_splits(P, C, bf16);
   DISPATCH_T(bf16, (gn_bwd_reduce_kernel<T><<<dim3(splits, N), GN_THREADS, 0, st>>>(
                        (const T*)dy, (const T*)x, gamma, beta, stats, partial, P, C, splits)));
   DISPATCH_T(bf16, (gn_bwd_apply_kernel<T><<<dim3(apply_slabs(P, C, Vec<T>::N), N), GN_THREADS, 0, st>>>(
                        (const T*)dy, (const T*)x, (const T*)addend, (T*)dx, gamma, beta, stats, partial, P, C, splits)));
+  return 2;
 }
 
 // ------------------------------------------------------------------------------------
@@ -451,19 +457,21 @@ __global__ void maxpool_bwd_kernel(const T* __restrict__ dy, const int8_t* __res
   Vec<T> out; out.pack(acc); out.store(dx + i * V);
 }
 
-void launch_maxpool_forward(const void* x, void* y, int8_t* amax, int N, int Hs, int Ws, int C, bool bf16,
-                            cudaStream_t st) {
+int launch_maxpool_forward(const void* x, void* y, int8_t* amax, int N, int Hs, int Ws, int C, bool bf16,
+                           cudaStream_t st) {
   DISPATCH_T(bf16, {
     size_t total = (size_t)N * (Hs / 2) * (Ws / 2) * (C / Vec<T>::N);
     maxpool_fwd_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const T*)x, (T*)y, amax, Hs, Ws, C, total);
   });
+  return 1;
 }
-void launch_maxpool_backward(const void* dy, const int8_t* amax, void* dx, int N, int Hs, int Ws, int C, bool bf16,
-                             cudaStream_t st) {
+int launch_maxpool_backward(const void* dy, const int8_t* amax, void* dx, int N, int Hs, int Ws, int C, bool bf16,
+                            cudaStream_t st) {
   DISPATCH_T(bf16, {
     size_t total = (size_t)N * Hs * Ws * (C / Vec<T>::N);
     maxpool_bwd_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const T*)dy, amax, (T*)dx, Hs, Ws, C, total);
   });
+  return 1;
 }
 
 // ------------------------------------------------------------------------------------
@@ -502,10 +510,11 @@ __global__ void head_pool_kernel(const T* __restrict__ x, const float* __restric
     }
   }
 }
-void launch_head_pool(const void* x, const float* gamma, const float* beta, const float* stats, float* pooled,
-                      int N, int P, int C, bool bf16, cudaStream_t st) {
+int launch_head_pool(const void* x, const float* gamma, const float* beta, const float* stats, float* pooled,
+                     int N, int P, int C, bool bf16, cudaStream_t st) {
   DISPATCH_T(bf16, (head_pool_kernel<T><<<dim3(C / (Vec<T>::N * 32), N), dim3(32, 8), 0, st>>>(
                        (const T*)x, gamma, beta, stats, pooled, P, C)));
+  return 1;
 }
 
 template <typename T>
@@ -520,11 +529,12 @@ __global__ void pool_grad_bcast_kernel(const float* __restrict__ dp, T* __restri
   for (int k = 0; k < V; ++k) f[k] = dp[n * C + col * V + k] / P;
   Vec<T> v; v.pack(f); v.store(dy + i * V);
 }
-void launch_pool_grad_bcast(const float* dpooled, void* dy, int N, int P, int C, bool bf16, cudaStream_t st) {
+int launch_pool_grad_bcast(const float* dpooled, void* dy, int N, int P, int C, bool bf16, cudaStream_t st) {
   DISPATCH_T(bf16, {
     size_t total = (size_t)N * P * (C / Vec<T>::N);
     pool_grad_bcast_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(dpooled, (T*)dy, P, C, total);
   });
+  return 1;
 }
 
 // ------------------------------------------------------------------------------------
@@ -560,17 +570,19 @@ __global__ void subsample2_adj_kernel(const T* __restrict__ dy, T* __restrict__ 
   for (int k = 0; k < V; ++k) fb[k] += fa[k];
   b.pack(fb); b.store(dst);
 }
-void launch_subsample2(const void* x, void* y, int N, int H, int W, int C, bool bf16, cudaStream_t st) {
+int launch_subsample2(const void* x, void* y, int N, int H, int W, int C, bool bf16, cudaStream_t st) {
   DISPATCH_T(bf16, {
     size_t total = (size_t)N * ((H + 1) / 2) * ((W + 1) / 2) * (C / Vec<T>::N);
     subsample2_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const T*)x, (T*)y, H, W, C, total);
   });
+  return 1;
 }
-void launch_subsample2_adjoint_add(const void* dy, void* dx, int N, int H, int W, int C, bool bf16, cudaStream_t st) {
+int launch_subsample2_adjoint_add(const void* dy, void* dx, int N, int H, int W, int C, bool bf16, cudaStream_t st) {
   DISPATCH_T(bf16, {
     size_t total = (size_t)N * ((H + 1) / 2) * ((W + 1) / 2) * (C / Vec<T>::N);
     subsample2_adj_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const T*)dy, (T*)dx, H, W, C, total);
   });
+  return 1;
 }
 
 // ====================================================================================
@@ -1184,29 +1196,29 @@ static bool launch_gn2_backward(const void* dy, const void* x, const void* adden
 
 // gn2 where its plan fits and the cluster launch succeeds; otherwise the two-pass kernels (fp32 at C = 2048, whose
 // 512 vector columns no plan takes, and slabs beyond 16 x 224 KB).
-void launch_gn_relu_forward(const void* x, void* y, const float* gamma, const float* beta, float* partial,
-                            float* stats, int N, int P, int C, bool bf16, cudaStream_t st) {
-  if (launch_gn2_forward(x, y, gamma, beta, stats, N, P, C, bf16, st)) return;
-  launch_gn_relu_forward_2pass(x, y, gamma, beta, partial, stats, N, P, C, bf16, st);
+int launch_gn_relu_forward(const void* x, void* y, const float* gamma, const float* beta, float* partial,
+                           float* stats, int N, int P, int C, bool bf16, cudaStream_t st) {
+  if (launch_gn2_forward(x, y, gamma, beta, stats, N, P, C, bf16, st)) return 1;
+  return launch_gn_relu_forward_2pass(x, y, gamma, beta, partial, stats, N, P, C, bf16, st);
 }
 
-void launch_gn_relu_backward(const void* dy, const void* x, const void* addend, void* dx, const float* gamma,
-                             const float* beta, const float* stats, float* partial, int N, int P, int C, bool bf16,
-                             cudaStream_t st, bool gamma_pos) {
-  if (launch_gn2_backward(dy, x, addend, dx, gamma, beta, stats, N, P, C, bf16, gamma_pos, st)) return;
-  launch_gn_relu_backward_2pass(dy, x, addend, dx, gamma, beta, stats, partial, N, P, C, bf16, st);
+int launch_gn_relu_backward(const void* dy, const void* x, const void* addend, void* dx, const float* gamma,
+                            const float* beta, const float* stats, float* partial, int N, int P, int C, bool bf16,
+                            cudaStream_t st, bool gamma_pos) {
+  if (launch_gn2_backward(dy, x, addend, dx, gamma, beta, stats, N, P, C, bf16, gamma_pos, st)) return 1;
+  return launch_gn_relu_backward_2pass(dy, x, addend, dx, gamma, beta, stats, partial, N, P, C, bf16, st);
 }
 
-void launch_gn_stats(const void* x, float* partial, float* stats, int N, int P, int C, bool bf16, cudaStream_t st) {
+int launch_gn_stats(const void* x, float* partial, float* stats, int N, int P, int C, bool bf16, cudaStream_t st) {
   const int V = bf16 ? 8 : 4, cols = C / V;
   const size_t nvec = (size_t)P * cols;
   const int tiles = (int)((nvec + gn2::ST_TILE - 1) / gn2::ST_TILE);
   if (cols <= gn2::ST_TH && gn2::ST_TH % cols == 0 && C % V == 0 && tiles * 64 <= GN_WS_FLOATS_PER_SAMPLE) {
     DISPATCH_T(bf16, (gn2::stats_kernel<T><<<dim3(tiles, N), gn2::ST_TH, 0, st>>>((const T*)x, partial, P, C, tiles)));
     DISPATCH_T(bf16, (gn_finalize_kernel<T><<<N, 32, 0, st>>>(partial, stats, P, C, tiles)));
-    return;
+    return 2;
   }
-  launch_gn_stats_2pass(x, partial, stats, N, P, C, bf16, st);
+  return launch_gn_stats_2pass(x, partial, stats, N, P, C, bf16, st);
 }
 
 }  // namespace dp

@@ -54,9 +54,10 @@ __global__ void __launch_bounds__(1024) paste_kernel(const float* __restrict__ x
     }
   }
 }
-void launch_paste(const float* x, const float* mask, const float* pattern, float* adv_x, float* l2, float* scale,
-                  int B, int H, int W, float eps, cudaStream_t st) {
+int launch_paste(const float* x, const float* mask, const float* pattern, float* adv_x, float* l2, float* scale,
+                 int B, int H, int W, float eps, cudaStream_t st) {
   paste_kernel<<<B, 1024, 0, st>>>(x, mask, pattern, adv_x, l2, scale, H * W, eps);
+  return 1;
 }
 
 // =====================================================================================
@@ -298,7 +299,7 @@ void get_expand_last(int* out4) { for (int i = 0; i < 4; ++i) out4[i] = g_k1_las
 void set_expand_tuning(int rows, int sg, int mode) { g_k1_rows = rows < 0 ? 0 : rows; g_k1_sg = sg < 0 ? 0 : sg; g_k1_mode = mode; }
 
 template <typename T, int CP, bool FUSED>
-static void expand_launch(const ExpandParams& p, int num_sms, cudaStream_t st) {
+static int expand_launch(const ExpandParams& p, int num_sms, cudaStream_t st) {
   if (g_k1_rows == -2) {
     const char* e = getenv("DORPATCH_K1_ROWS"); g_k1_rows = e ? atoi(e) : 0;
     const char* g = getenv("DORPATCH_K1_SG"); g_k1_sg = g ? atoi(g) : 0;
@@ -344,6 +345,7 @@ static void expand_launch(const ExpandParams& p, int num_sms, cudaStream_t st) {
   q.mode = g_k1_mode;
   g_k1_last[0] = best_R; g_k1_last[1] = best_sg; g_k1_last[2] = best_grid; g_k1_last[3] = resident(best_R);
   expand_kernel<T, CP, FUSED><<<best_grid, EXP_THREADS, smem, st>>>(q);
+  return 1;
 }
 
 // f(T{}, integral_constant<int, CP>{}) for an activation type and channels per pixel, Cp in {3, 4, 8} (the engine
@@ -359,14 +361,15 @@ static void dispatch_t_cp(bool bf16, int Cp, F&& f) {
   else by_cp(0.f);
 }
 
-void launch_expand(const float* img, const float* x, const float* mask, const float* pattern, const float* scale,
-                   const int16_t* rects, void* out, int B, int S, int n0, int n, int H, int W, int Cp, bool bf16,
-                   bool fused, int num_sms, cudaStream_t st) {
+int launch_expand(const float* img, const float* x, const float* mask, const float* pattern, const float* scale,
+                  const int16_t* rects, void* out, int B, int S, int n0, int n, int H, int W, int Cp, bool bf16,
+                  bool fused, int num_sms, cudaStream_t st) {
   ExpandParams p{img, x, mask, pattern, scale, rects, out, B, S, n0, n, H, W, 1, EXP_R_DEFAULT, 0};
+  int k = 0;
   dispatch_t_cp(bf16, Cp, [&](auto t, auto cp) {
-    if (fused) expand_launch<decltype(t), cp, true>(p, num_sms, st);
-    else expand_launch<decltype(t), cp, false>(p, num_sms, st);
+    k = fused ? expand_launch<decltype(t), cp, true>(p, num_sms, st) : expand_launch<decltype(t), cp, false>(p, num_sms, st);
   });
+  return k;
 }
 
 // =====================================================================================
@@ -447,21 +450,23 @@ __global__ void __launch_bounds__(256) reduce_affine_kernel(const T* __restrict_
   }
 }
 
-void launch_expand_affine(const float* adv, const float* xf, const int16_t* rects, void* out, int S, int n0, int n,
-                          int H, int W, int Cp, bool bf16, cudaStream_t st) {
+int launch_expand_affine(const float* adv, const float* xf, const int16_t* rects, void* out, int S, int n0, int n,
+                         int H, int W, int Cp, bool bf16, cudaStream_t st) {
   dim3 grid((H * W + 255) / 256, n);
   dispatch_t_cp(bf16, Cp, [&](auto t, auto cp) {
     using T = decltype(t);
     expand_affine_kernel<T, cp><<<grid, 256, 0, st>>>(adv, xf, rects, (T*)out, S, n0, H, W);
   });
+  return 1;
 }
-void launch_reduce_affine(const void* dz, const float* adv, const float* xf, const int16_t* rects, float* G, int S, int n0,
-                          int n, int H, int W, int Cp, bool bf16, cudaStream_t st) {
+int launch_reduce_affine(const void* dz, const float* adv, const float* xf, const int16_t* rects, float* G, int S, int n0,
+                         int n, int H, int W, int Cp, bool bf16, cudaStream_t st) {
   dim3 grid((H * W + 255) / 256, n);
   dispatch_t_cp(bf16, Cp, [&](auto t, auto cp) {
     using T = decltype(t);
     reduce_affine_kernel<T, cp><<<grid, 256, 0, st>>>((const T*)dz, adv, xf, rects, G, S, n0, H, W);
   });
+  return 1;
 }
 
 // =====================================================================================
@@ -507,14 +512,16 @@ __global__ void cw_kernel(const float* __restrict__ logits, const int32_t* __res
     }
   }
 }
-void launch_cw(const float* logits, const int32_t* y, const uint8_t* targeted, float confidence, float inv_s_total,
-               float* loss, int32_t* preds, float* dlogits, int N, int K, cudaStream_t st) {
+int launch_cw(const float* logits, const int32_t* y, const uint8_t* targeted, float confidence, float inv_s_total,
+              float* loss, int32_t* preds, float* dlogits, int N, int K, cudaStream_t st) {
   const size_t threads = (size_t)N * 32;
   cw_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(logits, y, targeted, confidence, inv_s_total, loss, preds, dlogits, N, K);
+  return 1;
 }
-void launch_argmax(const float* logits, int32_t* preds, int N, int K, cudaStream_t st) {
+int launch_argmax(const float* logits, int32_t* preds, int N, int K, cudaStream_t st) {
   const size_t threads = (size_t)N * 32;
   cw_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(logits, nullptr, nullptr, 0.f, 0.f, nullptr, preds, nullptr, N, K);
+  return 1;
 }
 
 // =====================================================================================
@@ -560,13 +567,14 @@ __global__ void __launch_bounds__(256) reduce_kernel(const T* __restrict__ dz, c
     }
   }
 }
-void launch_reduce(const void* dz, const int16_t* rects, float* G, int B, int S, int n0, int n, int H, int W,
-                   int Cp, bool bf16, cudaStream_t st) {
+int launch_reduce(const void* dz, const int16_t* rects, float* G, int B, int S, int n0, int n, int H, int W,
+                  int Cp, bool bf16, cudaStream_t st) {
   const dim3 grid((H * W + 255) / 256, images_touched(S, n0, n));
   dispatch_t_cp(bf16, Cp, [&](auto t, auto cp) {
     using T = decltype(t);
     reduce_kernel<T, cp><<<grid, 256, 0, st>>>((const T*)dz, rects, G, S, n0, n, H, W);
   });
+  return 1;
 }
 
 // =====================================================================================
@@ -628,8 +636,9 @@ __global__ void __launch_bounds__(1024) struct_kernel(const float* __restrict__ 
   const float tot = block_sum(s, red);
   if (threadIdx.x == 0) loss[b] = tot * inv_hw;
 }
-void launch_struct(const float* adv_x, const float* x, float* loss_struc, float* dLs, int B, int H, int W, cudaStream_t st) {
+int launch_struct(const float* adv_x, const float* x, float* loss_struc, float* dLs, int B, int H, int W, cudaStream_t st) {
   struct_kernel<<<B, 1024, 0, st>>>(adv_x, x, loss_struc, dLs, H, W);
+  return 1;
 }
 
 // =====================================================================================
@@ -701,9 +710,10 @@ __global__ void __launch_bounds__(1024) maskreg_kernel(const float* __restrict__
     for (int i = 0; i < NW; ++i) win_dev[(size_t)b * 64 + i] = 2.0f * (ws[i] - mean) / (NW - 1);
   }
 }
-void launch_maskreg(const float* mask, float* loss_density, float* group_lasso, float* win_dev, float* grp_ss,
-                    int B, int H, int W, int unit, cudaStream_t st) {
+int launch_maskreg(const float* mask, float* loss_density, float* group_lasso, float* win_dev, float* grp_ss,
+                   int B, int H, int W, int unit, cudaStream_t st) {
   maskreg_kernel<<<B, 1024, 0, st>>>(mask, loss_density, group_lasso, win_dev, grp_ss, H, W, unit);
+  return 1;
 }
 
 // =====================================================================================
@@ -748,13 +758,14 @@ __global__ void __launch_bounds__(256) update_kernel(const float* __restrict__ x
     if (step != 0.f) mask[(size_t)b * HW + i] = fminf(fmaxf(m - step * sgn(gm), lo), hi);
   }
 }
-void launch_update(const float* x, float* mask, float* pattern, const float* G, const float* dLs,
-                   const float* scale, const float* win_dev, const float* grp_ss, const float* lr,
-                   const float* structured, const float* coeff_gl, float density, float lo, float hi, int stage,
-                   float* gp_out, float* gm_out, const float* gp_bias, int B, int H, int W, int unit, cudaStream_t st) {
+int launch_update(const float* x, float* mask, float* pattern, const float* G, const float* dLs,
+                  const float* scale, const float* win_dev, const float* grp_ss, const float* lr,
+                  const float* structured, const float* coeff_gl, float density, float lo, float hi, int stage,
+                  float* gp_out, float* gm_out, const float* gp_bias, int B, int H, int W, int unit, cudaStream_t st) {
   update_kernel<<<dim3((H * W + 255) / 256, B), 256, 0, st>>>(x, mask, pattern, G, dLs, scale, win_dev, grp_ss, lr,
                                                               structured, coeff_gl, density, lo, hi, stage, gp_out,
                                                               gm_out, gp_bias, H, W, unit);
+  return 1;
 }
 
 // =====================================================================================
@@ -771,9 +782,10 @@ __global__ void window_sum_kernel(const float* __restrict__ t, float* __restrict
     for (int dx = 0; dx < k; ++dx) { const float v = tb[(gy * k + dy) * W + gx * k + dx]; s += square ? v * v : v; }
   out[(size_t)b * NG + g] = s;
 }
-void launch_window_sum(const float* t, float* out, int B, int H, int W, int k, bool square, cudaStream_t st) {
+int launch_window_sum(const float* t, float* out, int B, int H, int W, int k, bool square, cudaStream_t st) {
   const int NG = (H / k) * (W / k);
   window_sum_kernel<<<dim3((NG + 127) / 128, B), 128, 0, st>>>(t, out, H, W, k, square ? 1 : 0);
+  return 1;
 }
 
 // =====================================================================================
@@ -806,9 +818,10 @@ __global__ void failed_update_kernel(uint32_t* __restrict__ bits, int words, con
   __syncthreads();
   if (threadIdx.x == 0) { int t = 0; for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i]; count[b] = t; }
 }
-void launch_failed_update(uint32_t* bits, int words, const int32_t* idx, const float* loss, const int32_t* nff, const uint8_t* active,
-                          int B, int S, float thresh, int32_t* count, cudaStream_t st) {
+int launch_failed_update(uint32_t* bits, int words, const int32_t* idx, const float* loss, const int32_t* nff, const uint8_t* active,
+                         int B, int S, float thresh, int32_t* count, cudaStream_t st) {
   failed_update_kernel<<<B, 128, 0, st>>>(bits, words, idx, loss, nff, active, S, thresh, count);
+  return 1;
 }
 
 }  // namespace dp

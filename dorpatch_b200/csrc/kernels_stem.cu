@@ -120,14 +120,16 @@ __global__ void stem_pack_kernel(const __nv_bfloat16* __restrict__ w_krsc, __nv_
   w_kn[i] = v;
 }
 
-void launch_stem_pack(const void* w_krsc, void* w_kn, int cin_pad, cudaStream_t st) {
+int launch_stem_pack(const void* w_krsc, void* w_kn, int cin_pad, cudaStream_t st) {
   stem_pack_kernel<<<(stem::KP * 64 + 255) / 256, 256, 0, st>>>((const __nv_bfloat16*)w_krsc, (__nv_bfloat16*)w_kn, cin_pad);
+  return 1;
 }
-void launch_stem_forward(const void* in, const void* w_kn, void* out, int N, int H, int W, cudaStream_t st) {
+int launch_stem_forward(const void* in, const void* w_kn, void* out, int N, int H, int W, cudaStream_t st) {
   cudaFuncSetAttribute(stem_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)stem::SMEM);
   const int Ho = H / 2;
   dim3 grid((Ho + stem::TOY - 1) / stem::TOY, N);
   stem_fwd_kernel<<<grid, stem::THREADS, stem::SMEM, st>>>((const __nv_bfloat16*)in, (const __nv_bfloat16*)w_kn, (__nv_bfloat16*)out, H, W);
+  return 1;
 }
 
 
@@ -374,22 +376,23 @@ __global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_reduce_kernel(Src 
 }
 
 template <class Src>
-static void launch_stem_bwd(Src in, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int S, int n0, int n,
-                            int H, int W, cudaStream_t st) {
+static int launch_stem_bwd(Src in, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int S, int n0, int n,
+                           int H, int W, cudaStream_t st) {
   cudaFuncSetAttribute(stem_bwd_reduce_kernel<Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Src::SMEM);
   const int tiles = ((H / 2 + stemb::TI - 1) / stemb::TI) * ((W / 2 + stemb::TJ - 1) / stemb::TJ);
   stem_bwd_reduce_kernel<Src><<<dim3(tiles, images_touched(S, n0, n)), stemb::THREADS, Src::SMEM, st>>>(
       in, (const __nv_bfloat16*)w_krsc, cin_pad, rects, G, S, n0, n, H, W);
+  return 1;
 }
-void launch_stem_bwd_reduce(const void* dY, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int B, int S,
-                            int n0, int n, int H, int W, cudaStream_t st) {
+int launch_stem_bwd_reduce(const void* dY, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int B, int S,
+                           int n0, int n, int H, int W, cudaStream_t st) {
   (void)B;
-  launch_stem_bwd(stemb::DyPatch{(const __nv_bfloat16*)dY}, w_krsc, cin_pad, rects, G, S, n0, n, H, W, st);
+  return launch_stem_bwd(stemb::DyPatch{(const __nv_bfloat16*)dY}, w_krsc, cin_pad, rects, G, S, n0, n, H, W, st);
 }
-void launch_stem_bwd_pool_reduce(const void* dpool, const int8_t* amax, const void* w_krsc, int cin_pad, const int16_t* rects,
-                                 float* G, int B, int S, int n0, int n, int H, int W, cudaStream_t st) {
+int launch_stem_bwd_pool_reduce(const void* dpool, const int8_t* amax, const void* w_krsc, int cin_pad, const int16_t* rects,
+                                float* G, int B, int S, int n0, int n, int H, int W, cudaStream_t st) {
   (void)B;
-  launch_stem_bwd(stemb::PoolPatch{(const __nv_bfloat16*)dpool, amax}, w_krsc, cin_pad, rects, G, S, n0, n, H, W, st);
+  return launch_stem_bwd(stemb::PoolPatch{(const __nv_bfloat16*)dpool, amax}, w_krsc, cin_pad, rects, G, S, n0, n, H, W, st);
 }
 
 }  // namespace dp

@@ -38,11 +38,12 @@ __global__ void gn_apply_kernel(const T* __restrict__ x, T* __restrict__ y, cons
   y[i] = from_float<T>(fmaxf(fmaf(sa, to_float(x[i]), sb), 0.f));
 }
 
-void launch_gn_apply(const void* x, void* y, const float* gamma, const float* beta, const float* stats, int N, int P,
-                     int C, bool bf16, cudaStream_t st) {
+int launch_gn_apply(const void* x, void* y, const float* gamma, const float* beta, const float* stats, int N, int P,
+                    int C, bool bf16, cudaStream_t st) {
   const size_t total = (size_t)N * P * C;
   WG_DISPATCH_T(bf16, (gn_apply_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const T*)x, (T*)y, gamma, beta,
                                                                                             stats, P, C, total)));
+  return 1;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -83,11 +84,12 @@ __global__ void __launch_bounds__(256) gn_affine_partial_kernel(const T* __restr
   }
 }
 
-void launch_gn_affine_partial(const void* dy, const void* x, const float* gamma, const float* beta, const float* stats,
-                              float* partial, int N, int P, int C, bool bf16, cudaStream_t st) {
+int launch_gn_affine_partial(const void* dy, const void* x, const float* gamma, const float* beta, const float* stats,
+                             float* partial, int N, int P, int C, bool bf16, cudaStream_t st) {
   dim3 grid((C + 31) / 32, N);
   WG_DISPATCH_T(bf16, (gn_affine_partial_kernel<T><<<grid, 256, 0, st>>>((const T*)dy, (const T*)x, gamma, beta, stats,
                                                                           partial, P, C)));
+  return 1;
 }
 
 // acc[j] += sum_{r < rows} src[r * M + j], rows summed in order
@@ -99,8 +101,9 @@ __global__ void colsum_add_kernel(const float* __restrict__ src, float* __restri
   acc[j] += s;
 }
 
-void launch_colsum_add(const float* src, float* acc, int rows, int M, cudaStream_t st) {
+int launch_colsum_add(const float* src, float* acc, int rows, int M, cudaStream_t st) {
   colsum_add_kernel<<<(M + 255) / 256, 256, 0, st>>>(src, acc, rows, M);
+  return 1;
 }
 
 __global__ void add_bf16_kernel(const __nv_bfloat16* __restrict__ src, float* __restrict__ acc, size_t n) {
@@ -108,8 +111,9 @@ __global__ void add_bf16_kernel(const __nv_bfloat16* __restrict__ src, float* __
   if (i < n) acc[i] += __bfloat162float(src[i]);
 }
 
-void launch_add_bf16(const void* src, float* acc, size_t n, cudaStream_t st) {
+int launch_add_bf16(const void* src, float* acc, size_t n, cudaStream_t st) {
   add_bf16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const __nv_bfloat16*)src, acc, n);
+  return 1;
 }
 
 // out[i] = (accumulate ? out[i] : 0) + a[i] (+ b[i])
@@ -122,8 +126,9 @@ __global__ void vec_finish_kernel(const float* __restrict__ a, const float* __re
   out[i] = accumulate ? out[i] + v : v;
 }
 
-void launch_vec_finish(const float* a, const float* b, float* out, size_t n, bool accumulate, cudaStream_t st) {
+int launch_vec_finish(const float* a, const float* b, float* out, size_t n, bool accumulate, cudaStream_t st) {
   vec_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, b, out, n, accumulate ? 1 : 0);
+  return 1;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -167,9 +172,10 @@ __global__ void __launch_bounds__(256) ws_backward_kernel(const float* __restric
   }
 }
 
-void launch_ws_backward(const float* w_raw, const float* g_a, const float* g_b, float* out, int O, int I, int kh, int kw,
-                        int Ipad, bool accumulate, cudaStream_t st) {
+int launch_ws_backward(const float* w_raw, const float* g_a, const float* g_b, float* out, int O, int I, int kh, int kw,
+                       int Ipad, bool accumulate, cudaStream_t st) {
   ws_backward_kernel<<<O, 256, 0, st>>>(w_raw, g_a, g_b, out, I, kh * kw, Ipad, accumulate ? 1 : 0);
+  return 1;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -270,8 +276,8 @@ __global__ void stem_wgrad_reduce_kernel(const float* __restrict__ partial, floa
 
 size_t stem_wgrad_partial_floats() { return (size_t)stemw::MAX_CTAS * 64 * stemw::KP; }
 
-void launch_stem_wgrad(const void* in, const void* dY, float* partial, float* acc, int N, int H, int W, int cin_pad,
-                       cudaStream_t st) {
+int launch_stem_wgrad(const void* in, const void* dY, float* partial, float* acc, int N, int H, int W, int cin_pad,
+                      cudaStream_t st) {
   using namespace stemw;
   const long long Q = (long long)N * (H / 2) * (W / 2);
   long long ctas = (Q + 8 * QS - 1) / (8 * QS);                   // at least 8 steps per CTA
@@ -282,6 +288,7 @@ void launch_stem_wgrad(const void* in, const void* dY, float* partial, float* ac
   ctas = (Q + per - 1) / per;
   stem_wgrad_kernel<<<(unsigned)ctas, THREADS, 0, st>>>((const __nv_bfloat16*)in, (const __nv_bfloat16*)dY, partial, H, W, Q, per);
   stem_wgrad_reduce_kernel<<<(64 * KR + 255) / 256, 256, 0, st>>>(partial, acc, (int)ctas, cin_pad);
+  return 2;
 }
 
 }  // namespace dp

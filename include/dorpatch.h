@@ -80,7 +80,8 @@ int32_t dp_engine_load_weights_dev(dp_engine* e, int32_t n_tensors, const char* 
 
 /* bytes of device memory the engine holds (workspace + weights) */
 int64_t dp_engine_device_bytes(const dp_engine* e);
-/* number of CUDA kernels / library launches issued by the engine since create */
+/* launches since create: every CUDA kernel the engine's own code enqueued, plus one per cuDNN / cublasLt call, whatever
+ * the library enqueues inside it (the trials of library algorithm selection are not counted) */
 int64_t dp_engine_launch_count(const dp_engine* e);
 /* number of dp_attack_grad calls served by replaying a captured CUDA graph (the launch count above still counts the
  * kernels each replay executes) */
