@@ -81,6 +81,10 @@ SIGNATURES = {
     "dp_debug_maxpool": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp]),
     "dp_debug_gn_gemm": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_vp]),
     "dp_debug_gn": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp]),
+    "dp_expand_bank": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp]),
+    "dp_predict_bank": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    "dp_eot_forward_bank": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp]),
+    "dp_debug_stem_bwd_reduce_bank": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
 }
 
 _lib = None

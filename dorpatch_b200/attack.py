@@ -553,23 +553,30 @@ class DorPatch(object):
     def collect_failure(self, adv_x, y, mask_set_universe, targeted, model, batch_size=128, transforms=None):
         """attack.py:384-406 with the reference's signature: `mask_set_universe` may be the bool
         tensor of the reference or an int16 rectangle table [n,2,4]."""
-        if isinstance(mask_set_universe, np.ndarray):
-            net = unwrap_native(model)
-            eng = net.engine(adv_x.shape[-1], max_images=adv_x.shape[0])
-            n = mask_set_universe.shape[0]
-            rects = _masks.gather(mask_set_universe, np.arange(n))
-            B = adv_x.shape[0]
-            preds = eng.predict(adv_x.contiguous().float(), n, np.broadcast_to(rects, (B,) + rects.shape))
-            yv = np.asarray(y.tolist() if torch.is_tensor(y) else y).reshape(B, -1)[:, :1]
-            f = preds.reshape(B, n) == yv
-            if targeted:
-                f = ~f
-            failed = np.nonzero(f.any(0))[0].tolist()
-        else:
-            # the reference's bool universe [n,1,H,W] (True = keep): every mask is "all but <= 4 rectangles", which is
-            # what the native K1 kernel consumes -- recover the rectangles and take the same dp_predict path
+        bank = None
+        if not isinstance(mask_set_universe, np.ndarray):
+            # the reference's bool universe [n,1,H,W] (True = keep): masks that are "all but <= 2 rectangles" take the
+            # rectangle path of the native K1 kernel; any other universe is packed into a mask bank (dp_predict_bank)
             if transforms is not None:
                 raise NotImplementedError("collect_failure(transforms=...) is an unused hook of the reference (attack.py:395-396)")
-            return self.collect_failure(adv_x, y, _masks.from_bool(mask_set_universe), targeted, model, batch_size)
+            try:
+                mask_set_universe = _masks.from_bool(mask_set_universe)
+            except NotImplementedError:
+                bank = _masks.pack_bank(mask_set_universe, device=adv_x.device)
+        net = unwrap_native(model)
+        eng = net.engine(adv_x.shape[-1], max_images=adv_x.shape[0])
+        B = adv_x.shape[0]
+        if bank is None:
+            n = mask_set_universe.shape[0]
+            rects = _masks.gather(mask_set_universe, np.arange(n))
+            preds = eng.predict(adv_x.contiguous().float(), n, np.broadcast_to(rects, (B,) + rects.shape))
+        else:
+            n = bank.shape[0]
+            preds = eng.predict(adv_x.contiguous().float(), n, bank=bank, idx=np.tile(np.arange(n), B))
+        yv = np.asarray(y.tolist() if torch.is_tensor(y) else y).reshape(B, -1)[:, :1]
+        f = preds.reshape(B, n) == yv
+        if targeted:
+            f = ~f
+        failed = np.nonzero(f.any(0))[0].tolist()
         print(">> %d failures collected!" % len(failed))
         return failed

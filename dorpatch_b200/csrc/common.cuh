@@ -140,4 +140,26 @@ struct Occlusion {
   }
 };
 
+// ----------------------------------------------------------------------------
+// Occlusion bank (MaskBank, kernels.h): the only place its format is decoded.  Mask m is H rows of words(W) uint32;
+// bit w % 32 of word w / 32 of row h set = pixel (h, w) occluded.  A sample selects two masks (idx[n], -1 = none) and
+// is occluded where either is set.
+// ----------------------------------------------------------------------------
+namespace occl_bank {
+__device__ __forceinline__ int words(int W) { return bank_words(W); }
+// sample n's two mask indices
+__device__ __forceinline__ int2 select(const MaskBank& b, int n) { return __ldg(reinterpret_cast<const int2*>(b.idx) + n); }
+// word k of row h of the occlusion of a sample that selected `sel`
+__device__ __forceinline__ uint32_t row_bits(const MaskBank& b, int2 sel, int h, int k) {
+  const size_t mw = (size_t)b.H * words(b.W), o = (size_t)h * words(b.W) + k;
+  uint32_t v = 0u;
+  if (sel.x >= 0) v |= __ldg(b.bits + sel.x * mw + o);
+  if (sel.y >= 0) v |= __ldg(b.bits + sel.y * mw + o);
+  return v;
+}
+__device__ __forceinline__ bool hit(const MaskBank& b, int2 sel, int h, int w) {
+  return (row_bits(b, sel, h, w >> 5) >> (w & 31)) & 1u;
+}
+}  // namespace occl_bank
+
 }  // namespace dp

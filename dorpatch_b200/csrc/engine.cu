@@ -180,10 +180,14 @@ struct dp_engine {
   // activations (pre-norm outputs, GroupNorm statistics, max-pool argmax) the lane still holds.
   // xf: the forward warped its samples (dp_eot_forward_xform) with the transforms in eot_xf_d.
   // whole: the forward's K1 wrote every sample to net_in_all (a held chunk's input is its slice there).
-  struct EotSig { int64_t gen = -1; const float* img = nullptr; int B = 0, S = 0; bool rects = false, xf = false, whole = false; };
+  // bank: the forward occluded from this caller-owned mask bank with the indices in eot_bank_idx_d (dp_eot_forward_bank).
+  struct EotSig { int64_t gen = -1; const float* img = nullptr; int B = 0, S = 0; bool rects = false, xf = false, whole = false;
+                  const uint32_t* bank = nullptr; };
   int64_t fwd_gen = 0;
   EotSig eot;
   int16_t* eot_rects_d = nullptr; int eot_rects_cap = 0;   // the forward's rectangles (rects_d is shared scratch)
+  int32_t* eot_bank_idx_d = nullptr; int eot_bank_idx_cap = 0;   // the forward's mask indices [N][2]
+  int32_t* bank_idx_d = nullptr; int bank_idx_cap = 0;     // scratch: the mask indices of dp_predict_bank / dp_expand_bank
   float* eot_xf_d = nullptr; int eot_xf_cap = 0;           // the forward's transforms (xf_d is dp_attack_grad's)
   void forward_clobbered() {
     ++fwd_gen;
@@ -817,7 +821,11 @@ struct dp_engine {
   // Wgrad: the weight-gradient pass of one chunk (dp_eot_backward_params): accumulates d/d(parameter) of the requested
   // parameters (`want`) into the lane's accumulators.  input: the chunk's network input.  need_dx: the input gradient
   // is wanted too (else the backward stops at block `lo`, the lowest block whose gradients are wanted).
-  struct FusedReduce { const int16_t* rects; float* G; int B, S, n0; };
+  struct FusedReduce {
+    const int16_t* rects; float* G; int B, S, n0;
+    dp::MaskBank bank;                                   // bank.idx null: occluded by rects
+    const dp::MaskBank* bank_or_null() const { return bank.idx ? &bank : nullptr; }
+  };
   struct Wgrad { const void* input; bool need_dx; int lo; };
   struct EotIn;
 
@@ -886,10 +894,11 @@ struct dp_engine {
       return dp::launch_stem_wgrad(input, dY, partial, acc, N, e->H, e->H, cin_pad, st);
     }
     int fused_reduce(const void* dY, const FusedReduce& fr, int N, cudaStream_t st) const {
-      return dp::launch_stem_bwd_reduce(dY, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st);
+      return dp::launch_stem_bwd_reduce(dY, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st, fr.bank_or_null());
     }
     int fused_pool_reduce(const void* dpool, const int8_t* amax, const FusedReduce& fr, int N, cudaStream_t st) const {
-      return dp::launch_stem_bwd_pool_reduce(dpool, amax, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st);
+      return dp::launch_stem_bwd_pool_reduce(dpool, amax, conv.w, conv.cin_pad, fr.rects, fr.G, fr.B, fr.S, fr.n0, N, e->H, e->H, st,
+                                             fr.bank_or_null());
     }
     // input [N,H,H,in_ch] -> conv -> max-pool into L.x0 (train: keep the argmax for the backward)
     void forward(const Lane& L, int N, const void* input, bool train, cudaStream_t st) const {
@@ -1087,18 +1096,22 @@ struct dp_engine {
   // ---- EOT input: K1 and its adjoint K1^T for the chunk loops and the dp_expand* entry points ------------------------
   // What K1 expands into network input: `img` (plain, or warped per sample by the transforms `xf` [B*S][8]) or the
   // attack's paste of x / mask / pattern with the clip scale (fused), repeated S times per image and occluded by
-  // `rects` [B*S][4][4] (null: none).
+  // `rects` [B*S][4][4] (null: none), or by the mask bank `bank` when bank.idx is set (img only, not warped).
   struct EotIn {
     const float* img;
     const float *x, *mask, *pattern, *scale;
     const float* xf;
     const int16_t* rects;
     int B, S;
+    dp::MaskBank bank;
     static EotIn image(const float* img, const float* xf, const int16_t* rects, int B, int S) {
-      return EotIn{img, nullptr, nullptr, nullptr, nullptr, xf, rects, B, S};
+      return EotIn{img, nullptr, nullptr, nullptr, nullptr, xf, rects, B, S, dp::MaskBank{}};
     }
     static EotIn paste(const float* x, const float* mask, const float* pattern, const float* scale, const int16_t* rects, int B, int S) {
-      return EotIn{nullptr, x, mask, pattern, scale, nullptr, rects, B, S};
+      return EotIn{nullptr, x, mask, pattern, scale, nullptr, rects, B, S, dp::MaskBank{}};
+    }
+    static EotIn banked(const float* img, const dp::MaskBank& bank, int B, int S) {
+      return EotIn{img, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, S, bank};
     }
   };
   // K1 for samples [n0, n0 + n) into dst.  Algorithmic bytes: the samples written, plus the fp32 planes read once per
@@ -1106,7 +1119,13 @@ struct dp_engine {
   void launch_k1(const EotIn& in, int n0, int n, void* dst, cudaStream_t st) {
     const bool fused = in.x != nullptr;
     const double bytes = (double)n * H * H * 3 * es + (fused ? 7.0 : 3.0) * H * H * 4 * (double)n / in.S;
-    if (in.xf)
+    if (in.bank.idx) {                                   // + each sample's bank rows (one mask) and indices
+      if (in.xf || fused) fail("K1: a mask bank occludes an unwarped image only");
+      const double bank_bytes = (double)n * (H * dp::bank_words(H) * 4.0 + 8.0);
+      run("expand_k1_bank", bytes + bank_bytes, 0, st, [&] {
+        return dp::launch_expand(in.img, nullptr, nullptr, nullptr, nullptr, nullptr, dst, in.B, in.S, n0, n, H, H, stem.in_ch, bf16, false, num_sms, st, &in.bank);
+      });
+    } else if (in.xf)
       run("expand_affine", bytes, 0, st, [&] { return dp::launch_expand_affine(in.img, in.xf, in.rects, dst, in.S, n0, n, H, H, stem.in_ch, bf16, st); });
     else
       run("expand_k1", bytes, 0, st, [&] {
@@ -1125,11 +1144,14 @@ struct dp_engine {
   // gradient (weight gradients only).
   void backward_reduce(const Lane& L, const EotIn& in, int n0, int n, float* G, cudaStream_t st, const Wgrad* wg = nullptr) {
     const bool fuse = G && stem.folds_k1t(in);
-    const FusedReduce fr{in.rects, G, in.B, in.S, n0};
+    const FusedReduce fr{in.rects, G, in.B, in.S, n0, in.bank};
     const void* dx = backward(L, n, L.dlogits, st, fuse ? &fr : nullptr, wg);
     if (!G || fuse) return;
     const double bytes = (double)n * H * H * 3 * es + 3.0 * H * H * 4 * (double)n / in.S;
-    if (in.xf)
+    if (in.bank.idx)
+      run("reduce_k1t_bank", bytes + (double)n * (H * dp::bank_words(H) * 4.0 + 8.0), 0, st,
+          [&] { return dp::launch_reduce(dx, nullptr, G, in.B, in.S, n0, n, H, H, stem.dx_ch, bf16, st, &in.bank); });
+    else if (in.xf)
       run("reduce_affine", bytes, 0, st, [&] { return dp::launch_reduce_affine(dx, in.img, in.xf, in.rects, G, in.S, n0, n, H, H, stem.dx_ch, bf16, st); });
     else
       run("reduce_k1t", bytes, 0, st, [&] { return dp::launch_reduce(dx, in.rects, G, in.B, in.S, n0, n, H, H, stem.dx_ch, bf16, st); });
@@ -1153,6 +1175,21 @@ struct dp_engine {
   void h2d_samples(const int16_t* rects_host, int N, cudaStream_t st) {
     ensure_samples(N);                   // every per-sample buffer holds N rows: rects_d does not grow on its own
     if (rects_host != nullptr) stage(rects_d, cap_samples, rects_host, N, dp::RECT_SHORTS * sizeof(int16_t), st);
+  }
+  // The mask-bank occlusion of N samples: checks the indices idx_host [N][2] against n_bank masks, stages them into
+  // `table` and returns the MaskBank the kernels read.
+  dp::MaskBank stage_bank(int32_t*& table, int& cap, const uint32_t* bank, int n_bank, const int32_t* idx_host, int N,
+                          const char* fn, cudaStream_t st) {
+    if (n_bank < 1) fail("%s: n_bank=%d < 1", fn, n_bank);
+    if (!idx_host) fail("%s: null index array", fn);
+    if (dp::bank_words(H) > 32) fail("%s: a mask bank needs img <= 1024 (img=%d)", fn, H);
+    for (size_t i = 0; i < (size_t)N * 2; ++i) {
+      const int32_t k = idx_host[i];
+      if (k < -1 || k >= n_bank) fail("%s: mask index %d of sample %d outside [-1, %d)", fn, k, (int)(i / 2), n_bank);
+      if (k >= 0 && !bank) fail("%s: sample %d selects mask %d of a null bank", fn, (int)(i / 2), k);
+    }
+    stage(table, cap, idx_host, N, 2 * sizeof(int32_t), st);
+    return dp::MaskBank{bank, table, H, H};
   }
   void check_B(int B) const {
     if (B < 1 || B > cfg.max_images) fail("B=%d outside [1, max_images=%d]", B, cfg.max_images);
@@ -1388,6 +1425,17 @@ int32_t dp_expand(dp_engine* e, const float* img, int32_t B, int32_t S, const in
   });
 }
 
+int32_t dp_expand_bank(dp_engine* e, const float* img, int32_t B, int32_t S, const uint32_t* bank_dev, int32_t n_bank,
+                       const int32_t* idx_host, void* out, void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    const int N = B * S;
+    if (!img || N < 1) fail("dp_expand_bank: bad arguments");
+    if (out == nullptr && N > e->chunk) fail("dp_expand_bank: B*S=%d exceeds chunk=%d and no output buffer was given", N, e->chunk);
+    const dp::MaskBank bank = e->stage_bank(e->bank_idx_d, e->bank_idx_cap, bank_dev, n_bank, idx_host, N, "dp_expand_bank", st);
+    e->launch_k1(dp_engine::EotIn::banked(img, bank, B, S), 0, N, out ? out : e->lanes[0].net_in, st);
+  });
+}
+
 int32_t dp_expand_dev(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_dev, void* out, void* stream) {
   return on_engine(e, stream, [&](cudaStream_t st) {
     if (!out) fail("dp_expand_dev needs an output buffer");
@@ -1410,6 +1458,23 @@ int32_t dp_k1_samples_per_launch(const dp_engine* e, int32_t n_samples) {
   return e->k1_whole_ok(n_samples) ? n_samples : std::min(n_samples, e->chunk);
 }
 
+// forward-only scan (collect_failure, PatchCleanser) of N samples expanded from `in`: chunks alternate between the two
+// lanes like dp_attack_grad
+static void predict_chunks(dp_engine* e, const dp_engine::EotIn& in, int N, int32_t* preds_host, float* logits_host, cudaStream_t st) {
+  LaneWalk walk(e, st, N > e->chunk);
+  for (int n0 = 0, c = 0; n0 < N; n0 += e->chunk, ++c) {
+    const int n = std::min(e->chunk, N - n0);
+    const dp_engine::Lane& L = e->lanes[walk.lane_of(c)];
+    cudaStream_t const ls = walk.stream(walk.lane_of(c));
+    e->forward(L, n, e->chunk_input(L, in, n0, n, false, ls), false, ls);
+    e->run(ls, [&] { return dp::launch_argmax(L.logits, e->preds_d + n0, n, e->K, ls); });
+    if (logits_host) CUDA_OK(cudaMemcpyAsync(logits_host + (size_t)n0 * e->K, L.logits, (size_t)n * e->K * 4, cudaMemcpyDeviceToHost, ls));
+  }
+  walk.join();
+  CUDA_OK(cudaMemcpyAsync(preds_host, e->preds_d, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+}
+
 int32_t dp_predict(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host, int32_t* preds_host,
                    float* logits_host, void* stream) {
   return on_engine(e, stream, [&](cudaStream_t st) {
@@ -1418,20 +1483,20 @@ int32_t dp_predict(dp_engine* e, const float* img, int32_t B, int32_t S, const i
     if (N < 1) fail("dp_predict: empty batch");
     e->forward_clobbered();
     e->h2d_samples(rects_host, N, st);
-    const dp_engine::EotIn in = dp_engine::EotIn::image(img, nullptr, rects_host ? e->rects_d : nullptr, B, S);
-    // forward-only scan (collect_failure, PatchCleanser): chunks alternate between the two lanes like dp_attack_grad
-    LaneWalk walk(e, st, N > e->chunk);
-    for (int n0 = 0, c = 0; n0 < N; n0 += e->chunk, ++c) {
-      const int n = std::min(e->chunk, N - n0);
-      const dp_engine::Lane& L = e->lanes[walk.lane_of(c)];
-      cudaStream_t const ls = walk.stream(walk.lane_of(c));
-      e->forward(L, n, e->chunk_input(L, in, n0, n, false, ls), false, ls);
-      e->run(ls, [&] { return dp::launch_argmax(L.logits, e->preds_d + n0, n, e->K, ls); });
-      if (logits_host) CUDA_OK(cudaMemcpyAsync(logits_host + (size_t)n0 * e->K, L.logits, (size_t)n * e->K * 4, cudaMemcpyDeviceToHost, ls));
-    }
-    walk.join();
-    CUDA_OK(cudaMemcpyAsync(preds_host, e->preds_d, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaStreamSynchronize(st));
+    predict_chunks(e, dp_engine::EotIn::image(img, nullptr, rects_host ? e->rects_d : nullptr, B, S), N, preds_host, logits_host, st);
+  });
+}
+
+int32_t dp_predict_bank(dp_engine* e, const float* img, int32_t B, int32_t S, const uint32_t* bank_dev, int32_t n_bank,
+                        const int32_t* idx_host, int32_t* preds_host, float* logits_host, void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    NvtxRange nvtx_("dorpatch.predict_bank");
+    const int N = B * S;
+    if (N < 1) fail("dp_predict_bank: empty batch");
+    const dp::MaskBank bank = e->stage_bank(e->bank_idx_d, e->bank_idx_cap, bank_dev, n_bank, idx_host, N, "dp_predict_bank", st);
+    e->forward_clobbered();
+    e->ensure_samples(N);
+    predict_chunks(e, dp_engine::EotIn::banked(img, bank, B, S), N, preds_host, logits_host, st);
   });
 }
 
@@ -1628,15 +1693,20 @@ int32_t dp_attack_step_host(dp_engine* e, const dp_attack_args* g, const dp_upda
 // Forward: dp_predict's chunk loop with the activations kept (train=true); K1 once for the whole call when its output
 // fits net_in_all, as dp_attack_grad does.  Lane l ends up holding its last chunk.
 // With transforms (xf_host, [N][8]) each chunk's input is dp_attack_grad's affine expansion instead, read from img.
+// With a mask bank (bank_idx_host, [N][2] indices into bank_dev's n_bank masks) each sample is occluded from the bank
+// instead; the backward reads the bank again, so it must stay unchanged until then.
 static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const int16_t* rects_host, const float* xf_host,
-                             float* logits, cudaStream_t st) {
-  NvtxRange nvtx_(xf_host ? "dorpatch.eot_forward_xform" : "dorpatch.eot_forward");
-  const char* fn = xf_host ? "dp_eot_forward_xform" : "dp_eot_forward";
+                             float* logits, cudaStream_t st, const uint32_t* bank_dev = nullptr, int n_bank = 0,
+                             const int32_t* bank_idx_host = nullptr) {
+  NvtxRange nvtx_(xf_host ? "dorpatch.eot_forward_xform" : (bank_idx_host ? "dorpatch.eot_forward_bank" : "dorpatch.eot_forward"));
+  const char* fn = xf_host ? "dp_eot_forward_xform" : (bank_idx_host ? "dp_eot_forward_bank" : "dp_eot_forward");
   if (!img || !logits) fail("%s: null pointer", fn);
   e->check_B(B);
   if (S < 1) fail("%s: S=%d < 1", fn, S);
-  if (!rects_host && !xf_host && S != 1) fail("dp_eot_forward: S=%d without rectangles (plain classification needs S=1)", S);
+  if (!rects_host && !xf_host && !bank_idx_host && S != 1) fail("dp_eot_forward: S=%d without rectangles (plain classification needs S=1)", S);
   const int N = B * S;
+  dp::MaskBank bank{};
+  if (bank_idx_host) bank = e->stage_bank(e->eot_bank_idx_d, e->eot_bank_idx_cap, bank_dev, n_bank, bank_idx_host, N, fn, st);
   if (xf_host)
     for (size_t i = 0; i < (size_t)N * 8; ++i)
       if (!std::isfinite(xf_host[i]))
@@ -1646,7 +1716,8 @@ static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const
   e->eot = dp_engine::EotSig{};
   if (rects_host) e->stage(e->eot_rects_d, e->eot_rects_cap, rects_host, N, dp::RECT_SHORTS * sizeof(int16_t), st);
   if (xf_host) e->stage(e->eot_xf_d, e->eot_xf_cap, xf_host, N, 8 * sizeof(float), st);
-  const dp_engine::EotIn in = dp_engine::EotIn::image(img, xf_host ? e->eot_xf_d : nullptr, rects_host ? e->eot_rects_d : nullptr, B, S);
+  const dp_engine::EotIn in = bank_idx_host ? dp_engine::EotIn::banked(img, bank, B, S)
+                                             : dp_engine::EotIn::image(img, xf_host ? e->eot_xf_d : nullptr, rects_host ? e->eot_rects_d : nullptr, B, S);
   const bool whole = !xf_host && e->ensure_net_in_all(N);
   if (whole) e->launch_k1(in, 0, N, e->net_in_all, st);
   LaneWalk walk(e, st, N > e->chunk);
@@ -1662,6 +1733,7 @@ static void eot_forward_impl(dp_engine* e, const float* img, int B, int S, const
   e->eot.gen = e->fwd_gen; e->eot.img = img; e->eot.B = B; e->eot.S = S; e->eot.rects = rects_host != nullptr;
   e->eot.xf = xf_host != nullptr;
   e->eot.whole = whole;
+  e->eot.bank = bank_idx_host ? bank_dev : nullptr;
 }
 
 // Backward: every chunk through dp_engine::backward and K1^T.  A chunk no lane holds any more is recomputed first (its
@@ -1689,8 +1761,9 @@ static void eot_backward_impl(dp_engine* e, const float* dlogits, float* G, cuda
   e->check_B(e->eot.B);
   const int B = e->eot.B, S = e->eot.S, N = B * S, H = e->H, K = e->K;
   const int n_chunks = (N + e->chunk - 1) / e->chunk, nl = (int)e->lanes.size();
-  const dp_engine::EotIn in = dp_engine::EotIn::image(e->eot.img, e->eot.xf ? e->eot_xf_d : nullptr,
-                                                      e->eot.rects ? e->eot_rects_d : nullptr, B, S);
+  const dp_engine::EotIn in = e->eot.bank ? dp_engine::EotIn::banked(e->eot.img, dp::MaskBank{e->eot.bank, e->eot_bank_idx_d, H, H}, B, S)
+                                          : dp_engine::EotIn::image(e->eot.img, e->eot.xf ? e->eot_xf_d : nullptr,
+                                                                    e->eot.rects ? e->eot_rects_d : nullptr, B, S);
   dp_engine::Wgrad wg{nullptr, G != nullptr, (int)e->blocks.size()};
   if (pc) {
     if (pc->n < 0 || (pc->n > 0 && (!pc->names || !pc->grads))) fail("%s: null name / gradient list", fn);
@@ -1791,6 +1864,14 @@ int32_t dp_eot_forward_xform(dp_engine* e, const float* img, int32_t B, int32_t 
                              const float* xform_host, float* logits_dev, void* stream) {
   return on_engine(e, stream, [&](cudaStream_t st) {
     eot_forward_impl(e, img, B, S, rects_host, xform_host, logits_dev, st);
+  });
+}
+
+int32_t dp_eot_forward_bank(dp_engine* e, const float* img, int32_t B, int32_t S, const uint32_t* bank_dev, int32_t n_bank,
+                            const int32_t* idx_host, float* logits_dev, void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!idx_host) fail("dp_eot_forward_bank: null index array");
+    eot_forward_impl(e, img, B, S, nullptr, nullptr, logits_dev, st, bank_dev, n_bank, idx_host);
   });
 }
 
@@ -1914,6 +1995,18 @@ int32_t dp_debug_stem_bwd_reduce(dp_engine* e, const void* dY, const int16_t* re
     const int N = B * S;
     e->h2d_samples(rects_host, N, st);
     const dp_engine::FusedReduce fr{rects_host ? e->rects_d : nullptr, G, B, S, 0};
+    e->run(st, [&] { return e->stem.fused_reduce(dY, fr, N, st); });
+  });
+}
+
+int32_t dp_debug_stem_bwd_reduce_bank(dp_engine* e, const void* dY, const uint32_t* bank_dev, int32_t n_bank, const int32_t* idx_host,
+                                      int32_t B, int32_t S, float* G, void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (e->stem.fwd != dp_engine::Stem::FWD_OWN) fail("dp_debug_stem_bwd_reduce_bank: the fused stem backward exists for the bf16 engine only");
+    if (!dY || !G || B < 1 || S < 1) fail("dp_debug_stem_bwd_reduce_bank: bad arguments");
+    const int N = B * S;
+    const dp::MaskBank bank = e->stage_bank(e->bank_idx_d, e->bank_idx_cap, bank_dev, n_bank, idx_host, N, "dp_debug_stem_bwd_reduce_bank", st);
+    const dp_engine::FusedReduce fr{nullptr, G, B, S, 0, bank};
     e->run(st, [&] { return e->stem.fused_reduce(dY, fr, N, st); });
   });
 }

@@ -16,6 +16,12 @@ constexpr int GN_WS_FLOATS_PER_SAMPLE = 8192;
 constexpr int GN_WS_FLOATS_EXTRA = 4096;
 // int16 per sample of an occlusion table `rects` [N][RECT_SHORTS]: four rectangles {r0, r1, c0, c1} (common.cuh decodes them)
 constexpr int RECT_SHORTS = 16;
+// The second occlusion format, a mask bank (common.cuh decodes it): `bits` uint32 [M][H][ceil(W/32)] (device, the
+// caller's), bit w % 32 of word w / 32 of row h set = pixel (h, w) occluded; `idx` int32 [N][2] (device): sample n is
+// occluded where mask idx[n][0] or mask idx[n][1] is set, -1 = none.  A launcher given a MaskBank reads it instead of
+// `rects`.
+struct MaskBank { const uint32_t* bits; const int32_t* idx; int H, W; };
+__host__ __device__ inline int bank_words(int W) { return (W + 31) >> 5; }   // words per bank row
 
 // ---- classifier-side kernels (kernels_net.cu) --------------------------------------
 // timm StdConv2d standardisation of OIHW fp32 weights -> KRSC (NHWC filter), channel-padded.
@@ -55,12 +61,14 @@ int launch_subsample2_adjoint_add(const void* dy, void* dx, int N, int H, int W,
 int launch_stem_pack(const void* w_krsc, void* w_kn, int cin_pad, cudaStream_t st);
 int launch_stem_forward(const void* in, const void* w_kn, void* out, int N, int H, int W, cudaStream_t st);
 // stem dgrad fused with the masked EOT reduce: G[b] (+)= 2 * sum_s keep_s * dX_s, dX never materialised
+// (bank: the occlusion from a mask bank instead of rects, here and in the launchers below that take one)
 int launch_stem_bwd_reduce(const void* dY, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int B, int S,
-                           int n0, int n, int H, int W, cudaStream_t st);
+                           int n0, int n, int H, int W, cudaStream_t st, const MaskBank* bank = nullptr);
 
 // same, additionally fusing the pad+max-pool backward (reads d_pool + the saved argmax; d_stem never hits HBM)
 int launch_stem_bwd_pool_reduce(const void* dpool, const int8_t* amax, const void* w_krsc, int cin_pad, const int16_t* rects,
-                                float* G, int B, int S, int n0, int n, int H, int W, cudaStream_t st);
+                                float* G, int B, int S, int n0, int n, int H, int W, cudaStream_t st,
+                                const MaskBank* bank = nullptr);
 
 // ---- opt-in: GroupNorm+ReLU applied in the prologue of a wgmma 1x1-convolution GEMM (kernels_gemm.cu, bf16)
 // out[m,n] = sum_k relu(gn(x))[m,k] * W[n,k] (+ shortcut[m,n]); `stats` from launch_gn_stats on x.
@@ -97,12 +105,12 @@ int launch_paste(const float* x, const float* mask, const float* pattern, float*
 // K1: EOT expansion (paste + normalise + occlude) -> [N,H,W,Cp] T.
 // fused==true: reads x/mask/pattern/scale (img ignored); else reads img [B,3,H,W].
 // rects [B*S][4][4] int16 dev or nullptr; samples [n0, n0+n) of the b-major ordering are
-// written to out + (n - n0) * H*W*Cp.
+// written to out + (n - n0) * H*W*Cp.  bank: occlude from a mask bank instead (not fused, W <= 1024; else returns 0).
 void set_expand_tuning(int rows, int sg, int mode);
 void get_expand_last(int* out4);   // tile rows, sample groups, grid, resident CTAs/SM of the last K1 launch   // K1 launch-shape / store-path overrides (0 = heuristic / default); sweeps only
 int launch_expand(const float* img, const float* x, const float* mask, const float* pattern, const float* scale,
                   const int16_t* rects, void* out, int B, int S, int n0, int n, int H, int W, int Cp, bool bf16,
-                  bool fused, int num_sms, cudaStream_t st);
+                  bool fused, int num_sms, cudaStream_t st, const MaskBank* bank = nullptr);
 // optional affine / colour EOT (gather) and its adjoint (atomic scatter into a zeroed G); xf [N][8] dev
 int launch_expand_affine(const float* adv, const float* xf, const int16_t* rects, void* out, int S, int n0, int n,
                          int H, int W, int Cp, bool bf16, cudaStream_t st);
@@ -114,7 +122,7 @@ int launch_cw(const float* logits, const int32_t* y, const uint8_t* targeted, fl
 int launch_argmax(const float* logits, int32_t* preds, int N, int K, cudaStream_t st);
 // K1^T: G[b] (+)= 2 * sum_s keep_s * dz[b,s]  for samples [n0,n0+n).
 int launch_reduce(const void* dz, const int16_t* rects, float* G, int B, int S, int n0, int n, int H, int W,
-                  int Cp, bool bf16, cudaStream_t st);
+                  int Cp, bool bf16, cudaStream_t st, const MaskBank* bank = nullptr);
 // structural loss value [B] + gradient field dLs [B,3,H,W]  (attack.py:33-45,227-228)
 int launch_struct(const float* adv_x, const float* x, float* loss_struc, float* dLs, int B, int H, int W,
                   cudaStream_t st);

@@ -116,6 +116,7 @@ struct ExpandParams {
   const int16_t* rects; void* out;
   int B, S, n0, n, H, W, sgroups, R;
   int mode;   // 0: bulk stores (cp.async.bulk) for untouched tiles / rows + 16-byte stores for occluded rows; 1: 16-byte stores only
+  MaskBank bank;   // the occlusion of the BANK variant (rects unused)
 };
 
 // Shared memory (dynamic): [mbarrier, 512 B][input planes NP*R*W fp32][clean tile R*W*CP T].
@@ -123,7 +124,9 @@ struct ExpandParams {
 // Per EOT sample a warp either bulk-stores the clean tile / clean rows (TMA, cp.async.bulk) when no
 // occluder crosses them, or writes an occluded row itself with 16-byte global stores whose keep /
 // zero / mixed status comes from <= 4 element intervals (no staging copy, no block barrier).
-template <typename T, int CP, bool FUSED>
+// BANK: the occlusion comes from the mask bank p.bank instead: a warp reads a row's bank words (one per lane, <= 32
+// words: W <= 1024) and builds the same per-lane element mask from the row's bits.
+template <typename T, int CP, bool FUSED, bool BANK>
 __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(ExpandParams p) {
   constexpr int NP = FUSED ? 7 : 3;
   constexpr int EPC = 16 / (int)sizeof(T);                 // elements per 16-byte chunk
@@ -172,7 +175,7 @@ __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(ExpandParams p) {
       }
     }
     // rectangle cache of this item's samples (hides the per-sample global-load latency)
-    const bool cached = p.rects != nullptr && (s_hi - s_lo) <= EXP_RCACHE;
+    const bool cached = !BANK && p.rects != nullptr && (s_hi - s_lo) <= EXP_RCACHE;
     if (cached)
       for (int i = threadIdx.x; i < 2 * (s_hi - s_lo); i += EXP_THREADS)
         srect[i] = __ldg(occl::row(p.rects, s_lo) + i);
@@ -203,7 +206,14 @@ __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(ExpandParams p) {
       unsigned char* dst = reinterpret_cast<unsigned char*>(p.out) + ((size_t)(n - p.n0) * HW + (size_t)r0 * W) * CP * sizeof(T);
       int rr0[4], rr1[4], el[4], eh[4];
       bool any = false;
-      if (p.rects != nullptr) {
+      [[maybe_unused]] int2 sel;
+      [[maybe_unused]] const int nw = occl_bank::words(W);
+      if constexpr (BANK) {                                     // any bit set in the tile's rows?
+        sel = occl_bank::select(p.bank, n);
+        uint32_t t = 0u;
+        for (int i = lane; i < EXP_R * nw; i += 32) t |= occl_bank::row_bits(p.bank, sel, r0 + i / nw, i % nw);
+        any = __any_sync(0xffffffffu, t != 0u);
+      } else if (p.rects != nullptr) {
         const Occlusion occ(cached ? occl::load_shared(srect + 2 * (n - s_lo)) : occl::load(p.rects, n));
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -224,7 +234,7 @@ __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(ExpandParams p) {
       for (int cb = 0; cb < row_chunks; cb += 32 * JB) {        // one pass for rows up to 2048 B (bf16) / 4096 B (fp32)
         uint32_t zm[4];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
+        for (int k = 0; k < (BANK ? 0 : 4); ++k) {
           uint32_t z = 0u;
 #pragma unroll
           for (int j = 0; j < JB; ++j) {
@@ -239,11 +249,30 @@ __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(ExpandParams p) {
           const int row = r0 + rr;
           uint32_t Z = 0u;
           bool rany = false;
+          if constexpr (BANK) {
+            // lane k holds word k of the row; field j of Z from the <= 2 words under the pixels of chunk cb + lane + 32 j
+            const uint32_t wv = lane < nw ? occl_bank::row_bits(p.bank, sel, row, lane) : 0u;
+            rany = __any_sync(0xffffffffu, wv != 0u);
+#pragma unroll (CP == 3 ? 1 : JB)                         // (unrolled at C = 3 this loop takes 112 registers)
+            for (int j = 0; j < JB; ++j) {
+              const int e0 = (cb + lane + 32 * j) * EPC, px0 = e0 / CP, k0 = px0 >> 5, off = e0 - px0 * CP;
+              const uint32_t w0 = __shfl_sync(0xffffffffu, wv, k0 & 31), w1 = __shfl_sync(0xffffffffu, wv, (k0 + 1) & 31);
+              const uint32_t bits = __funnelshift_r(w0, k0 + 1 < nw ? w1 : 0u, px0 & 31);   // bit i: pixel px0 + i
+              uint32_t m = 0u;
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const bool cov = row >= rr0[k] && row < rr1[k];
-            rany = rany || cov;
-            Z |= cov ? zm[k] : 0u;
+              for (int k = 0; k < (CP + EPC - 2) / CP + 1; ++k) {   // the pixels a chunk can touch: elements [k CP - off, (k + 1) CP - off)
+                const int lo = max(k * CP - off, 0), hi = min((k + 1) * CP - off, EPC);
+                if (hi > lo && ((bits >> k) & 1u)) m |= ((1u << hi) - 1u) & ~((1u << lo) - 1u);
+              }
+              Z |= m << (EPC * j);
+            }
+          } else {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const bool cov = row >= rr0[k] && row < rr1[k];
+              rany = rany || cov;
+              Z |= cov ? zm[k] : 0u;
+            }
           }
           if (!rany && use_bulk) {                              // clean row: bulk store
             if (cb == 0 && lane == 0) { ptx::bulk_store(dst + (size_t)rr * row_bytes, clean_b + (size_t)rr * row_bytes, row_bytes); ptx::bulk_commit(); }
@@ -298,7 +327,7 @@ static int g_k1_last[4] = {0, 0, 0, 0};                    // tile rows, sample 
 void get_expand_last(int* out4) { for (int i = 0; i < 4; ++i) out4[i] = g_k1_last[i]; }
 void set_expand_tuning(int rows, int sg, int mode) { g_k1_rows = rows < 0 ? 0 : rows; g_k1_sg = sg < 0 ? 0 : sg; g_k1_mode = mode; }
 
-template <typename T, int CP, bool FUSED>
+template <typename T, int CP, bool FUSED, bool BANK>
 static int expand_launch(const ExpandParams& p, int num_sms, cudaStream_t st) {
   if (g_k1_rows == -2) {
     const char* e = getenv("DORPATCH_K1_ROWS"); g_k1_rows = e ? atoi(e) : 0;
@@ -314,9 +343,9 @@ static int expand_launch(const ExpandParams& p, int num_sms, cudaStream_t st) {
   auto resident = [&](int R) {
     if (occ_cache[R] < 0) {
       const size_t sm = smem_of(R);
-      cudaFuncSetAttribute(expand_kernel<T, CP, FUSED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+      cudaFuncSetAttribute(expand_kernel<T, CP, FUSED, BANK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
       int nb = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, expand_kernel<T, CP, FUSED>, EXP_THREADS, sm) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 1; }
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, expand_kernel<T, CP, FUSED, BANK>, EXP_THREADS, sm) != cudaSuccess || nb < 1) { cudaGetLastError(); nb = 1; }
       occ_cache[R] = nb;
     }
     return occ_cache[R];
@@ -338,13 +367,13 @@ static int expand_launch(const ExpandParams& p, int num_sms, cudaStream_t st) {
   const int slots = num_sms * resident(best_R);
   const int best_grid = items_total < slots ? items_total : slots;
   const size_t smem = smem_of(best_R);
-  cudaFuncSetAttribute(expand_kernel<T, CP, FUSED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaFuncSetAttribute(expand_kernel<T, CP, FUSED, BANK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   ExpandParams q = p;
   q.R = best_R;
   q.sgroups = best_sg;
   q.mode = g_k1_mode;
   g_k1_last[0] = best_R; g_k1_last[1] = best_sg; g_k1_last[2] = best_grid; g_k1_last[3] = resident(best_R);
-  expand_kernel<T, CP, FUSED><<<best_grid, EXP_THREADS, smem, st>>>(q);
+  expand_kernel<T, CP, FUSED, BANK><<<best_grid, EXP_THREADS, smem, st>>>(q);
   return 1;
 }
 
@@ -363,11 +392,16 @@ static void dispatch_t_cp(bool bf16, int Cp, F&& f) {
 
 int launch_expand(const float* img, const float* x, const float* mask, const float* pattern, const float* scale,
                   const int16_t* rects, void* out, int B, int S, int n0, int n, int H, int W, int Cp, bool bf16,
-                  bool fused, int num_sms, cudaStream_t st) {
+                  bool fused, int num_sms, cudaStream_t st, const MaskBank* bank) {
   ExpandParams p{img, x, mask, pattern, scale, rects, out, B, S, n0, n, H, W, 1, EXP_R_DEFAULT, 0};
+  if (bank != nullptr) {                                        // the bank variant expands img only
+    if (fused || bank_words(W) > 32) return 0;
+    p.bank = *bank;
+  }
   int k = 0;
   dispatch_t_cp(bf16, Cp, [&](auto t, auto cp) {
-    k = fused ? expand_launch<decltype(t), cp, true>(p, num_sms, st) : expand_launch<decltype(t), cp, false>(p, num_sms, st);
+    if (bank != nullptr) k = expand_launch<decltype(t), cp, false, true>(p, num_sms, st);
+    else k = fused ? expand_launch<decltype(t), cp, true, false>(p, num_sms, st) : expand_launch<decltype(t), cp, false, false>(p, num_sms, st);
   });
   return k;
 }
@@ -528,11 +562,12 @@ int launch_argmax(const float* logits, int32_t* preds, int N, int K, cudaStream_
 // K1^T reduce: G[b,c,h,w] (+)= 2 * sum_{samples n of image b in [n0,n0+n)} keep_n(h,w) * dz[n,h,w,c]
 // grid (ceil(HW/256), images touched)
 // =====================================================================================
+// BANK: keep_n from the mask bank `bank` (rects unused).
 constexpr int RED_MAXS = 128;
-template <typename T, int CP>
+template <typename T, int CP, bool BANK>
 __global__ void __launch_bounds__(256) reduce_kernel(const T* __restrict__ dz, const int16_t* __restrict__ rects,
-                                                     float* __restrict__ G, int S, int n0, int n, int H, int W) {
-  __shared__ __align__(16) short sr[RED_MAXS * RECT_SHORTS];   // the rows of up to RED_MAXS samples
+                                                     float* __restrict__ G, int S, int n0, int n, int H, int W, MaskBank bank) {
+  __shared__ __align__(16) short sr[RED_MAXS * RECT_SHORTS];   // the rows of up to RED_MAXS samples (BANK: their mask indices)
   const int HW = H * W;
   const auto [b, lo, hi, first] = image_span(S, n0, n, blockIdx.y);
   const int px = blockIdx.x * blockDim.x + threadIdx.x;
@@ -541,12 +576,20 @@ __global__ void __launch_bounds__(256) reduce_kernel(const T* __restrict__ dz, c
   for (int base = lo; base < hi; base += RED_MAXS) {
     const int m = min(RED_MAXS, hi - base);
     __syncthreads();
-    for (int i = threadIdx.x; i < m * RECT_SHORTS; i += blockDim.x)
-      sr[i] = rects != nullptr ? rects[(size_t)base * RECT_SHORTS + i] : (short)0;
+    if constexpr (BANK) {
+      for (int i = threadIdx.x; i < m; i += blockDim.x) reinterpret_cast<int2*>(sr)[i] = occl_bank::select(bank, base + i);
+    } else {
+      for (int i = threadIdx.x; i < m * RECT_SHORTS; i += blockDim.x)
+        sr[i] = rects != nullptr ? rects[(size_t)base * RECT_SHORTS + i] : (short)0;
+    }
     __syncthreads();
     if (px < HW) {
       for (int j = 0; j < m; ++j) {
-        if (occl::hit(sr + j * RECT_SHORTS, row, col)) continue;
+        if constexpr (BANK) {
+          if (occl_bank::hit(bank, reinterpret_cast<const int2*>(sr)[j], row, col)) continue;
+        } else {
+          if (occl::hit(sr + j * RECT_SHORTS, row, col)) continue;
+        }
         const T* q = dz + ((size_t)(base + j - n0) * HW + px) * CP;
         if (CP * sizeof(T) == 16) {
           Vec<T> v; v.load(q);
@@ -568,11 +611,12 @@ __global__ void __launch_bounds__(256) reduce_kernel(const T* __restrict__ dz, c
   }
 }
 int launch_reduce(const void* dz, const int16_t* rects, float* G, int B, int S, int n0, int n, int H, int W,
-                  int Cp, bool bf16, cudaStream_t st) {
+                  int Cp, bool bf16, cudaStream_t st, const MaskBank* bank) {
   const dim3 grid((H * W + 255) / 256, images_touched(S, n0, n));
   dispatch_t_cp(bf16, Cp, [&](auto t, auto cp) {
     using T = decltype(t);
-    reduce_kernel<T, cp><<<grid, 256, 0, st>>>((const T*)dz, rects, G, S, n0, n, H, W);
+    if (bank != nullptr) reduce_kernel<T, cp, true><<<grid, 256, 0, st>>>((const T*)dz, nullptr, G, S, n0, n, H, W, *bank);
+    else reduce_kernel<T, cp, false><<<grid, 256, 0, st>>>((const T*)dz, rects, G, S, n0, n, H, W, MaskBank{});
   });
   return 1;
 }

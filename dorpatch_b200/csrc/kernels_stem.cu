@@ -267,12 +267,12 @@ struct PoolPatch {   // stage: [PR][PC][PIX] patch, then [2][RR*RC][128 + 64] re
 
 // `in` (a stemb::DyPatch or stemb::PoolPatch) gives each sample's dY [.., H/2, W/2, 64] patch; w_krsc: [64][7][7][cin_pad]
 // bf16.  One CTA = one 8x16 tile of positions (i,j) of one image = a 16x32 block of input pixels; all four parity
-// classes share the dY patch (one per sample).
-template <class Src>
+// classes share the dY patch (one per sample).  BANK: keep_n from the mask bank `bank` (rects unused).
+template <class Src, bool BANK>
 __global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_reduce_kernel(Src in, const __nv_bfloat16* __restrict__ w_krsc,
                                                                              int cin_pad, const int16_t* __restrict__ rects,
                                                                              float* __restrict__ G, int S, int n0, int n,
-                                                                             int H, int W) {
+                                                                             int H, int W, MaskBank bank) {
   using namespace stemb;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned char* Ws = smem_raw;                                   // [49 taps, class-major][k][8] bf16, 16 B per (tap, k)
@@ -313,7 +313,9 @@ __global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_reduce_kernel(Src 
     __syncthreads();
     const unsigned char* pb = in.patch(stage, tile, buf);
     Occlusion occ;
-    if (rects != nullptr) occ.set(occl::load(rects, s));
+    [[maybe_unused]] int2 sel;
+    if constexpr (BANK) sel = occl_bank::select(bank, s);
+    else if (rects != nullptr) occ.set(occl::load(rects, s));
     // The 49 taps use only 16 distinct patch shifts (di, dj) in {-1..2}^2: load each A fragment once and feed
     // every parity class that has a tap at this shift (shared-memory bandwidth is the limit: N is only 8).
     float acc[4][4];
@@ -345,8 +347,14 @@ __global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_reduce_kernel(Src 
     for (int cls = 0; cls < 4; ++cls) {
       const int py = cls >> 1, px = cls & 1;
       const int y = 2 * irow + py, xA = 2 * (j0 + g) + px, xB = 2 * (j0 + g + 8) + px;
-      const bool keepA = rects == nullptr || !occ.hit(y, xA);
-      const bool keepB = rects == nullptr || !occ.hit(y, xB);
+      bool keepA, keepB;
+      if constexpr (BANK) {
+        keepA = y >= H || xA >= W || !occl_bank::hit(bank, sel, y, xA);   // (a position past the image is never stored)
+        keepB = y >= H || xB >= W || !occl_bank::hit(bank, sel, y, xB);
+      } else {
+        keepA = rects == nullptr || !occ.hit(y, xA);
+        keepB = rects == nullptr || !occ.hit(y, xB);
+      }
       if (keepA) { tot[cls][0] += acc[cls][0]; tot[cls][1] += acc[cls][1]; }
       if (keepB) { tot[cls][2] += acc[cls][2]; tot[cls][3] += acc[cls][3]; }
     }
@@ -375,24 +383,30 @@ __global__ void __launch_bounds__(stemb::THREADS, 2) stem_bwd_reduce_kernel(Src 
   }
 }
 
-template <class Src>
-static int launch_stem_bwd(Src in, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int S, int n0, int n,
-                           int H, int W, cudaStream_t st) {
-  cudaFuncSetAttribute(stem_bwd_reduce_kernel<Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Src::SMEM);
+template <class Src, bool BANK>
+static int launch_stem_bwd_as(Src in, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int S, int n0, int n,
+                              int H, int W, const MaskBank& bank, cudaStream_t st) {
+  cudaFuncSetAttribute(stem_bwd_reduce_kernel<Src, BANK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Src::SMEM);
   const int tiles = ((H / 2 + stemb::TI - 1) / stemb::TI) * ((W / 2 + stemb::TJ - 1) / stemb::TJ);
-  stem_bwd_reduce_kernel<Src><<<dim3(tiles, images_touched(S, n0, n)), stemb::THREADS, Src::SMEM, st>>>(
-      in, (const __nv_bfloat16*)w_krsc, cin_pad, rects, G, S, n0, n, H, W);
+  stem_bwd_reduce_kernel<Src, BANK><<<dim3(tiles, images_touched(S, n0, n)), stemb::THREADS, Src::SMEM, st>>>(
+      in, (const __nv_bfloat16*)w_krsc, cin_pad, rects, G, S, n0, n, H, W, bank);
   return 1;
 }
+template <class Src>
+static int launch_stem_bwd(Src in, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int S, int n0, int n,
+                           int H, int W, const MaskBank* bank, cudaStream_t st) {
+  if (bank != nullptr) return launch_stem_bwd_as<Src, true>(in, w_krsc, cin_pad, nullptr, G, S, n0, n, H, W, *bank, st);
+  return launch_stem_bwd_as<Src, false>(in, w_krsc, cin_pad, rects, G, S, n0, n, H, W, MaskBank{}, st);
+}
 int launch_stem_bwd_reduce(const void* dY, const void* w_krsc, int cin_pad, const int16_t* rects, float* G, int B, int S,
-                           int n0, int n, int H, int W, cudaStream_t st) {
+                           int n0, int n, int H, int W, cudaStream_t st, const MaskBank* bank) {
   (void)B;
-  return launch_stem_bwd(stemb::DyPatch{(const __nv_bfloat16*)dY}, w_krsc, cin_pad, rects, G, S, n0, n, H, W, st);
+  return launch_stem_bwd(stemb::DyPatch{(const __nv_bfloat16*)dY}, w_krsc, cin_pad, rects, G, S, n0, n, H, W, bank, st);
 }
 int launch_stem_bwd_pool_reduce(const void* dpool, const int8_t* amax, const void* w_krsc, int cin_pad, const int16_t* rects,
-                                float* G, int B, int S, int n0, int n, int H, int W, cudaStream_t st) {
+                                float* G, int B, int S, int n0, int n, int H, int W, cudaStream_t st, const MaskBank* bank) {
   (void)B;
-  return launch_stem_bwd(stemb::PoolPatch{(const __nv_bfloat16*)dpool, amax}, w_krsc, cin_pad, rects, G, S, n0, n, H, W, st);
+  return launch_stem_bwd(stemb::PoolPatch{(const __nv_bfloat16*)dpool, amax}, w_krsc, cin_pad, rects, G, S, n0, n, H, W, bank, st);
 }
 
 }  // namespace dp

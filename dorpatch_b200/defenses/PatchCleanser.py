@@ -9,6 +9,9 @@ the bool mask tensors of the reference are materialised lazily, only if someone 
 ``MaskWindow(img, r, n_patch=2)`` is the two-patch window (reference :31-37): 630 first-round pairs and
 22 680 certificate masks of 3 rectangles each.  Its second round puts 4 rectangles on a sample, which is
 K1's per-sample limit, so the same code and kernels serve both windows.
+
+A window without rectangle tables (any object with bool ``mask_set`` / ``double_mask_set``, as the reference accepts)
+is packed into mask banks (``masks.pack_bank``) and runs the same rounds through ``dp_predict_bank``.
 """
 import math
 
@@ -68,8 +71,31 @@ class PatchCleanser(object):
         x = img.reshape(1, 3, img.shape[-2], img.shape[-1]).contiguous().float()
         return eng.predict(x, rects.shape[0], rects)
 
+    def _predict_bank(self, img, bank, idx):
+        """The same on a mask bank: sample k occluded by mask idx[k] (or the pair idx[k, 0], idx[k, 1])."""
+        eng = self._engine(img)
+        x = img.reshape(1, 3, img.shape[-2], img.shape[-1]).contiguous().float()
+        return eng.predict(x, len(idx), bank=bank, idx=idx)
+
+    def _bank(self, name, img):
+        """A window without rectangle tables (any object with bool mask_set / double_mask_set, as the reference
+        accepts): its set `name` packed into a mask bank on img's device, when first needed (the doubles only when a
+        certificate is asked for, as the reference reads them only then), and kept while the window, the set object
+        and the device stay the same."""
+        mw = self.mask_window
+        masks = getattr(mw, name)
+        cache = self.__dict__.setdefault("_bank_cache", {})
+        key = (name, str(img.device))
+        hit = cache.get(key)
+        if hit is None or hit[0] is not mw or hit[1] is not masks:
+            hit = (mw, masks, _masks.pack_bank(masks, device=img.device))
+            cache[key] = hit
+        return hit[2]
+
     def robust_predict(self, img, certify=False):
         mw = self.mask_window
+        if getattr(mw, "mask_rects", None) is None:
+            return self._robust_predict_bank(img, certify)
         single = _masks.gather(mw.mask_rects, np.arange(len(mw.mask_rects)))          # [36 or 630,4,4]
         preds_1 = self._predict(img, single)                                          # :70-72
         labels, counts = torch.from_numpy(preds_1.astype(np.int64)).unique(sorted=False, return_counts=True)
@@ -94,6 +120,31 @@ class PatchCleanser(object):
         return PatchCleanserRecord(pred, certifiable, preds_1.astype(np.int64),
                                    None if preds_2 is None else np.asarray(preds_2))
 
+    def _robust_predict_bank(self, img, certify):
+        """robust_predict for a window given as bool mask sets: the same rounds, tie rules and records, each
+        occlusion read from a mask bank; the second round occludes with the pair (mask j, mask k)."""
+        singles = self._bank("mask_set", img)
+        n = singles.shape[0]
+        preds_1 = self._predict_bank(img, singles, np.arange(n))                      # :70-72
+        labels, counts = torch.from_numpy(preds_1.astype(np.int64)).unique(sorted=False, return_counts=True)
+        label_majority = labels[counts.argmax()].item()                               # :74-75
+        pred, preds_2 = label_majority, None
+        if len(labels) == 1:                                                          # :78-79
+            certifiable, preds_2 = self.robustness_certificate(img, pred)
+        else:                                                                         # :80-90
+            certifiable = False
+            for label in labels.tolist():
+                if label == label_majority:
+                    continue
+                for k in np.nonzero(preds_1 == label)[0]:
+                    pairs = np.stack([np.arange(n), np.full(n, k)], axis=1)
+                    if (self._predict_bank(img, singles, pairs) == label).all():
+                        pred = label
+        if certify and preds_2 is None:                                               # :93-94
+            preds_2 = self.robustness_certificate(img, label_majority)[1]
+        return PatchCleanserRecord(pred, certifiable, preds_1.astype(np.int64),
+                                   None if preds_2 is None else np.asarray(preds_2))
+
     def mask(self, img, msk):
         return img * msk + 0.5 * ~msk
 
@@ -101,7 +152,11 @@ class PatchCleanser(object):
         """All double-mask predictions (630, or 22 680 for n_patch 2) must equal `label` (:102-112).  `batch_size` is kept
         for signature compatibility; batching is the engine's `chunk`."""
         mw = self.mask_window
-        preds = self._predict(img, _masks.gather(mw.double_mask_rects, np.arange(len(mw.double_mask_rects))))
+        if getattr(mw, "double_mask_rects", None) is None:
+            doubles = self._bank("double_mask_set", img)
+            preds = self._predict_bank(img, doubles, np.arange(doubles.shape[0]))
+        else:
+            preds = self._predict(img, _masks.gather(mw.double_mask_rects, np.arange(len(mw.double_mask_rects))))
         consistent = preds == label
         return bool(consistent.all()), consistent
 

@@ -47,6 +47,33 @@ def _host_rects(rects, N):
     return _host(np.asarray(rects).reshape(N, 4, 4), np.int16)
 
 
+def _bank_args(bank, idx, N, img, device):
+    """The mask-bank occlusion of N samples: (bank pointer, number of masks, index array [N][2] int32, its pointer).
+    bank: masks.pack_bank's int32 CUDA tensor [M, img, ceil(img/32)]; idx: [..] or [.., 2] mask indices (-1 = none)."""
+    if not (isinstance(bank, torch.Tensor) and bank.is_cuda and bank.dtype == torch.int32 and bank.is_contiguous()):
+        raise TypeError("bank must be a contiguous int32 CUDA tensor (masks.pack_bank)")
+    if bank.device.index != device:
+        raise ValueError("bank is on cuda:%d, the engine on cuda:%d" % (bank.device.index, device))
+    if bank.dim() != 3 or bank.shape[0] < 1 or bank.shape[1] != img or bank.shape[2] != (img + 31) // 32:
+        raise ValueError("bank must be [M >= 1, %d, %d], got %s" % (img, (img + 31) // 32, tuple(bank.shape)))
+    if idx is None:
+        raise ValueError("a bank needs idx, the mask indices of every sample")
+    if isinstance(idx, torch.Tensor):
+        idx = idx.detach().cpu().numpy()
+    idx = np.asarray(idx)
+    if idx.dtype.kind not in "iu":
+        raise TypeError("idx must be an integer array, got %s" % idx.dtype)
+    if idx.size == N:
+        idx = np.stack([idx.reshape(N), np.full(N, -1)], axis=1)
+    elif idx.size != 2 * N or idx.shape[-1] != 2:
+        raise ValueError("idx must hold one or two mask indices per sample (%d samples), got shape %s" % (N, idx.shape))
+    M = int(bank.shape[0])
+    if idx.size and (idx.min() < -1 or idx.max() >= M):
+        raise ValueError("idx holds mask indices outside [-1, %d)" % M)
+    a, p = _host(idx.reshape(N, 2), np.int32)
+    return C.c_void_p(bank.data_ptr()), M, a, p
+
+
 class Engine:
     """ResNetV2-50x1-BiT attack engine on one CUDA device."""
 
@@ -183,27 +210,55 @@ class Engine:
                                       self._stream()))
         return out
 
-    def predict(self, img, S=1, rects=None, return_logits=False):
-        """argmax of model(occlude(img)) for S occlusions per image; img [B,3,H,W] in [0,1]."""
+    def expand_bank(self, img, S, bank, idx):
+        """K1 occluding from a mask bank (tests / profiling): expand()'s output for the bank's occlusions."""
         B = img.shape[0]
         N = B * S
+        bp, M, ia, ip = _bank_args(bank, idx, N, self.img, self.device)
+        dt = torch.bfloat16 if self.elem_bytes == 2 else torch.float32
+        out = torch.empty((N, self.img, self.img, self.c_pad), dtype=dt, device=img.device)
+        _lib.check(self.lib.dp_expand_bank(self.handle, _dev_ptr(img), B, S, bp, M, ip, C.c_void_p(out.data_ptr()),
+                                           self._stream()))
+        return out
+
+    def predict(self, img, S=1, rects=None, return_logits=False, bank=None, idx=None):
+        """argmax of model(occlude(img)) for S occlusions per image; img [B,3,H,W] in [0,1].  The occlusions are
+        rects (rectangle tables) or a mask bank: bank (masks.pack_bank) with idx [B*S] or [B*S, 2] mask indices."""
+        B = img.shape[0]
+        N = B * S
+        if bank is not None and rects is not None:
+            raise ValueError("predict: give rects or a bank, not both")
         preds = np.empty(N, np.int32)
         logits = np.empty((N, self.n_classes), np.float32) if return_logits else None
-        rects, rp = _host_rects(rects, N)
-        _lib.check(self.lib.dp_predict(self.handle, _dev_ptr(img), B, S, rp, C.c_void_p(preds.ctypes.data),
-                                       C.c_void_p(logits.ctypes.data) if return_logits else None, self._stream()))
+        lp = C.c_void_p(logits.ctypes.data) if return_logits else None
+        if bank is not None:
+            bp, M, ia, ip = _bank_args(bank, idx, N, self.img, self.device)
+            _lib.check(self.lib.dp_predict_bank(self.handle, _dev_ptr(img), B, S, bp, M, ip,
+                                                C.c_void_p(preds.ctypes.data), lp, self._stream()))
+        else:
+            rects, rp = _host_rects(rects, N)
+            _lib.check(self.lib.dp_predict(self.handle, _dev_ptr(img), B, S, rp, C.c_void_p(preds.ctypes.data), lp,
+                                           self._stream()))
         return (preds, logits) if return_logits else preds
 
     # ------------------------------------------------------------------------------
-    def eot_forward(self, img, S=1, rects=None, xforms=None):
+    def eot_forward(self, img, S=1, rects=None, xforms=None, bank=None, idx=None):
         """model(occlude(img)) as [B*S, K] logits on the device (dp_predict's values), keeping what eot_backward needs.
         img [B,3,H,W] fp32 in [0,1]; rects [B,S,4,4] int16 or None (then S must be 1 unless xforms are given).
-        xforms: [B,S,8] affine / colour transforms (eot.sample's layout) applied before the occlusion, or None."""
+        xforms: [B,S,8] affine / colour transforms (eot.sample's layout) applied before the occlusion, or None.
+        bank / idx: occlude from a mask bank (masks.pack_bank) instead of rects, idx [B,S] or [B,S,2] mask indices;
+        not with rects or xforms.  The backward reads the bank again: it must stay unchanged until then."""
         B = img.shape[0]
         N = B * int(S)
+        if bank is not None and (rects is not None or xforms is not None):
+            raise ValueError("eot_forward: a bank cannot be combined with %s" % ("rects" if rects is not None else "xforms"))
         logits = torch.empty((N, self.n_classes), dtype=torch.float32, device=img.device)
         rects, rp = _host_rects(rects, N)
-        if xforms is None:
+        if bank is not None:
+            bp, M, ia, ip = _bank_args(bank, idx, N, self.img, self.device)
+            _lib.check(self.lib.dp_eot_forward_bank(self.handle, _dev_ptr(img), B, int(S), bp, M, ip, _dev_ptr(logits),
+                                                    self._stream()))
+        elif xforms is None:
             _lib.check(self.lib.dp_eot_forward(self.handle, _dev_ptr(img), B, int(S), rp, _dev_ptr(logits),
                                                self._stream()))
         else:
@@ -218,9 +273,14 @@ class Engine:
         # alive (a caller's temporary would otherwise be freed and its memory handed to the next allocation, such as
         # the gradient itself) and remember its version to refuse a backward after an in-place change.
         self._eot_img, self._eot_img_version = img, _version(img)
+        self._eot_bank, self._eot_bank_version = bank, (_version(bank) if bank is not None else None)
         return logits
 
     def _check_eot_img(self, fn, out):
+        bank = getattr(self, "_eot_bank", None)
+        if bank is not None and _version(bank) != self._eot_bank_version:
+            raise RuntimeError("%s: the mask bank of the last eot_forward was modified in place since; run the forward "
+                               "again" % fn)
         img = getattr(self, "_eot_img", None)
         if img is None:
             return

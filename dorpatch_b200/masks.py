@@ -183,3 +183,49 @@ def _decompose(occ, k=0):
                         out[1] = (rb[c0], rb[c1], cb[d0], cb[d1])
                         return out
     raise NotImplementedError("mask %d is not a union of <= 2 axis-aligned rectangles" % k)
+
+
+# ---- mask banks: arbitrary occlusions -------------------------------------------------------------------------------
+def bank_words(W):
+    """uint32 words per row of a mask bank of width W."""
+    return (int(W) + 31) // 32
+
+
+def pack_bank(keep, device=None):
+    """Bool keep-masks [M,1,H,W] or [M,H,W] (torch or numpy; True = keep, as the reference's mask sets) -> the mask
+    bank the engine reads: a contiguous int32 CUDA tensor [M, H, ceil(W/32)] holding uint32 words, bit w % 32 of word
+    w / 32 of row h set = pixel (h, w) occluded.  Any shape of occluder works (``Engine.predict(bank=...)``,
+    ``eot_logits(bank=...)``).  device: the CUDA device (default: the masks' own if they are on one, else the current)."""
+    import torch
+    m = keep if isinstance(keep, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(keep))
+    if m.dim() == 4:
+        if m.shape[1] != 1:
+            raise ValueError("pack_bank: masks must be [M,1,H,W] or [M,H,W], got %s" % (tuple(m.shape),))
+        m = m[:, 0]
+    if m.dim() != 3 or m.shape[0] < 1:
+        raise ValueError("pack_bank: masks must be [M,1,H,W] or [M,H,W] with M >= 1, got %s" % (tuple(keep.shape),))
+    if m.dtype != torch.bool:
+        raise TypeError("pack_bank: masks must be bool (True = keep), got %s" % (m.dtype,))
+    if device is None:
+        device = m.device if m.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    M, H, W = m.shape
+    nw = bank_words(W)
+    out = torch.empty((M, H, nw), dtype=torch.int32, device=device)
+    shift = torch.arange(32, device=device, dtype=torch.int64)
+    for m0 in range(0, M, 512):                                  # bounded scratch for large universes
+        part = m[m0:m0 + 512]
+        occ = torch.zeros((part.shape[0], H, nw * 32), dtype=torch.int64, device=device)
+        occ[:, :, :W] = (~part).to(device=device, dtype=torch.int64)
+        w = (occ.view(-1, H, nw, 32) << shift).sum(-1)
+        out[m0:m0 + 512] = torch.where(w >= 2 ** 31, w - 2 ** 32, w).to(torch.int32)
+    return out
+
+
+def unpack_bank(bank, W):
+    """Inverse of pack_bank: bank [M,H,ceil(W/32)] (torch int32) -> bool keep-masks [M,1,H,W] on the bank's device."""
+    import torch
+    M, H, nw = bank.shape
+    if nw != bank_words(W):
+        raise ValueError("unpack_bank: %d words per row do not hold W=%d" % (nw, W))
+    bits = (bank.to(torch.int64)[..., None] >> torch.arange(32, device=bank.device, dtype=torch.int64)) & 1
+    return (bits.reshape(M, H, nw * 32)[:, :, :W] == 0)[:, None]

@@ -28,10 +28,12 @@ from .utils import unwrap_native
 
 class _EotLogits(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, img, eng, S, rects, xforms, names, *params):
-        logits = eng.eot_forward(img, S, rects, xforms)
+    def forward(ctx, img, eng, S, rects, xforms, bank, idx, names, *params):
+        logits = eng.eot_forward(img, S, rects, xforms, bank=bank, idx=idx)
         ctx.eng, ctx.token, ctx.names = eng, eng.eot_forwards, names
-        ctx.save_for_backward(img, *params)           # autograd then refuses a backward after an in-place change
+        ctx.banked = bank is not None
+        # autograd then refuses a backward after an in-place change of the image or the bank
+        ctx.save_for_backward(img, *((bank,) if ctx.banked else ()), *params)
         return logits
 
     @staticmethod
@@ -40,21 +42,22 @@ class _EotLogits(torch.autograd.Function):
             raise RuntimeError("eot_logits: double backward (create_graph=True) is not supported; the engine computes "
                                "first-order input gradients only")
         saved = ctx.saved_tensors
-        params = saved[1:]
+        params = saved[2:] if ctx.banked else saved[1:]
+        none = (None,) * 7                              # eng, S, rects, xforms, bank, idx, names
         eng = ctx.eng
         if eng.eot_forwards != ctx.token:
             raise RuntimeError("eot_logits: the engine ran another eot_forward after this one; its activations are "
                                "gone, so this graph can no longer be differentiated (run the forward again)")
         d = dlogits.contiguous().float()
         if ctx.names is None:
-            return eng.eot_backward(d), None, None, None, None, None
-        live = [i for i in range(len(params)) if ctx.needs_input_grad[6 + i]]
+            return (eng.eot_backward(d),) + none
+        live = [i for i in range(len(params)) if ctx.needs_input_grad[8 + i]]
         grads = [torch.empty(params[i].shape, dtype=torch.float32, device=d.device) for i in live]
         g_img = eng.eot_backward_params(d, [ctx.names[i] for i in live], grads, grad_img=ctx.needs_input_grad[0])
         out = [None] * len(params)
         for i, g in zip(live, grads):
             out[i] = g if g.device == params[i].device else g.to(params[i].device)
-        return (g_img, None, None, None, None, None) + tuple(out)
+        return (g_img,) + none + tuple(out)
 
 
 def _check_xforms(xforms, img, S):
@@ -72,7 +75,29 @@ def _check_xforms(xforms, img, S):
     return np.ascontiguousarray(xforms, dtype=np.float32)
 
 
-def eot_logits(model, img, rects=None, S=1, xforms=None, param_grads=False):
+def _check_bank(bank, idx, img, S):
+    """idx of a mask bank as a [B*S, 2] int32 host array, or TypeError / ValueError."""
+    if not (isinstance(bank, torch.Tensor) and bank.dtype == torch.int32 and bank.dim() == 3):
+        raise TypeError("eot_logits: bank must be the int32 tensor [M, H, ceil(W/32)] of masks.pack_bank")
+    if idx is None:
+        raise ValueError("eot_logits: a bank needs idx, [B, S] or [B, S, 2] mask indices")
+    if isinstance(idx, torch.Tensor):
+        idx = idx.detach().cpu().numpy()
+    idx = np.asarray(idx)
+    if idx.dtype.kind not in "iu":
+        raise TypeError("eot_logits: idx must be an integer array, got %s" % idx.dtype)
+    B = img.shape[0] if isinstance(img, torch.Tensor) and img.dim() >= 1 else None
+    if idx.ndim == 2:
+        idx = np.stack([idx, np.full(idx.shape, -1, idx.dtype)], axis=-1)
+    if idx.ndim != 3 or idx.shape[1:] != (S, 2) or (B is not None and idx.shape[0] != B):
+        raise ValueError("eot_logits: idx must be [B, S] or [B, S, 2] with B = %s, S = %d, got %s" % (B, S, idx.shape))
+    M = int(bank.shape[0])
+    if idx.size and (idx.min() < -1 or idx.max() >= M):
+        raise ValueError("eot_logits: idx holds mask indices outside [-1, %d)" % M)
+    return np.ascontiguousarray(idx, dtype=np.int32)
+
+
+def eot_logits(model, img, rects=None, S=1, xforms=None, param_grads=False, bank=None, idx=None):
     """Differentiable ``model(occlude(img))``: [B*S, K] logits, sample b*S+s occluding image b with rects[b, s].
 
     model: ``ResNetV2``, ``NormModel(ResNetV2)`` or ``DataParallel`` of either (the native engine; anything else
@@ -86,8 +111,20 @@ def eot_logits(model, img, rects=None, S=1, xforms=None, param_grads=False):
     Differentiable with respect to ``img``; the transform parameters get no gradient (see the module docstring).
     With xforms the input gradient is summed with fp32 atomics, so its last bits can differ from run to run.
     param_grads: also differentiate the classifier's fp32 parameters that require grad (frozen ones get None and
-    cost nothing); the logits are then differentiable even when img does not require grad."""
+    cost nothing); the logits are then differentiable even when img does not require grad.
+    bank / idx: occlude with arbitrary masks instead of rectangles: bank = ``masks.pack_bank(keep)`` (bool keep-masks
+    [M, 1, H, W], True = keep), idx [B, S] or [B, S, 2] int mask indices (sample b*S+s is occluded where mask
+    idx[b, s, 0] or idx[b, s, 1] is, -1 = none).  Not with rects or xforms.  The bank is saved for the backward like
+    img: changing it in place before the backward raises."""
     net = unwrap_native(model)
+    if bank is not None:
+        if rects is not None:
+            raise ValueError("eot_logits: give rects or a bank, not both")
+        if xforms is not None:
+            raise ValueError("eot_logits: a bank cannot be combined with xforms (the warped path reads rectangles)")
+        idx = _check_bank(bank, idx, img, int(S))
+    elif idx is not None:
+        raise ValueError("eot_logits: idx without a bank")
     if not isinstance(param_grads, bool):
         raise TypeError("eot_logits: param_grads must be True or False, got %r" % (param_grads,))
     names, params = None, ()
@@ -102,10 +139,10 @@ def eot_logits(model, img, rects=None, S=1, xforms=None, param_grads=False):
     if not (isinstance(img, torch.Tensor) and img.is_cuda):
         raise RuntimeError("eot_logits runs on the native CUDA engine only (no CPU fallback)")
     S = int(S)
-    if rects is None and S != 1 and xforms is None:
+    if rects is None and S != 1 and xforms is None and bank is None:
         raise ValueError("eot_logits: S=%d needs rectangle tables or xforms (rects=None without xforms is plain "
                          "classification, S=1)" % S)
     if img.dim() != 4 or img.shape[1] != 3:
         raise ValueError("eot_logits: img must be [B, 3, H, W], got %s" % (tuple(img.shape),))
     eng = net.engine(img.shape[-1], max_images=img.shape[0])
-    return _EotLogits.apply(img.contiguous().float(), eng, S, rects, xforms, names, *params)
+    return _EotLogits.apply(img.contiguous().float(), eng, S, rects, xforms, bank, idx, names, *params)

@@ -121,6 +121,15 @@ int32_t dp_expand(dp_engine* e, const float* img, int32_t B, int32_t S, const in
  * synchronisation -- exactly one kernel launch on `stream` (what bench.py brackets with CUDA events). */
 int32_t dp_expand_dev(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_dev,
                       void* out, void* stream);
+/* Mask banks: the second occlusion format, for occluders that are not rectangles.  bank_dev: uint32
+ * [n_bank][H][ceil(H/32)] dev, owned by the caller; bit w % 32 of word w / 32 of row h of mask m set = pixel (h, w) of
+ * mask m occluded (0 = keep: an all-zero mask occludes nothing).  idx_host: int32 [B*S][2] host; sample n is occluded
+ * where mask idx[n][0] or mask idx[n][1] is set, -1 = no mask.  Refused: n_bank < 1, an index outside [-1, n_bank),
+ * a non-negative index with bank_dev NULL, img > 1024.  The engine copies the indices, never the bank.
+ * dp_expand_bank: dp_expand occluding from a bank; the output is dp_expand's, bit for bit, whenever the bank
+ * encodes the same pixels as the rectangle table.  Added without changing any other entry point: the ABI stays 9. */
+int32_t dp_expand_bank(dp_engine* e, const float* img, int32_t B, int32_t S, const uint32_t* bank_dev, int32_t n_bank,
+                       const int32_t* idx_host, void* out, void* stream);
 /* The variant of K1 the hot loop launches (attack.py:184-185 fused in: reads x / mask / pattern [B,...] dev and the
  * clip scale of the last dp_paste / dp_attack_grad on these tensors), for samples [n0, n0+n) of the b-major
  * [B*S] ordering -- one classifier chunk.  Rectangles on the device; exactly one kernel launch, no synchronisation
@@ -136,6 +145,10 @@ int32_t dp_input_layout(const dp_engine* e, int32_t* c_pad, int32_t* elem_bytes)
 /* preds_host[B*S] = argmax logits; logits_host[B*S*n_classes] optional (NULL to skip). */
 int32_t dp_predict(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host,
                    int32_t* preds_host, float* logits_host, void* stream);
+/* dp_predict occluding from a mask bank (see dp_expand_bank): same chunks, same lanes; the logits are dp_predict's,
+ * bit for bit, whenever the bank encodes the same pixels as the rectangle table.  The ABI stays 9. */
+int32_t dp_predict_bank(dp_engine* e, const float* img, int32_t B, int32_t S, const uint32_t* bank_dev, int32_t n_bank,
+                        const int32_t* idx_host, int32_t* preds_host, float* logits_host, void* stream);
 
 /* ---- differentiable classifier: forward and backward-to-input as two calls ---------------- */
 /* logits_dev[B*S, K] = model(occlude(img_b, rects[b*S+s])), img [B,3,H,W] fp32 dev in [0,1] (NormModel's 0.5/0.5
@@ -156,6 +169,14 @@ int32_t dp_eot_backward(dp_engine* e, const float* dlogits_dev, float* grad_img_
  * bits of the gradient may vary from run to run.  Added without changing any other entry point: the ABI stays 9. */
 int32_t dp_eot_forward_xform(dp_engine* e, const float* img, int32_t B, int32_t S, const int16_t* rects_host,
                              const float* xform_host, float* logits_dev, void* stream);
+/* dp_eot_forward occluding from a mask bank (see dp_expand_bank): logits_dev[B*S, K] = model(occlude(img_b, bank,
+ * idx[b*S+s])).  dp_eot_backward and dp_eot_backward_params then differentiate this forward; they read the bank again
+ * for the chunks whose activations the engine no longer holds, so bank_dev must stay allocated and unchanged until
+ * then (the indices are copied).  The logits and the input gradient are those of dp_eot_forward, bit for bit, whenever
+ * the bank encodes the same pixels as the rectangle table.  Added without changing any other entry point: the ABI
+ * stays 9. */
+int32_t dp_eot_forward_bank(dp_engine* e, const float* img, int32_t B, int32_t S, const uint32_t* bank_dev, int32_t n_bank,
+                            const int32_t* idx_host, float* logits_dev, void* stream);
 /* dp_eot_backward plus the gradients of the classifier's parameters (fine-tuning).  For each of the n timm names
  * (dp_engine_load_weights's names) grad_dev_ptrs[i] (fp32 dev, OIHW / vector, the tensor's shape) receives
  * d<dlogits, logits>/d tensor of the last dp_eot_forward[_xform]: written (accumulate = 0) or added (accumulate = 1).
@@ -264,6 +285,9 @@ int32_t dp_failed_set_read(dp_engine* e, int32_t b, int32_t* idx_host_out, int32
  *   kernel in front of the wgmma GEMM and the classifier head). */
 int32_t dp_debug_stem_bwd_reduce(dp_engine* e, const void* dY, const int16_t* rects_host, int32_t B, int32_t S, float* G,
                                  void* stream);
+/* dp_debug_stem_bwd_reduce occluding from a mask bank (bank_dev / n_bank / idx_host as for dp_expand_bank). */
+int32_t dp_debug_stem_bwd_reduce_bank(dp_engine* e, const void* dY, const uint32_t* bank_dev, int32_t n_bank,
+                                      const int32_t* idx_host, int32_t B, int32_t S, float* G, void* stream);
 /* The bf16 engine's stem on caller-supplied tensors (tests/test_gpu_stem_ops.py), through the launches the engine runs.
  * G is written by the kernels alone: every element of every image, nothing is zeroed first.
  * dp_debug_stem_bwd_pool_reduce: dp_debug_stem_bwd_reduce with the max-pool backward fused in (DORPATCH_POOL_BWD=fused):
