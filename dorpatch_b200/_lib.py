@@ -85,6 +85,8 @@ SIGNATURES = {
     "dp_predict_bank": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     "dp_eot_forward_bank": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp]),
     "dp_debug_stem_bwd_reduce_bank": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
+    "dp_debug_cw": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_f32, c_f32, c_vp, c_vp, c_vp, c_i32, c_i32, c_vp]),
+    "dp_debug_reduce": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp]),
 }
 
 _lib = None

@@ -2011,6 +2011,45 @@ int32_t dp_debug_stem_bwd_reduce_bank(dp_engine* e, const void* dY, const uint32
   });
 }
 
+int32_t dp_debug_cw(dp_engine* e, const float* logits, const int32_t* y, const uint8_t* targeted, float confidence, float inv_s,
+                    float* loss, int32_t* preds, float* dlogits, int32_t N, int32_t K, void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!logits || N < 1 || K < 1) fail("dp_debug_cw: bad arguments");
+    if (!y) {
+      if (!preds) fail("dp_debug_cw: the argmax needs preds");
+      e->run(st, [&] { return dp::launch_argmax(logits, preds, N, K, st); });
+      return;
+    }
+    if (!targeted || !loss) fail("dp_debug_cw: the CW loss needs targeted and loss");
+    std::vector<int32_t> ys(N);                          // the kernel reads logits[n][y[n]]: check the labels first
+    CUDA_OK(cudaMemcpyAsync(ys.data(), y, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    for (int i = 0; i < N; ++i)
+      if (ys[i] < 0 || ys[i] >= K) fail("dp_debug_cw: label %d of sample %d outside [0, %d)", ys[i], i, K);
+    e->run(st, [&] { return dp::launch_cw(logits, y, targeted, confidence, inv_s, loss, preds, dlogits, N, K, st); });
+  });
+}
+
+// G images b of the samples [n0, n0 + n) are written where the launch holds b's first sample, otherwise added to.
+int32_t dp_debug_reduce(dp_engine* e, const void* dz, const int16_t* rects_host, const uint32_t* bank_dev, int32_t n_bank,
+                        const int32_t* idx_host, int32_t B, int32_t S, int32_t n0, int32_t n, float* G, void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!dz || !G || B < 1 || S < 1 || n0 < 0 || n < 1 || (int64_t)n0 + n > (int64_t)B * S)
+      fail("dp_debug_reduce: bad arguments (B=%d S=%d samples [%d, %d))", B, S, n0, n0 + n);
+    const bool banked = bank_dev || idx_host;
+    if (banked && rects_host) fail("dp_debug_reduce: rectangles or a mask bank, not both");
+    const int N = B * S, H = e->H;
+    if (banked) {
+      const dp::MaskBank bank = e->stage_bank(e->bank_idx_d, e->bank_idx_cap, bank_dev, n_bank, idx_host, N, "dp_debug_reduce", st);
+      e->run(st, [&] { return dp::launch_reduce(dz, nullptr, G, B, S, n0, n, H, H, e->stem.dx_ch, e->bf16, st, &bank); });
+    } else {
+      e->h2d_samples(rects_host, N, st);
+      const int16_t* rects = rects_host ? e->rects_d : nullptr;
+      e->run(st, [&] { return dp::launch_reduce(dz, rects, G, B, S, n0, n, H, H, e->stem.dx_ch, e->bf16, st); });
+    }
+  });
+}
+
 int32_t dp_debug_stem_bwd_pool_reduce(dp_engine* e, const void* dpool, const int8_t* amax, const int16_t* rects_host, int32_t B,
                                       int32_t S, float* G, void* stream) {
   return on_engine(e, stream, [&](cudaStream_t st) {

@@ -504,8 +504,18 @@ int launch_reduce_affine(const void* dz, const float* adv, const float* xf, cons
 }
 
 // =====================================================================================
-// K4: CW loss / argmax / dlogits -- one warp per sample
+// K4: CW loss / argmax / dlogits -- one warp per sample.  Bit for bit the reference's torch arithmetic (attack.py:16-23,
+// restated by oracle.attack.cw_loss) and its autograd gradient, scaled by w:
+//   real  = sum_k l[k] * onehot[k]   -> l[y], or NaN when any logit of the row is not finite (0 * inf = NaN)
+//   other = max_k ((1 - onehot) * l - onehot * 1e4)   -> the label slot holds -1e4
+//   loss  = clamp((confidence + other) - real, min=0)  (untargeted: (confidence + real) - other); NaN stays NaN
+// Maxima follow torch's max / argmax: NaN is the largest value, ties go to the lowest index, so the index is in [0, K).
 // =====================================================================================
+__device__ __forceinline__ bool cw_beats(float v, int i, float b, int bi) {   // does (v, i) replace the running max (b, bi)?
+  const bool vn = isnan(v), bn = isnan(b);
+  if (vn || bn) return vn && (!bn || i < bi);
+  return v > b || (v == b && i < bi);
+}
 __global__ void cw_kernel(const float* __restrict__ logits, const int32_t* __restrict__ y,
                           const uint8_t* __restrict__ targeted, float confidence, float w, float* __restrict__ loss,
                           int32_t* __restrict__ preds, float* __restrict__ dlogits, int N, int K) {
@@ -513,34 +523,36 @@ __global__ void cw_kernel(const float* __restrict__ logits, const int32_t* __res
   if (n >= N) return;
   const float* l = logits + (size_t)n * K;
   const int yy = y != nullptr ? y[n] : -1;
+  // (-inf, INT_MAX) loses to every (value, index) of the row: a lane without an element never wins
   float best = -INFINITY, obest = -INFINITY; int bi = 0x7fffffff, oi = 0x7fffffff;
+  bool finite = true;
   for (int k = lane; k < K; k += 32) {
     const float v = l[k];
-    if (v > best) { best = v; bi = k; }
-    if (k != yy && v > obest) { obest = v; oi = k; }
+    finite = finite && isfinite(v);
+    if (cw_beats(v, k, best, bi)) { best = v; bi = k; }
+    const float ov = k == yy ? -1e4f : v;   // attack.py:19: the label slot contributes -1e4
+    if (cw_beats(ov, k, obest, oi)) { obest = ov; oi = k; }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     const float v2 = __shfl_xor_sync(0xffffffffu, best, o); const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (v2 > best || (v2 == best && i2 < bi)) { best = v2; bi = i2; }
+    if (cw_beats(v2, i2, best, bi)) { best = v2; bi = i2; }
     const float w2 = __shfl_xor_sync(0xffffffffu, obest, o); const int j2 = __shfl_xor_sync(0xffffffffu, oi, o);
-    if (w2 > obest || (w2 == obest && j2 < oi)) { obest = w2; oi = j2; }
+    if (cw_beats(w2, j2, obest, oi)) { obest = w2; oi = j2; }
   }
   if (lane == 0 && preds != nullptr) preds[n] = bi;
   if (loss == nullptr) return;
-  const float real = l[yy];
-  // attack.py:19: the label slot contributes -1e4 to the max
-  const bool other_is_label_slot = !(obest > -1e4f);
-  const float other = other_is_label_slot ? -1e4f : obest;
+  finite = __all_sync(0xffffffffu, finite);
+  const float real = finite ? l[yy] : __int_as_float(0x7fffffff);
   const bool tg = targeted[n] != 0;
-  const float margin = tg ? (other - real) : (real - other);
-  const float pre = confidence + margin;
-  if (lane == 0) loss[n] = fmaxf(pre, 0.f);
+  const float pre = tg ? __fsub_rn(__fadd_rn(confidence, obest), real) : __fsub_rn(__fadd_rn(confidence, real), obest);
+  if (lane == 0) loss[n] = pre < 0.f ? 0.f : pre;
   if (dlogits != nullptr) {
     float* d = dlogits + (size_t)n * K;
     for (int k = lane; k < K; k += 32) d[k] = 0.f;
     __syncwarp();
-    if (lane == 0 && pre >= 0.f) {     // clamp(min=0) passes the gradient where input >= 0
+    const bool other_is_label_slot = oi == yy;   // its -1e4 is a constant: no gradient
+    if (lane == 0 && pre >= 0.f) {     // clamp(min=0) passes the gradient where input >= 0 (not NaN)
       d[yy] = tg ? -w : w;
       if (!other_is_label_slot) d[oi] = tg ? w : -w;
     }

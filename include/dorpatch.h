@@ -288,6 +288,20 @@ int32_t dp_debug_stem_bwd_reduce(dp_engine* e, const void* dY, const int16_t* re
 /* dp_debug_stem_bwd_reduce occluding from a mask bank (bank_dev / n_bank / idx_host as for dp_expand_bank). */
 int32_t dp_debug_stem_bwd_reduce_bank(dp_engine* e, const void* dY, const uint32_t* bank_dev, int32_t n_bank,
                                       const int32_t* idx_host, int32_t B, int32_t S, float* G, void* stream);
+/* K4 and K1^T on caller-supplied device buffers (tests/test_gpu_attack_ops.py), through the launches the engine runs.
+ * dp_debug_cw: the CW loss of logits [N,K] fp32 with labels y [N] int32 (each in [0, K), checked) and criterion flags
+ *   targeted [N] uint8: loss [N] fp32, preds [N] int32 (argmax, may be NULL) and dlogits [N,K] fp32 = d(inv_s * sum_n
+ *   loss_n)/d logits (may be NULL).  y == NULL: the argmax alone into preds.  Any N >= 1, K >= 1 (not only the engine's K).
+ * dp_debug_reduce: the masked EOT reduce of the fp32 / tf32 engines (and of the bf16 engine's DORPATCH_STEM_BWD=cudnn
+ *   end): G[b,c] (+)= 2 * sum over the samples s of image b in [n0, n0 + n) of keep_s * dz[s - n0][..][c], with dz
+ *   [n,H,W,c_pad] in the engine's activation dtype (c_pad = 4 at fp32 / tf32, 8 at bf16, or DORPATCH_CPAD).  An image
+ *   whose first sample is in the launch is written, any other added to.  The occlusion of the B*S samples is
+ *   rects_host [B*S][4][4] int16, or a mask bank (bank_dev / n_bank / idx_host [B*S][2] as for dp_expand_bank), or
+ *   neither (every pixel kept). */
+int32_t dp_debug_cw(dp_engine* e, const float* logits, const int32_t* y, const uint8_t* targeted, float confidence, float inv_s,
+                    float* loss, int32_t* preds, float* dlogits, int32_t N, int32_t K, void* stream);
+int32_t dp_debug_reduce(dp_engine* e, const void* dz, const int16_t* rects_host, const uint32_t* bank_dev, int32_t n_bank,
+                        const int32_t* idx_host, int32_t B, int32_t S, int32_t n0, int32_t n, float* G, void* stream);
 /* The bf16 engine's stem on caller-supplied tensors (tests/test_gpu_stem_ops.py), through the launches the engine runs.
  * G is written by the kernels alone: every element of every image, nothing is zeroed first.
  * dp_debug_stem_bwd_pool_reduce: dp_debug_stem_bwd_reduce with the max-pool backward fused in (DORPATCH_POOL_BWD=fused):

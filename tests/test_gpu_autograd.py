@@ -30,14 +30,14 @@ def _rects(H, B, S, seed, dropout=2):
 
 
 def _cw_dlogits(logits, y, targeted, confidence, w):
-    """d(w * sum_n cw_n)/d logits as the CW kernel forms it (attack.py:16-23; no top-2 ties in these inputs)."""
+    """d(w * sum_n cw_n)/d logits of the reference's CW loss (attack.py:16-23, its association order (confidence +
+    other) - real; no top-2 ties in these inputs)."""
     N, K = logits.shape
     onehot = F.one_hot(y, K).bool()
     real = logits[torch.arange(N), y]
     oi = logits.masked_fill(onehot, float("-inf")).argmax(1)
     other = logits[torch.arange(N), oi]
-    margin = torch.where(targeted, other - real, real - other)
-    live = (confidence + margin) >= 0
+    live = torch.where(targeted, (confidence + other) - real, (confidence + real) - other) >= 0
     d = torch.zeros_like(logits)
     sgn = torch.where(targeted, -1.0, 1.0).to(logits.device) * w
     d[torch.arange(N), y] = torch.where(live, sgn, 0.0)

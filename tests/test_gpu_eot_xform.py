@@ -49,13 +49,14 @@ def _xforms(B, S, seed, affine=0.1, colour=0.1):
 
 
 def _cw(logits, y, targeted, confidence, w):
-    """Per-sample CW loss and d(w * sum_n cw_n)/d logits as cw_kernel forms them (attack.py:16-23; no top-2 ties)."""
+    """Per-sample CW loss and d(w * sum_n cw_n)/d logits of the reference (attack.py:16-23, its association order
+    (confidence + other) - real; no top-2 ties)."""
     N, K = logits.shape
     n = torch.arange(N, device=logits.device)
     real = logits[n, y]
     oi = logits.masked_fill(F.one_hot(y, K).bool(), float("-inf")).argmax(1)
     other = logits[n, oi]
-    pre = confidence + torch.where(targeted, other - real, real - other)
+    pre = torch.where(targeted, (confidence + other) - real, (confidence + real) - other)
     live = pre >= 0
     d = torch.zeros_like(logits)
     sgn = torch.where(targeted, -1.0, 1.0).to(logits.device) * w

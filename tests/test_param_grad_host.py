@@ -13,7 +13,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 @pytest.mark.parametrize("name,nargs", [("dp_eot_backward_params", 8), ("dp_engine_load_weights_dev", 6),
                                         ("dp_debug_stem_wgrad", 6), ("dp_debug_gn_wgrad", 12),
                                         ("dp_debug_ws_backward", 10), ("dp_debug_stem_forward", 6),
-                                        ("dp_debug_maxpool", 10), ("dp_debug_stem_bwd_pool_reduce", 8)])
+                                        ("dp_debug_maxpool", 10), ("dp_debug_stem_bwd_pool_reduce", 8),
+                                        ("dp_debug_cw", 12), ("dp_debug_reduce", 12)])
 def test_header_and_signatures_declare_param_grad_entries(name, nargs):
     from dorpatch_b200 import _lib
     header = open(os.path.join(ROOT, "include", "dorpatch.h")).read()
