@@ -17,6 +17,8 @@ Semantics beyond the reference (see DESIGN.md):
   * EOT sharding: with torch.distributed initialised, each rank evaluates S/world samples and
     the ranks all-reduce the patch gradient once per step; the periodic universe scan
     (collect_failure) is split over the ranks by distinct occlusion and its fail bits all-gathered.
+    PatchCleanser evaluation shards its masked forwards with the same split (shard_range, sharded_predict,
+    sharded_checks).
   * ``pc_n_patch=2`` draws the universe from the two-patch PatchCleanser window (the reference
     always uses the one-patch window, attack.py:25-31); the universe scans forward each distinct
     occlusion once.
@@ -228,6 +230,61 @@ def exchange_shards(dist, G, loss_adv, preds, defer=False):
     return loss_all, preds_all
 
 
+def shard_range(n, rank, world, unit=1):
+    """The contiguous shard [lo, hi) of n items that `rank` of `world` takes: ceil(units / world) whole units of `unit`
+    items each, in rank order, the last unit keeping its length.  Every item lands in exactly one shard, cuts fall at
+    multiples of `unit` only, and a rank past the last unit gets an empty shard.  The one sharding convention of the
+    universe scan (unit 1) and of PatchCleanser's masked forwards (unit = the engine's chunk)."""
+    units = -(-n // unit)
+    per = -(-units // world) * unit
+    return min(rank * per, n), min((rank + 1) * per, n)
+
+
+def _all_gather_rows(dist, row, device):
+    """All-gather one equally long 1-D tensor per rank -> numpy [world, len] in rank order, on every rank."""
+    row = row.to(device)
+    outs = [torch.empty_like(row) for _ in range(dist.get_world_size())]
+    dist.all_gather(outs, row)
+    return torch.stack(outs).cpu().numpy()
+
+
+def collective_device(dist):
+    """Where the tensors of a collective live: the current GPU under NCCL, else the host (gloo)."""
+    return torch.device("cuda", torch.cuda.current_device()) if dist.get_backend() == "nccl" else torch.device("cpu")
+
+
+def sharded_predict(predict, n, chunk, dist=None):
+    """The int32 labels of one forward call over n samples that the engine runs in chunks of `chunk`:
+    `predict(lo, hi)` forwards samples [lo, hi) of the call as one call.  Without dist this is predict(0, n), the single
+    call.  With torch.distributed every rank forwards its shard_range in whole chunks, so each of its chunks holds the
+    samples of one chunk of the single call and gives the same logits (the engine computes a sample from its chunk
+    alone, DESIGN section 5); the labels are all-gathered in rank order and every rank returns the single call's array.
+    A rank with an empty shard forwards nothing and still joins the all-gather."""
+    if dist is None:
+        return np.asarray(predict(0, n), dtype=np.int32)
+    rank, world = dist.get_rank(), dist.get_world_size()
+    per = shard_range(n, 0, world, chunk)[1]
+    lo, hi = shard_range(n, rank, world, chunk)
+    mine = torch.zeros(per, dtype=torch.int32)
+    if hi > lo:
+        mine[:hi - lo] = torch.from_numpy(np.asarray(predict(lo, hi), dtype=np.int32))
+    return np.ascontiguousarray(_all_gather_rows(dist, mine, collective_device(dist)).reshape(-1)[:n])
+
+
+def sharded_checks(check, m, dist=None):
+    """[check(i) for i in range(m)] as bools, each check a whole call: without dist all of them in order on this rank;
+    with torch.distributed check i runs on rank i % world (round-robin in the given order) and the results are
+    all-gathered, so every rank returns the same list, in the same order.  m must be the same on every rank."""
+    if dist is None or m == 0:
+        return [bool(check(i)) for i in range(m)]
+    rank, world = dist.get_rank(), dist.get_world_size()
+    mine = torch.zeros(-(-m // world), dtype=torch.uint8)
+    for j, i in enumerate(range(rank, m, world)):
+        mine[j] = bool(check(i))
+    rows = _all_gather_rows(dist, mine, collective_device(dist))
+    return [bool(rows[i % world, i // world]) for i in range(m)]
+
+
 def scan_failures(predict, all_rects, y, targeted, dist=None, device="cpu", inv=None):
     """collect_failure for one image (attack.py:384-406): indices of the universe masks under
     which the attack fails.  `predict(rects[k,4,4]) -> labels[k]`.  With torch.distributed the
@@ -242,15 +299,12 @@ def scan_failures(predict, all_rects, y, targeted, dist=None, device="cpu", inv=
         f = np.asarray(predict(all_rects)) == y
     else:
         rank, world = dist.get_rank(), dist.get_world_size()
-        per = -(-n // world)
-        lo, hi = min(rank * per, n), min((rank + 1) * per, n)
+        per = shard_range(n, 0, world)[1]
+        lo, hi = shard_range(n, rank, world)
         bits = torch.zeros(per, dtype=torch.uint8)
         if hi > lo:
             bits[:hi - lo] = torch.from_numpy((np.asarray(predict(all_rects[lo:hi])) == y).astype(np.uint8))
-        bits = bits.to(device)
-        outs = [torch.empty_like(bits) for _ in range(world)]
-        dist.all_gather(outs, bits)
-        f = torch.cat(outs).cpu().numpy()[:n].astype(bool)
+        f = _all_gather_rows(dist, bits, device).reshape(-1)[:n].astype(bool)
     if inv is not None:
         f = f[inv]
     if targeted:

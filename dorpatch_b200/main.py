@@ -16,6 +16,9 @@ two-patch run never resumes from, or overwrites, one-patch patches.  The usual r
 --basic_unit N (default 7, the reference's) sets the side of the square cells the group lasso and patch_selection work
 on (DorPatch.generate(basic_unit=N)); it must divide the image size.  It changes the patches and the stage-0 mask, so a
 non-default unit is also appended to the first path component (`__basic_unit=N`).
+
+Under torchrun the PatchCleanser evaluation is sharded too (PatchCleanser(..., shard=True)): each rank forwards a share of
+every robust_predict call and the labels are gathered, so every rank holds the single-process records and rank 0 writes them (DESIGN section 5).
 """
 import argparse
 import os
@@ -73,7 +76,8 @@ parser.add_argument('--basic_unit', default=7, type=int,
 
 def _init_distributed():
     """Under torchrun (RANK / WORLD_SIZE / LOCAL_RANK set): one process per GPU, NCCL process group, the EOT axis of
-    every generate() call sharded over the ranks (attack._dist).  Returns (rank, world)."""
+    every generate() call and the masked forwards of every robust_predict call sharded over the ranks (attack._dist).
+    Returns (rank, world)."""
     if "RANK" not in os.environ or int(os.environ.get("WORLD_SIZE", "1")) < 2:
         return 0, 1
     import torch.distributed as dist
@@ -114,7 +118,8 @@ def main(args):
                              synthetic=args.synthetic, img_size=args.img_size)
     attack = DorPatch()
     img = args.img_size if args.synthetic else 224
-    defense = [PatchCleanser(MaskWindow(img, r, args.pc_n_patch), model) for r in [0.015, 0.03, 0.06, 0.12]]
+    # shard=True: every rank evaluates every image below, so robust_predict shares the forwards over the ranks
+    defense = [PatchCleanser(MaskWindow(img, r, args.pc_n_patch), model, shard=True) for r in [0.015, 0.03, 0.06, 0.12]]
     pc_name = "adv_PC_%d.pt" if args.pc_n_patch == 1 else "adv_PC2_%d.pt"
 
     target_list, preds_list, y_list, preds_adv_list, records = [], [], [], [], []

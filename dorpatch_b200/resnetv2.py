@@ -189,8 +189,10 @@ class ResNetV2(nn.Module):
             ent[0].close()
             ent = None
         if ent is None:
+            # DORPATCH_AUTOTUNE=0: library algorithms by heuristic instead of timing trials, the same in every process
             eng = Engine(img=img, n_classes=self.num_classes, precision=precision, chunk=chunk,
-                         max_images=max(int(max_images), 1))
+                         max_images=max(int(max_images), 1),
+                         autotune=os.environ.get("DORPATCH_AUTOTUNE", "1") != "0")
             eng.load_state_dict({k: v for k, v in self.state_dict().items()})
             eng._weights_state = self._param_state()
             from . import runtime

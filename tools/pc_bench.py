@@ -8,6 +8,12 @@ evaluation main.py runs per image -- on a random-init ResNetV2-50x1-BiT.  Per pr
 seconds per image, the masked forwards per image counted from the records (round 1 + round 2 + certificate) and their
 rate; as the yardstick for that rate, a plain dp_predict over the 2520-mask universe on the same engine.  Every shape is
 warmed up on an extra image first.  The GPU's name and power limit are read in the same process.
+
+    torchrun --nproc-per-node N tools/pc_bench.py [...]
+
+runs the same evaluation with the masked forwards sharded over N GPUs (every rank gets the single-GPU records); rank 0
+prints the line, with the world size, every rank's GPU name and power limit, and per window the masked forwards each
+rank ran.
 """
 import argparse
 import contextlib
@@ -32,10 +38,10 @@ IMG = 224
 RATIOS = (0.015, 0.03, 0.06, 0.12)
 
 
-def gpu_info():
-    info = {"name": torch.cuda.get_device_name(0)}
+def gpu_info(dev=0):
+    info = {"name": torch.cuda.get_device_name(dev)}
     try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+        q = subprocess.run(["nvidia-smi", "-i", str(dev), "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
                            capture_output=True, text=True, timeout=30).stdout.strip().split(",")
         info["power_limit_w"], info["max_sm_mhz"] = float(q[0]), float(q[1])
     except Exception as ex:            # the figures stay usable without it; the line says why the field is missing
@@ -53,8 +59,10 @@ def forwards(rec):
     return len(p1), round2, len(rec.preds_2)
 
 
-def evaluate(defs, images):
+def evaluate(defs, images, dist=None):
     torch.cuda.synchronize()
+    if dist:
+        dist.barrier()                           # every rank starts the timed window together
     t0 = time.perf_counter()
     recs = [[d.robust_predict(im, True) for d in defs] for im in images]
     torch.cuda.synchronize()                     # dp_predict already ends in a stream synchronise; this makes it explicit
@@ -68,7 +76,13 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("tools/pc_bench.py needs a CUDA device (H100)")
-    torch.cuda.set_device(0)
+    dist, rank, world = None, 0, 1
+    local = int(os.environ.get("LOCAL_RANK", "0"))
+    torch.cuda.set_device(local)
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:     # torchrun: one process per GPU, robust_predict shards over them
+        import torch.distributed as dist
+        dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+        rank, world = dist.get_rank(), dist.get_world_size()
     K = args.images
     g = torch.Generator().manual_seed(1234)
     x = torch.rand(K + 1, 3, IMG, IMG, generator=g).cuda()
@@ -78,7 +92,11 @@ def main():
     model = torch.nn.DataParallel(NormModel(net, get_normalize("imagenet", "resnetv2")))
     uni = PM.gather(PM.universe(IMG, 2), np.arange(2520))
     out = {"tool": "pc_bench", "img": IMG, "images": K, "ratios": list(RATIOS), "model": "ResNetV2-50x1-BiT random-init (seed 0)",
-           "gpu": gpu_info(), "legs": {}}
+           "gpu": gpu_info(local), "legs": {}}
+    if dist:
+        out["world"] = world
+        out["gpus"] = [None] * world
+        dist.all_gather_object(out["gpus"], out["gpu"])
     for prec in args.precisions.split(","):
         os.environ["DORPATCH_PRECISION"] = prec          # the engine PatchCleanser asks the model for
         eng = net.engine(IMG, max_images=K + 1)
@@ -86,9 +104,10 @@ def main():
         leg = {"chunk": eng.chunk}
         for n_patch in (1, 2):
             with contextlib.redirect_stdout(io.StringIO()):
-                defs = [PatchCleanser(MaskWindow(IMG, r, n_patch), model) for r in RATIOS]
-            evaluate(defs, adv[K:])                                             # warm-up image: every call shape once
-            dt, recs = evaluate(defs, adv[:K])
+                defs = [PatchCleanser(MaskWindow(IMG, r, n_patch), model, shard=True) for r in RATIOS]
+            evaluate(defs, adv[K:], dist)                                       # warm-up image: every call shape once
+            ran0 = sum(d.forwards for d in defs)
+            dt, recs = evaluate(defs, adv[:K], dist)
             n = np.array([[forwards(r) for r in row] for row in recs])          # [K, ratios, (round 1, round 2, certificate)]
             per_img = n.sum(axis=(1, 2))
             leg["n_patch_%d" % n_patch] = {
@@ -96,6 +115,10 @@ def main():
                 "forwards_per_image_by_round": dict(zip(("round1", "round2", "certificate"), n.sum(axis=1).mean(0).tolist())),
                 "forwards_per_s": float(per_img.sum()) / dt,
                 "certified": [[bool(r.certification) for r in row] for row in recs]}
+            if dist:
+                ran = [None] * world                                            # masked forwards each rank ran per image
+                dist.all_gather_object(ran, (sum(d.forwards for d in defs) - ran0) / K)
+                leg["n_patch_%d" % n_patch]["forwards_per_image_by_rank"] = ran
         img0 = x[:1].contiguous()
         eng.predict(img0, 2520, uni)
         ts = []
@@ -112,7 +135,10 @@ def main():
         out["legs"][prec] = leg
         eng.close()
         net._engines.clear()
-    print(json.dumps(out))
+    if rank == 0:
+        print(json.dumps(out))
+    if dist:
+        dist.destroy_process_group()
 
 
 if __name__ == "__main__":
