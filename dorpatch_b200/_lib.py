@@ -75,6 +75,11 @@ SIGNATURES = {
     "dp_failed_set_write": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_vp]),
     "dp_failed_set_update": (c_i32, [c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_f32, c_vp, c_vp]),
     "dp_failed_set_read": (c_i32, [c_vp, c_i32, c_vp, c_i32, c_vp, c_vp]),
+    "dp_failed_set_update_drawn": (c_i32, [c_vp, c_i32, c_i32, c_vp, c_vp, c_f32, c_vp, c_vp]),
+    "dp_eot_universe_upload": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp]),
+    "dp_eot_draw": (c_i32, [c_vp, c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    "dp_eot_draw_rects": (c_i32, [c_vp, c_vp, c_i32, c_vp]),
+    "dp_attack_grad_drawn": (c_i32, [c_vp, C.POINTER(DpAttackArgs), c_vp]),
     "dp_debug_stem_bwd_reduce": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp]),
     "dp_debug_stem_bwd_pool_reduce": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp]),
     "dp_debug_stem_forward": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),

@@ -22,6 +22,9 @@ Semantics beyond the reference (see DESIGN.md):
   * ``pc_n_patch=2`` draws the universe from the two-patch PatchCleanser window (the reference
     always uses the one-patch window, attack.py:25-31); the universe scans forward each distinct
     occlusion once.
+  * ``eot_sampler="device"`` draws the EOT occlusions on the GPU (dp_eot_draw): the rule of attack.py:193-218 from a
+    counter-based generator seeded per image, so the draws are reproducible but not numpy's; indices, rectangles and the
+    failed-set update never leave the device.
 """
 import os
 
@@ -320,14 +323,24 @@ class DorPatch(object):
     def generate(self, model, x, patch_budget, n_classes, save_dir, batch_id, y=None, targeted=False,
                  lr=1e-2, confidence=1e-1, clip_min=0, clip_max=1, max_iterations=5000, basic_unit=7,
                  selection='topk', dropout=2, sampling_size=128, density=1e-3, structured=1e-3, eps=4., dual=False,
-                 eot_affine=0.0, eot_colour=0.0, eot_seed=0, pc_n_patch=1, **kwargs):
+                 eot_affine=0.0, eot_colour=0.0, eot_seed=0, pc_n_patch=1, eot_sampler="host", **kwargs):
         """Reference signature (attack.py:51-53) plus three opt-in keywords for the affine / colour
         EOT extension (default 0 = off = the reference's behaviour).  `image_seeds=[s_0..s_{B-1}]` (keyword)
         makes row b of a B > 1 call replay the B == 1 run seeded with s_b (SURVEY section 0: parity of the
         batched configs is defined per image against a B == 1 reference run).
         `pc_n_patch=2` trains against the two-patch PatchCleanser: the EOT occlusions and the universe scans come from
         MaskWindow(W, r, 2) (dropout 1: its 630 pairs per ratio; dropout 2: its 22 680 three-rectangle masks per ratio)
-        instead of the reference's one-patch window (1, the default)."""
+        instead of the reference's one-patch window (1, the default).
+        `eot_sampler="device"` draws every step's EOT occlusions on the GPU (dp_eot_draw) instead of with numpy on the
+        host (`"host"`, the default and the reference's stream): the indices, their rectangles and the failed-set update
+        stay on the device, so a long run is paced by the GPU.  The draws are reproducible from per-image seeds --
+        `image_seeds[b]`, else B seeds drawn once from the global numpy stream -- but are not numpy's."""
+        if eot_sampler not in ("host", "device"):
+            raise ValueError("eot_sampler=%r: 'host' or 'device'" % (eot_sampler,))
+        on_device = eot_sampler == "device"
+        if on_device and os.environ.get("DORPATCH_FAILED", "device") == "host":
+            raise ValueError("eot_sampler='device' samples from the failed sets on the device; DORPATCH_FAILED=host keeps "
+                             "them on the host")
         W = x.shape[-1]
         if isinstance(basic_unit, bool) or not isinstance(basic_unit, (int, np.integer)) or basic_unit < 1 \
                 or W % basic_unit != 0:
@@ -389,7 +402,11 @@ class DorPatch(object):
         distinct, inv = _masks.distinct_occlusions(table, len(_masks.DROPOUT_SIZES))   # scans forward each once
         scan_rects = _masks.gather(distinct, np.arange(len(distinct)))
 
-        if image_seeds is not None:
+        if on_device:                                            # the draws' per-image seeds; no host stream
+            seeds = [int(s) for s in image_seeds] if image_seeds is not None else \
+                [int(np.random.randint(0, 2 ** 31 - 1)) for _ in range(B)]
+            rngs = [None] * B
+        elif image_seeds is not None:
             rngs = [np.random.RandomState(int(s)) for s in image_seeds]
         elif B == 1:
             rngs = [np.random]                                   # the global legacy stream, as the reference
@@ -402,6 +419,8 @@ class DorPatch(object):
             for b, s in enumerate(st):
                 s.dev = (eng, b)
                 s.set_failed([])
+        if on_device:
+            eng.eot_universe(table)
         dir_0 = os.path.dirname(save_dir.rstrip('/')) if save_dir else None
         G = torch.zeros_like(x)
         use_eot = (eot_affine != 0.0) or (eot_colour != 0.0)
@@ -426,6 +445,10 @@ class DorPatch(object):
             return failed
 
         def draw(i):                                             # attack.py:193-204 (+ :208-218 dual) for every active image
+            if on_device:                                        # indices and rectangles stay on the device
+                got = eng.eot_draw(seeds, stage, i, [s.active for s in st], S, dual, rank, world,
+                                   host=bool(dist) and i % 100 == 0)
+                return (got[0] if got else None), None, None, None
             idx = np.zeros((B, S), np.int64)
             idx2 = np.zeros((B, S), np.int64) if dual else None
             nff = [0] * B
@@ -493,7 +516,7 @@ class DorPatch(object):
                 # consumption is provably unchanged: the draw depends on nothing this step can alter (i+1 < 1000: no
                 # failed-set samples), the stage does run an iteration i+1, and no image can stop at step i (a stop needs
                 # lr * 0.1 < 1e-3 together with a plateau, i.e. not_decay >= PATIENCE before the step).
-                if _may_prefetch(st, i, max_iterations):
+                if not on_device and _may_prefetch(st, i, max_iterations):
                     prefetched = ((stage, i + 1), sampler.submit(draw, i + 1))
                 if dist and i % 100 == 0:
                     # every rank must have drawn the same indices (same RNG streams): a diverged rank would evaluate a
@@ -507,7 +530,7 @@ class DorPatch(object):
                     xf = _eot.sample(eot_rng, B, S, eot_affine, eot_colour)[:, rank * S_loc:(rank + 1) * S_loc]
                 r = eng.attack_grad(x, adv_mask, adv_pattern, rects, [s.y for s in st],
                                     [s.crit_targeted for s in st], confidence, eps, stage, G, S_total=S, xforms=xf,
-                                    basic_unit=basic_unit)
+                                    basic_unit=basic_unit, S=S_loc)
                 loss_adv, preds = r["loss_adv"], r["preds"]
                 reduce_work = None
                 if dist:                                         # one all-reduce of the patch gradient per step, under the bookkeeping
@@ -515,14 +538,17 @@ class DorPatch(object):
                 last_preds = preds
                 loss_target = r["group_lasso"] if stage == 0 else r["loss_struc"]
                 counts = None
-                if device_sets:                                  # attack.py:259-267 as one kernel over the bitmaps; the host reads set sizes only
+                if on_device:                                    # on the drawn indices, which never left the device
+                    counts = eng.failed_update_drawn(B, S, [s.active for s in st], loss=loss_adv if dist else None)
+                elif device_sets:                                # attack.py:259-267 as one kernel over the bitmaps; the host reads set sizes only
                     counts = eng.failed_update(idx, nff, [s.active for s in st], loss=loss_adv if dist else None)
                 lr_used = np.zeros(B, np.float32)
                 stopped_now = []
                 for b, s in enumerate(st):
                     if not s.active:
                         continue
-                    improved, stop = s.bookkeeping(stage, i, loss_adv[b], idx[b], nff[b], loss_target[b],
+                    improved, stop = s.bookkeeping(stage, i, loss_adv[b], None if on_device else idx[b],
+                                                   None if on_device else nff[b], loss_target[b],
                                                    n_failed=None if counts is None else counts[b])
                     if stop:
                         stopped_now.append(b)

@@ -163,6 +163,20 @@ struct dp_engine {
   int failed_masks = 4096, failed_words = 128, failed_words_alloc = 128;
   uint32_t* failed_bits = nullptr; int32_t* failed_count = nullptr; int32_t* failed_idx = nullptr; int32_t* failed_nff = nullptr;
   uint8_t* failed_active = nullptr; float* failed_loss = nullptr; int failed_cap = 0;
+  // on-device EOT draw (dp_eot_universe_upload / dp_eot_draw): the universe's rectangle table [uni_n][uni_k][4], the
+  // last draw's indices idx [B][S] | idx2 [B][S], nff [max_images], its local rectangles [B][S_loc][4][4] (what
+  // dp_attack_grad_drawn's K1 reads) and the kernel's scratch.  The draw's parameters go through draw_pin ->
+  // draw_par_d: seeds [max_images] uint64 | {stage, iter} int32 | active [max_images]; draw_ev marks the copy's end.
+  int16_t* uni_d = nullptr; int uni_n = 0, uni_k = 0, uni_cap = 0;
+  int32_t* draw_idx_d = nullptr; int32_t* draw_tmp_d = nullptr; int draw_cap = 0;
+  int16_t* draw_rects_d = nullptr; int draw_rects_cap = 0;
+  int32_t* draw_nff_d = nullptr; unsigned char* draw_par_d = nullptr; unsigned char* draw_pin = nullptr;
+  cudaEvent_t draw_ev = nullptr;
+  // the last draw's shape; `fresh` until dp_failed_set_update_drawn consumes it or a universe upload / set reset
+  // invalidates it
+  struct DrawSig { bool fresh = false; int B = 0, S = 0, S_loc = 0; bool dual = false; };
+  DrawSig draw;
+  size_t draw_par_bytes() const { return (size_t)cfg.max_images * 9 + 16; }
   float* helper_scale = nullptr; float* helper_l2 = nullptr; float* helper_ws = nullptr;   // scratch of dp_paste(out) / dp_window_sum
   float* lr_d = nullptr; float* structured_d = nullptr; float* coeff_d = nullptr;
   float* host_x = nullptr; float* host_mask = nullptr; float* host_pattern = nullptr; float* host_G = nullptr;  // dp_attack_step_host
@@ -428,6 +442,10 @@ struct dp_engine {
     failed_bits = (uint32_t*)dmalloc(B * failed_words_alloc * 4);
     CUDA_OK(cudaMemset(failed_bits, 0, B * failed_words_alloc * 4));
     failed_count = (int32_t*)dmalloc(B * 4); failed_nff = (int32_t*)dmalloc(B * 4); failed_active = (uint8_t*)dmalloc(B);
+    draw_nff_d = (int32_t*)dmalloc(B * 4);
+    draw_par_d = (unsigned char*)dmalloc(draw_par_bytes());
+    CUDA_OK(cudaMallocHost((void**)&draw_pin, draw_par_bytes()));
+    CUDA_OK(cudaEventCreateWithFlags(&draw_ev, cudaEventDisableTiming));
     win_dev = (float*)dmalloc(B * 64 * 4);
     grp_ss = (float*)dmalloc(B * HW * 4);
     ensure_samples(chunk);
@@ -1191,6 +1209,11 @@ struct dp_engine {
     stage(table, cap, idx_host, N, 2 * sizeof(int32_t), st);
     return dp::MaskBank{bank, table, H, H};
   }
+  // A dp_eot_draw of B images x S samples that no dp_failed_set_update_drawn, universe upload or set reset has used up.
+  void check_drawn(const char* fn, int B, int S) const {
+    if (!draw.fresh) fail("%s: no fresh dp_eot_draw (each draw serves one step: dp_attack_grad_drawn, then dp_failed_set_update_drawn)", fn);
+    if (B != draw.B || S != draw.S) fail("%s: B=%d x S=%d, the last draw is %d x %d", fn, B, S, draw.B, draw.S);
+  }
   void check_B(int B) const {
     if (B < 1 || B > cfg.max_images) fail("B=%d outside [1, max_images=%d]", B, cfg.max_images);
   }
@@ -1335,6 +1358,8 @@ void dp_engine_destroy(dp_engine* e) {
   if (e->net_in_all) cudaFree(e->net_in_all);
   for (void* p : e->allocs) cudaFree(p);
   if (e->pin) cudaFreeHost(e->pin);
+  if (e->draw_pin) cudaFreeHost(e->draw_pin);
+  if (e->draw_ev) cudaEventDestroy(e->draw_ev);
   if (e->lt) cublasLtDestroy(e->lt);
   delete e;
 }
@@ -1502,7 +1527,8 @@ int32_t dp_predict_bank(dp_engine* e, const float* img, int32_t B, int32_t S, co
 
 // Everything dp_attack_grad puts on the stream: staging H2D copies, per-image kernels, the chunk loop on one or two
 // lanes, result D2H copies into the pinned staging area.  No host synchronisation inside (capturable).
-struct GradLayout { size_t rect_bytes, xf_bytes, d2h_off; int32_t* ys; uint8_t* tg; unsigned char* rp; };
+// rects_dev: the occlusions are already on the device (dp_attack_grad_drawn: the last dp_eot_draw's rectangles).
+struct GradLayout { size_t rect_bytes, xf_bytes, d2h_off; int32_t* ys; uint8_t* tg; unsigned char* rp; const int16_t* rects_dev; };
 static void attack_grad_enqueue(dp_engine* e, const dp_attack_args* a, const GradLayout& L_, cudaStream_t st) {
   const int B = a->B, S = a->S, N = B * S, H = e->H;
   const size_t rect_bytes = L_.rect_bytes, xf_bytes = L_.xf_bytes;
@@ -1513,7 +1539,7 @@ static void attack_grad_enqueue(dp_engine* e, const dp_attack_args* a, const Gra
     CUDA_OK(cudaMemcpyAsync(e->xf_d, L_.rp + rect_bytes, xf_bytes, cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaMemsetAsync(a->grad_adv, 0, (size_t)B * 3 * H * H * sizeof(float), st));   // the adjoint scatters with atomics
   }
-  const int16_t* rects = rect_bytes ? e->rects_d : nullptr;
+  const int16_t* rects = rect_bytes ? e->rects_d : L_.rects_dev;
 
   const double img_bytes = (double)B * H * H * 4;
   e->run("paste", 10.0 * img_bytes, 0, st, [&] { return dp::launch_paste(a->x, a->mask, a->pattern, e->adv_x, e->l2, e->scale, B, H, H, a->eps, st); });
@@ -1553,7 +1579,7 @@ static void attack_grad_enqueue(dp_engine* e, const dp_attack_args* a, const Gra
   d2h(e->l2, (size_t)B * 4);
 }
 
-static void attack_grad_impl(dp_engine* e, const dp_attack_args* a, cudaStream_t st) {
+static void attack_grad_impl(dp_engine* e, const dp_attack_args* a, cudaStream_t st, const int16_t* rects_dev = nullptr) {
   NvtxRange nvtx_("dorpatch.attack_grad");
   if (!a) fail("null args");
   e->check_B(a->B);
@@ -1570,6 +1596,7 @@ static void attack_grad_impl(dp_engine* e, const dp_attack_args* a, cudaStream_t
   // [H2D region: ys | tg | rects | xforms][D2H region: results]; the regions never overlap.
   GradLayout L_;
   L_.rect_bytes = a->rects_host ? (size_t)N * dp::RECT_SHORTS * sizeof(int16_t) : 0;
+  L_.rects_dev = rects_dev;
   L_.xf_bytes = a->xform_host ? (size_t)N * 8 * sizeof(float) : 0;
   const size_t h2d_bytes = (((size_t)N * 5 + 15) / 16) * 16 + L_.rect_bytes + L_.xf_bytes;
   L_.d2h_off = (h2d_bytes + 255) / 256 * 256;
@@ -1586,7 +1613,7 @@ static void attack_grad_impl(dp_engine* e, const dp_attack_args* a, cudaStream_t
 
   bool done = false;
   if (e->graphs_on && !e->prof_on && !L_.xf_bytes) {
-    dp_engine::GraphKey key{B, S, a->S_total, a->stage, a->x, a->mask, a->pattern, a->grad_adv, a->eps, a->confidence, L_.rect_bytes ? 1 : 0, unit};
+    dp_engine::GraphKey key{B, S, a->S_total, a->stage, a->x, a->mask, a->pattern, a->grad_adv, a->eps, a->confidence, L_.rect_bytes ? 1 : (rects_dev ? 2 : 0), unit};
     dp_engine::GraphEnt& ent = e->graphs[key];
     ++ent.calls;
     if (ent.exec != nullptr) {
@@ -1659,6 +1686,16 @@ static void attack_update_impl(dp_engine* e, const dp_update_args* u, cudaStream
 int32_t dp_attack_grad(dp_engine* e, const dp_attack_args* a, void* stream) {
   return on_engine(e, stream, [&](cudaStream_t st) {
     attack_grad_impl(e, a, st);
+  });
+}
+
+int32_t dp_attack_grad_drawn(dp_engine* e, const dp_attack_args* a, void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!a) fail("null args");
+    if (a->rects_host) fail("dp_attack_grad_drawn: rects_host must be NULL: the occlusions are the last dp_eot_draw's");
+    e->check_drawn("dp_attack_grad_drawn", a->B, a->S_total);
+    if (a->S != e->draw.S_loc) fail("dp_attack_grad_drawn: S=%d, the draw's local slice has %d samples", a->S, e->draw.S_loc);
+    attack_grad_impl(e, a, st, e->draw_rects_d);
   });
 }
 
@@ -1919,6 +1956,7 @@ int32_t dp_failed_set_reset(dp_engine* e, int32_t n_mask, void* stream) {
     }
     e->failed_masks = n_mask;
     e->failed_words = words;
+    e->draw.fresh = false;
     CUDA_OK(cudaMemsetAsync(e->failed_bits, 0, B * words * 4, st));
     CUDA_OK(cudaStreamSynchronize(st));
   });
@@ -1937,32 +1975,126 @@ int32_t dp_failed_set_write(dp_engine* e, int32_t b, const int32_t* idx_host, in
   });
 }
 
+// One step of the failed-set update from the sampled indices idx_dev [B*S] and nff_dev [B] already on the device.
+static void failed_update_impl(dp_engine* e, int B, int S, const int32_t* idx_dev, const int32_t* nff_dev, const uint8_t* active_host,
+                               const float* loss_host, float thresh, int32_t* count_host, cudaStream_t st) {
+  const int N = B * S;
+  CUDA_OK(cudaMemcpyAsync(e->failed_active, active_host, (size_t)B, cudaMemcpyHostToDevice, st));
+  const float* loss = e->loss_d;                       // default: the per-sample CW losses the last dp_attack_grad left on the device
+  if (loss_host != nullptr) {                          // EOT-sharded runs pass the all-gathered losses
+    CUDA_OK(cudaMemcpyAsync(e->failed_loss, loss_host, (size_t)N * 4, cudaMemcpyHostToDevice, st));
+    loss = e->failed_loss;
+  } else if (N > e->cap_samples) fail("dp_failed_set_update: no device losses for %d samples", N);
+  e->run(st, [&] {
+    return dp::launch_failed_update(e->failed_bits, e->failed_words, idx_dev, loss, nff_dev, e->failed_active, B, S, thresh,
+                                    e->failed_count, st);
+  });
+  CUDA_OK(cudaMemcpyAsync(count_host, e->failed_count, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+}
+static void ensure_failed_cap(dp_engine* e, int N) {
+  if (N <= e->failed_cap) return;
+  e->failed_cap = std::max(N, e->failed_cap * 2);
+  e->failed_idx = (int32_t*)e->dmalloc((size_t)e->failed_cap * 4);
+  e->failed_loss = (float*)e->dmalloc((size_t)e->failed_cap * 4);
+}
+
 int32_t dp_failed_set_update(dp_engine* e, int32_t B, int32_t S, const int32_t* idx_host, const int32_t* nff_host, const uint8_t* active_host,
                              const float* loss_host, float thresh, int32_t* count_host, void* stream) {
   return on_engine(e, stream, [&](cudaStream_t st) {
     e->check_B(B);
     if (S < 1 || !idx_host || !nff_host || !active_host || !count_host) fail("dp_failed_set_update: bad arguments");
     const int N = B * S;
-    if (N > e->failed_cap) {
-      e->failed_cap = std::max(N, e->failed_cap * 2);
-      e->failed_idx = (int32_t*)e->dmalloc((size_t)e->failed_cap * 4);
-      e->failed_loss = (float*)e->dmalloc((size_t)e->failed_cap * 4);
-    }
+    ensure_failed_cap(e, N);
     for (int i = 0; i < N; ++i)
       if (idx_host[i] < 0 || idx_host[i] >= e->failed_masks) fail("mask index %d outside [0, %d)", idx_host[i], e->failed_masks);
     CUDA_OK(cudaMemcpyAsync(e->failed_idx, idx_host, (size_t)N * 4, cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaMemcpyAsync(e->failed_nff, nff_host, (size_t)B * 4, cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaMemcpyAsync(e->failed_active, active_host, (size_t)B, cudaMemcpyHostToDevice, st));
-    const float* loss = e->loss_d;                       // default: the per-sample CW losses the last dp_attack_grad left on the device
-    if (loss_host != nullptr) {                          // EOT-sharded runs pass the all-gathered losses
-      CUDA_OK(cudaMemcpyAsync(e->failed_loss, loss_host, (size_t)N * 4, cudaMemcpyHostToDevice, st));
-      loss = e->failed_loss;
-    } else if (N > e->cap_samples) fail("dp_failed_set_update: no device losses for %d samples", N);
-    e->run(st, [&] {
-      return dp::launch_failed_update(e->failed_bits, e->failed_words, e->failed_idx, loss, e->failed_nff, e->failed_active, B, S, thresh,
-                                      e->failed_count, st);
+    failed_update_impl(e, B, S, e->failed_idx, e->failed_nff, active_host, loss_host, thresh, count_host, st);
+  });
+}
+
+int32_t dp_failed_set_update_drawn(dp_engine* e, int32_t B, int32_t S, const uint8_t* active_host, const float* loss_host, float thresh,
+                                   int32_t* count_host, void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    e->check_B(B);
+    if (!active_host || !count_host) fail("dp_failed_set_update_drawn: bad arguments");
+    e->check_drawn("dp_failed_set_update_drawn", B, S);
+    ensure_failed_cap(e, B * S);
+    e->draw.fresh = false;                             // one update per draw: the next step draws again
+    failed_update_impl(e, B, S, e->draw_idx_d, e->draw_nff_d, active_host, loss_host, thresh, count_host, st);
+  });
+}
+
+/* ---- on-device EOT draw (DorPatch.generate(eot_sampler="device")) ------------------------------------------- */
+int32_t dp_eot_universe_upload(dp_engine* e, const int16_t* table_host, int32_t n_mask, int32_t k, void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!table_host || n_mask < 1 || k < 1 || k > 4) fail("dp_eot_universe_upload: bad arguments (n_mask=%d, k=%d)", n_mask, k);
+    if (dp::eot_draw_smem_bytes(n_mask) > (size_t)227 << 10) fail("dp_eot_universe_upload: %d masks exceed the draw kernel's shared memory", n_mask);
+    e->draw.fresh = false;
+    e->stage(e->uni_d, e->uni_cap, table_host, n_mask * k * 4, sizeof(int16_t), st);
+    e->uni_n = n_mask;
+    e->uni_k = k;
+  });
+}
+
+int32_t dp_eot_draw(dp_engine* e, int32_t B, int32_t S, const uint64_t* seeds_host, int32_t stage, int32_t iter, const uint8_t* active_host,
+                    int32_t dual, int32_t rank, int32_t world, int32_t* idx_host_out, int32_t* idx2_host_out, int32_t* nff_host_out,
+                    void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    NvtxRange nvtx_("dorpatch.eot_draw");
+    e->check_B(B);
+    if (!seeds_host || !active_host) fail("dp_eot_draw: null seeds or active flags");
+    if (e->uni_n == 0) fail("dp_eot_draw: no universe uploaded (dp_eot_universe_upload)");
+    if (S < 1 || S > e->uni_n) fail("dp_eot_draw: S=%d outside [1, n_mask=%d]", S, e->uni_n);
+    if (e->uni_n > e->failed_masks)
+      fail("dp_eot_draw: the universe's %d masks exceed the failed-set bitmaps of %d (dp_failed_set_reset)", e->uni_n, e->failed_masks);
+    if (world < 1 || rank < 0 || rank >= world || S % world != 0) fail("dp_eot_draw: rank %d of world %d does not slice S=%d", rank, world, S);
+    if (dual && e->uni_k > 2) fail("dp_eot_draw: dual needs <= 2 rectangles per universe mask, the universe has %d", e->uni_k);
+    if (idx2_host_out && !dual) fail("dp_eot_draw: idx2_host_out without dual");
+    if (stage < 0 || stage > 255 || iter < 0) fail("dp_eot_draw: bad step (stage %d, iteration %d)", stage, iter);
+    const int N = B * S, S_loc = S / world;
+    if (2 * N > e->draw_cap) {                           // the old buffers stay in `allocs` until destroy
+      e->draw_cap = std::max(2 * N, 2 * e->draw_cap);
+      e->draw_idx_d = (int32_t*)e->dmalloc((size_t)e->draw_cap * 4);
+      e->draw_tmp_d = (int32_t*)e->dmalloc((size_t)e->draw_cap * 4);
+    }
+    if (B * S_loc > e->draw_rects_cap) {
+      e->drop_graphs();                                  // captured dp_attack_grad_drawn launches hold the old rectangles
+      e->draw_rects_cap = std::max(B * S_loc, 2 * e->draw_rects_cap);
+      e->draw_rects_d = (int16_t*)e->dmalloc((size_t)e->draw_rects_cap * dp::RECT_SHORTS * sizeof(int16_t));
+    }
+    // staged parameters: seeds [B] | {stage, iter} | active [B]
+    CUDA_OK(cudaEventSynchronize(e->draw_ev));           // the previous draw's copy has left draw_pin
+    const size_t o_step = (size_t)B * 8, o_act = o_step + 8;
+    memcpy(e->draw_pin, seeds_host, (size_t)B * 8);
+    const int32_t step[2] = {stage, iter};
+    memcpy(e->draw_pin + o_step, step, sizeof(step));
+    memcpy(e->draw_pin + o_act, active_host, (size_t)B);
+    CUDA_OK(cudaMemcpyAsync(e->draw_par_d, e->draw_pin, o_act + B, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaEventRecord(e->draw_ev, st));
+    int32_t* idx2 = dual ? e->draw_idx_d + N : nullptr;
+    const double words = (e->uni_n + 31) / 32;
+    e->run("eot_draw", (double)B * (words * 4 + (double)N / B * 4 * (dual ? 2 : 1) + (double)S_loc * dp::RECT_SHORTS * 2), 0, st, [&] {
+      return dp::launch_eot_draw(e->failed_bits, e->failed_words, e->uni_d, e->uni_n, e->uni_k, (const uint64_t*)e->draw_par_d,
+                                 (const int32_t*)(e->draw_par_d + o_step), e->draw_par_d + o_act, B, S, dual ? 1 : 0, S_loc,
+                                 rank * S_loc, e->draw_idx_d, idx2, e->draw_nff_d, e->draw_rects_d, e->draw_tmp_d, st);
     });
-    CUDA_OK(cudaMemcpyAsync(count_host, e->failed_count, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    e->draw.fresh = true; e->draw.B = B; e->draw.S = S; e->draw.S_loc = S_loc; e->draw.dual = dual != 0;
+    if (idx_host_out || idx2_host_out || nff_host_out) {
+      if (idx_host_out) CUDA_OK(cudaMemcpyAsync(idx_host_out, e->draw_idx_d, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
+      if (idx2_host_out) CUDA_OK(cudaMemcpyAsync(idx2_host_out, idx2, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
+      if (nff_host_out) CUDA_OK(cudaMemcpyAsync(nff_host_out, e->draw_nff_d, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+      CUDA_OK(cudaStreamSynchronize(st));
+    }
+  });
+}
+
+int32_t dp_eot_draw_rects(dp_engine* e, int16_t* rects_host_out, int32_t n, void* stream) {
+  return on_engine(e, stream, [&](cudaStream_t st) {
+    if (!e->draw.fresh) fail("dp_eot_draw_rects: no fresh dp_eot_draw");
+    if (!rects_host_out || n != e->draw.B * e->draw.S_loc) fail("dp_eot_draw_rects: the last draw has %d samples, buffer holds %d", e->draw.B * e->draw.S_loc, n);
+    CUDA_OK(cudaMemcpyAsync(rects_host_out, e->draw_rects_d, (size_t)n * dp::RECT_SHORTS * sizeof(int16_t), cudaMemcpyDeviceToHost, st));
     CUDA_OK(cudaStreamSynchronize(st));
   });
 }

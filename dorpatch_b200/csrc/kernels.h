@@ -137,6 +137,13 @@ int launch_update(const float* x, float* mask, float* pattern, const float* G, c
 // failed-mask bitmap update of one step (attack.py:259-267) + popcount per image
 int launch_failed_update(uint32_t* bits, int words, const int32_t* idx, const float* loss, const int32_t* nff, const uint8_t* active,
                          int B, int S, float thresh, int32_t* count, cudaStream_t st);
+// on-device EOT draw of every active image (attack.py:193-218 semantics, Philox4x32-10 keyed by seeds[b]):
+// idx / idx2 [B][S] (idx2 with dual), nff [B], the local slice [lo, lo + S_loc) gathered from the universe table
+// [n_mask][k][4] into rects [B][S_loc][4][4].  step = {stage, iter} dev; tmp: [B][S] scratch.
+size_t eot_draw_smem_bytes(int n_mask);
+int launch_eot_draw(const uint32_t* failed_bits, int failed_words, const int16_t* table, int n_mask, int k, const uint64_t* seeds,
+                    const int32_t* step, const uint8_t* active, int B, int S, int dual, int S_loc, int lo, int32_t* idx,
+                    int32_t* idx2, int32_t* nff, int16_t* rects, int32_t* tmp, cudaStream_t st);
 // k x k window sums of [B,1,H,W] (optionally of the squares)
 int launch_window_sum(const float* t, float* out, int B, int H, int W, int k, bool square, cudaStream_t st);
 

@@ -8,6 +8,7 @@
 //   struct   attack.py:33-45,227-228                        structural loss + its (one-sided) gradient
 //   maskreg  attack.py:72-80,235-245                        density + group-lasso values / statistics
 //   update   K3: attack.py:332-342                          chain rule through clip + sign step + clip
+//   eot_draw attack.py:193-218 (eot_sampler="device")       EOT indices + rectangles from Philox, per image
 // (file:line into the reference).  Images are NCHW fp32; network input is NHWC(Cp) T.
 #include <cstdlib>
 #include <type_traits>
@@ -877,6 +878,141 @@ __global__ void failed_update_kernel(uint32_t* __restrict__ bits, int words, con
 int launch_failed_update(uint32_t* bits, int words, const int32_t* idx, const float* loss, const int32_t* nff, const uint8_t* active,
                          int B, int S, float thresh, int32_t* count, cudaStream_t st) {
   failed_update_kernel<<<B, 128, 0, st>>>(bits, words, idx, loss, nff, active, S, thresh, count);
+  return 1;
+}
+
+// =====================================================================================
+// On-device EOT draw (DorPatch.generate(eot_sampler="device"); the semantics of attack.py:193-218, not numpy's stream).
+// One CTA per image.  For draw d (0; 1 = the dual draw) of image b at step (stage, iter):
+//   n_ff = iter >= 1000 ? min(|F_b|, S/2) : 0, |F_b| = the set bits of the image's failed bitmap below n_mask;
+//   positions [0, n_ff): n_ff distinct members of F_b (distinct ranks, each mapped to its set bit by prefix popcounts);
+//   positions [n_ff, S): S - n_ff distinct universe indices, drawn independently of the first part.
+// Each part is Floyd's exact sampling without replacement (a membership bitmap in shared memory) followed by a
+// Fisher-Yates shuffle, so every ordered selection is equally likely and any slice of positions is a uniform sample.
+// Every random number is Philox4x32-10 keyed by seed_b at the counter (position, iter, stage | draw | part, attempt):
+// a draw depends on nothing but (seed_b, stage, iter) and the image's set -- not on B, the other images, the rank or on
+// whether the launch is replayed from a graph.  Then the CTA gathers its local slice [rank_lo, rank_lo + S_loc) of the
+// universe table [n_mask][k][4] into rects [B][S_loc][4][4] (masks.gather's layout: the k rectangles in slots 0..k-1, the
+// dual draw's in slots 2-3, the rest empty).  An inactive image is left untouched.
+// =====================================================================================
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u; k.y += 0xBB67AE85u;
+  }
+  return c;
+}
+// Uniform integer in [0, n), n >= 1: Lemire's multiply-shift with rejection of the 2^32 mod n low products (exact).
+// The candidates are the four words of each Philox block, attempt 0, 1, ... in the counter's last word.
+__device__ __forceinline__ uint32_t draw_below(uint2 key, uint32_t pos, uint32_t iter, uint32_t tag, uint32_t n) {
+  const uint32_t reject = (0u - n) % n;
+  for (uint32_t attempt = 0;; ++attempt) {
+    const uint4 r = philox4x32_10(make_uint4(pos, iter, tag, attempt), key);
+    const uint32_t w[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uint64_t m = (uint64_t)w[j] * n;
+      if ((uint32_t)m >= reject) return (uint32_t)(m >> 32);
+    }
+  }
+}
+// m distinct values of [0, n) into out[0..m) in uniformly random order, by the whole CTA.  `seen` holds ceil(n/32)
+// zeroed words and is left dirty; tmp is scratch of m words.  tag: stage | draw << 8 | part << 16, the Floyd pass and
+// the shuffle taking parts p and p + 1.  The random numbers do not depend on each other and are drawn in parallel; the
+// membership pass and the swaps are serial (thread 0).
+__device__ void sample_distinct(uint2 key, uint32_t iter, uint32_t tag, int n, int m, uint32_t* seen, int32_t* out, int32_t* tmp) {
+  for (int s = threadIdx.x; s < m; s += blockDim.x) {
+    out[s] = (int32_t)draw_below(key, (uint32_t)s, iter, tag, (uint32_t)(n - m + s) + 1u);   // Floyd step s: one of [0, n - m + s]
+    if (s > 0) tmp[s] = (int32_t)draw_below(key, (uint32_t)s, iter, tag + (1u << 16), (uint32_t)s + 1u);   // Fisher-Yates
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < m; ++s) {                        // Floyd: a value already taken is replaced by j = n - m + s
+      int t = out[s];
+      if (seen[t >> 5] & (1u << (t & 31))) t = n - m + s;
+      seen[t >> 5] |= 1u << (t & 31);
+      out[s] = t;
+    }
+    for (int s = m - 1; s > 0; --s) { const int u = tmp[s]; const int32_t v = out[s]; out[s] = out[u]; out[u] = v; }
+  }
+  __syncthreads();
+}
+
+struct DrawShape { int B, S, n_mask, k, dual, S_loc, lo; };
+__global__ void __launch_bounds__(256) eot_draw_kernel(const uint32_t* __restrict__ failed_bits, int failed_words,
+                                                       const int16_t* __restrict__ table, const uint64_t* __restrict__ seeds,
+                                                       const int32_t* __restrict__ step, const uint8_t* __restrict__ active,
+                                                       DrawShape sh, int32_t* __restrict__ idx, int32_t* __restrict__ idx2,
+                                                       int32_t* __restrict__ nff, int16_t* __restrict__ rects,
+                                                       int32_t* __restrict__ tmp) {
+  extern __shared__ uint32_t draw_smem[];
+  const int b = blockIdx.x;
+  if (!active[b]) return;
+  const int words = (sh.n_mask + 31) >> 5;
+  uint32_t* seen = draw_smem;                            // [words] Floyd membership bitmap
+  int* prefix = (int*)(draw_smem + words);               // [words] set bits of the failed bitmap before each word
+  __shared__ int part_sum[256], n_set_s;
+  const uint32_t* fb = failed_bits + (size_t)b * failed_words;
+  const uint32_t last = (sh.n_mask & 31) ? (1u << (sh.n_mask & 31)) - 1u : ~0u;
+  auto fword = [&](int w) { return w < words - 1 ? fb[w] : (fb[w] & last); };
+  // exclusive prefix popcounts: each thread one contiguous run of words, then a scan over the 256 run sums
+  const int per = (words + blockDim.x - 1) / blockDim.x, w0 = threadIdx.x * per, w1 = min(words, w0 + per);
+  int c = 0;
+  for (int w = w0; w < w1; ++w) c += __popc(fword(w));
+  part_sum[threadIdx.x] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int acc = 0;
+    for (int t = 0; t < (int)blockDim.x; ++t) { const int v = part_sum[t]; part_sum[t] = acc; acc += v; }
+    n_set_s = acc;
+  }
+  __syncthreads();
+  c = part_sum[threadIdx.x];
+  for (int w = w0; w < w1; ++w) { prefix[w] = c; c += __popc(fword(w)); }
+  const int n_set = n_set_s;
+  const int n_ff = step[1] >= 1000 ? min(n_set, sh.S / 2) : 0;
+  const uint2 key = make_uint2((uint32_t)seeds[b], (uint32_t)(seeds[b] >> 32));
+  const uint32_t iter = (uint32_t)step[1];
+  if (threadIdx.x == 0) nff[b] = n_ff;
+  for (int d = 0; d <= sh.dual; ++d) {
+    int32_t* row = (d ? idx2 : idx) + (size_t)b * sh.S;
+    const uint32_t tag = (uint32_t)step[0] | ((uint32_t)d << 8);
+    for (int part = 0; part < 2; ++part) {               // 0: ranks into F_b, 1: universe indices
+      const int n = part ? sh.n_mask : n_set, m = part ? sh.S - n_ff : n_ff;
+      if (m == 0) continue;
+      for (int w = threadIdx.x; w < words; w += blockDim.x) seen[w] = 0u;
+      __syncthreads();
+      sample_distinct(key, iter, tag | ((uint32_t)(2 * part) << 16), n, m, seen, row + (part ? n_ff : 0), tmp + (size_t)b * sh.S);
+    }
+    for (int s = threadIdx.x; s < n_ff; s += blockDim.x) {   // rank r -> the r-th set bit of F_b
+      const int r = row[s];
+      int lo = 0, hi = words - 1;                        // the last word whose prefix is <= r
+      while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (prefix[mid] <= r) lo = mid; else hi = mid - 1; }
+      uint32_t v = fword(lo);
+      for (int skip = r - prefix[lo]; skip > 0; --skip) v &= v - 1u;
+      row[s] = lo * 32 + __ffs(v) - 1;
+    }
+    __syncthreads();
+  }
+  for (int e = threadIdx.x; e < sh.S_loc * RECT_SHORTS; e += blockDim.x) {
+    const int s = e / RECT_SHORTS, slot = (e % RECT_SHORTS) >> 2, q = e & 3;
+    int16_t v = 0;
+    if (slot < sh.k) v = table[((size_t)idx[(size_t)b * sh.S + sh.lo + s] * sh.k + slot) * 4 + q];
+    else if (sh.dual && slot >= 2) v = table[((size_t)idx2[(size_t)b * sh.S + sh.lo + s] * sh.k + slot - 2) * 4 + q];
+    rects[((size_t)b * sh.S_loc + s) * RECT_SHORTS + e % RECT_SHORTS] = v;
+  }
+}
+size_t eot_draw_smem_bytes(int n_mask) { return (size_t)2 * ((n_mask + 31) / 32) * 4; }
+int launch_eot_draw(const uint32_t* failed_bits, int failed_words, const int16_t* table, int n_mask, int k, const uint64_t* seeds,
+                    const int32_t* step, const uint8_t* active, int B, int S, int dual, int S_loc, int lo, int32_t* idx,
+                    int32_t* idx2, int32_t* nff, int16_t* rects, int32_t* tmp, cudaStream_t st) {
+  const size_t smem = eot_draw_smem_bytes(n_mask);
+  if (smem > (48 << 10)) cudaFuncSetAttribute(eot_draw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  eot_draw_kernel<<<B, 256, smem, st>>>(failed_bits, failed_words, table, seeds, step, active, DrawShape{B, S, n_mask, k, dual, S_loc, lo},
+                                        idx, idx2, nff, rects, tmp);
   return 1;
 }
 

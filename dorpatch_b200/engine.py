@@ -329,13 +329,20 @@ class Engine:
         return out
 
     def attack_grad(self, x, mask, pattern, rects, y, crit_targeted, confidence, eps, stage, grad_adv,
-                    S_total=None, host=False, xforms=None, basic_unit=7):
+                    S_total=None, host=False, xforms=None, basic_unit=7, S=None):
         """attack.py:184-247.  rects [B,S,4,4] int16; y [B]; crit_targeted [B] bool; basic_unit: side of the
         group-lasso groups (must divide H), which the following attack_update also uses.
+        rects=None: the occlusions are the last eot_draw's rectangles on the device (dp_attack_grad_drawn); S is then
+        the draw's local slice and S_total its S.
         Fills grad_adv [B,3,H,W] and returns a dict of host numpy results."""
         B = x.shape[0]
-        rects = np.ascontiguousarray(rects, dtype=np.int16)
-        S = rects.size // (B * 16)
+        drawn = rects is None
+        if drawn:
+            if host or S is None:
+                raise ValueError("attack_grad on the drawn rectangles needs S (the local slice) and device tensors")
+        else:
+            rects = np.ascontiguousarray(rects, dtype=np.int16)
+            S = rects.size // (B * 16)
         N = B * S
         yh, yp = _host(y, np.int64)
         th, tp = _host(crit_targeted, np.uint8)
@@ -352,7 +359,7 @@ class Engine:
         else:
             a.x, a.mask, a.pattern = _dev_ptr(x), _dev_ptr(mask), _dev_ptr(pattern)
             a.grad_adv = _dev_ptr(grad_adv)
-        a.rects_host = rects.ctypes.data
+        a.rects_host = None if drawn else rects.ctypes.data
         a.y_host, a.targeted_host = yp, tp
         a.confidence, a.eps = float(confidence), float(eps)
         a.loss_adv_host = res["loss_adv"].ctypes.data
@@ -368,7 +375,8 @@ class Engine:
         self._live = (rects, yh, th, res, xf)
         if host:
             return a, res
-        _lib.check(self.lib.dp_attack_grad(self.handle, C.byref(a), self._stream()))
+        fn = self.lib.dp_attack_grad_drawn if drawn else self.lib.dp_attack_grad
+        _lib.check(fn(self.handle, C.byref(a), self._stream()))
         return res
 
     def _update_args(self, x, mask, pattern, grad_adv, lr, structured, coeff_gl, density, stage, clip_min,
@@ -433,6 +441,50 @@ class Engine:
         cnt = np.empty(B, np.int32)
         _lib.check(self.lib.dp_failed_set_update(self.handle, B, S, ip, np_, ap, lp, float(thresh), C.c_void_p(cnt.ctypes.data), self._stream()))
         return cnt
+
+    def failed_update_drawn(self, B, S, active, loss=None, thresh=0.1):
+        """failed_update on the last eot_draw's indices, which stay on the device; returns the set sizes [B]."""
+        ac, ap = _host(active, np.uint8)
+        lp = None
+        if loss is not None:
+            loss, lp = _host(np.asarray(loss).reshape(B * S), np.float32)
+        cnt = np.empty(B, np.int32)
+        _lib.check(self.lib.dp_failed_set_update_drawn(self.handle, int(B), int(S), ap, lp, float(thresh),
+                                                       C.c_void_p(cnt.ctypes.data), self._stream()))
+        return cnt
+
+    # ------------------------------------------------------------------------------
+    # on-device EOT draw (DorPatch.generate(eot_sampler="device"))
+    def eot_universe(self, table):
+        """Upload the universe's rectangle table [n_mask, k, 4] int16 (masks.universe) that eot_draw samples from."""
+        t, tp = _host(table, np.int16)
+        if t.ndim != 3 or t.shape[2] != 4:
+            raise ValueError("eot_universe: the table must be [n_mask, k, 4], got %s" % (t.shape,))
+        _lib.check(self.lib.dp_eot_universe_upload(self.handle, tp, int(t.shape[0]), int(t.shape[1]), self._stream()))
+
+    def eot_draw(self, seeds, stage, i, active, S, dual=False, rank=0, world=1, host=False):
+        """Draw step (stage, i)'s EOT samples of every active image on the device (dp_eot_draw), for the next
+        attack_grad(rects=None) and failed_update_drawn.  seeds: [B] per-image seeds.  host=True returns host copies
+        (idx [B,S], idx2 [B,S] or None, nff [B]); rows of inactive images hold whatever the device rows held."""
+        sd, sp = _host(np.array([int(v) % 2 ** 64 for v in seeds], dtype=np.uint64), np.uint64)
+        B = sd.size
+        ac, ap = _host(active, np.uint8)
+        if ac.size != B:
+            raise ValueError("eot_draw: %d seeds but %d active flags" % (B, ac.size))
+        out = [None, None, None]
+        ptrs = [None, None, None]
+        if host:
+            out = [np.zeros((B, S), np.int32), np.zeros((B, S), np.int32) if dual else None, np.zeros(B, np.int32)]
+            ptrs = [None if o is None else C.c_void_p(o.ctypes.data) for o in out]
+        _lib.check(self.lib.dp_eot_draw(self.handle, B, int(S), sp, int(stage), int(i), ap, 1 if dual else 0, int(rank),
+                                        int(world), ptrs[0], ptrs[1], ptrs[2], self._stream()))
+        return tuple(out) if host else None
+
+    def eot_draw_rects(self, n):
+        """Host copy of the last eot_draw's rectangles, [n = B * S/world, 4, 4] int16."""
+        out = np.empty((n, 4, 4), np.int16)
+        _lib.check(self.lib.dp_eot_draw_rects(self.handle, C.c_void_p(out.ctypes.data), int(n), self._stream()))
+        return out
 
     def failed_read(self, b):
         out = np.empty(self.failed_masks, np.int32)

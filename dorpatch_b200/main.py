@@ -3,7 +3,7 @@
 
 Flags added here (all excluded from the result-directory name so layouts stay compatible):
 --synthetic N, --random_init, --max_iterations, --sampling_size, --num_batches, --precision,
---chunk, --img_size, --seed, --pc_n_patch, --attack_pc_n_patch, --basic_unit.
+--chunk, --img_size, --seed, --pc_n_patch, --attack_pc_n_patch, --basic_unit, --eot_sampler.
 
 --pc_n_patch 2 evaluates against the two-patch PatchCleanser (MaskWindow(img, r, 2), reference
 defenses/PatchCleanser.py:34-37).  It does not change the generated patches, so a run on an existing
@@ -16,6 +16,10 @@ two-patch run never resumes from, or overwrites, one-patch patches.  The usual r
 --basic_unit N (default 7, the reference's) sets the side of the square cells the group lasso and patch_selection work
 on (DorPatch.generate(basic_unit=N)); it must divide the image size.  It changes the patches and the stage-0 mask, so a
 non-default unit is also appended to the first path component (`__basic_unit=N`).
+
+--eot_sampler device draws generate()'s EOT occlusions on the GPU (DorPatch.generate(eot_sampler="device")): seeded and
+reproducible, but not numpy's stream, so the patches differ from a host-sampler run.  It is appended to the first path
+component (`__eot_sampler=device`), so such a run has its own results and stage-0 cache.
 
 Under torchrun the PatchCleanser evaluation is sharded too (PatchCleanser(..., shard=True)): each rank forwards a share of
 every robust_predict call and the labels are gathered, so every rank holds the single-process records and rank 0 writes them (DESIGN section 5).
@@ -72,6 +76,9 @@ parser.add_argument('--attack_pc_n_patch', default=1, type=int, choices=[1, 2],
                     help='patches of the PatchCleanser window the EOT occlusions are drawn from (2: result path suffix)')
 parser.add_argument('--basic_unit', default=7, type=int,
                     help='side of the group-lasso / patch-selection cells, dividing the image size (non-7: path suffix)')
+parser.add_argument('--eot_sampler', default='host', choices=['host', 'device'],
+                    help="where generate() draws the EOT occlusions: 'host' (numpy, the reference's stream) or 'device' "
+                         "(seeded counter-based draws on the GPU; non-host: path suffix)")
 
 
 def _init_distributed():
@@ -159,7 +166,7 @@ def main(args):
                     y=target if args.targeted else None, lr=args.lr, num_patch=args.num_patch, dropout=args.dropout,
                     density=args.density, structured=args.structured, save_dir=result_dir, batch_id=i,
                     eps=args.epsilon, max_iterations=args.max_iterations, sampling_size=args.sampling_size,
-                    pc_n_patch=args.attack_pc_n_patch, basic_unit=args.basic_unit)
+                    pc_n_patch=args.attack_pc_n_patch, basic_unit=args.basic_unit, eot_sampler=args.eot_sampler)
                 if rank == 0:                     # every rank holds the identical result; one writer
                     torch.save(adv_mask, os.path.join(result_dir, "adv_mask_%d.pt" % i))
                     torch.save(adv_pattern, os.path.join(result_dir, "adv_pattern_%d.pt" % i))

@@ -32,7 +32,7 @@ def set_random_seed(seed=1234):
 # flags added by this implementation; excluded from the result path so that directory
 # layouts (and therefore resume) stay compatible with the reference's
 EXTRA_FLAGS = ("synthetic", "random_init", "max_iterations", "sampling_size", "num_batches",
-               "precision", "chunk", "img_size", "seed", "pc_n_patch", "attack_pc_n_patch", "basic_unit")
+               "precision", "chunk", "img_size", "seed", "pc_n_patch", "attack_pc_n_patch", "basic_unit", "eot_sampler")
 
 
 # extra flags that change WHAT is computed (and therefore the artefacts a later run would resume from), with the
@@ -40,7 +40,8 @@ EXTRA_FLAGS = ("synthetic", "random_init", "max_iterations", "sampling_size", "n
 # synthetic / random-init / truncated run can never be resumed as (or shadow) a real one.  precision / chunk /
 # num_batches do not change the artefacts' meaning and stay out of the path.
 ARTEFACT_FLAGS = (("synthetic", 0), ("random_init", False), ("max_iterations", 5000), ("sampling_size", 128),
-                  ("img_size", 224), ("seed", 0), ("attack_pc_n_patch", 1), ("basic_unit", 7))
+                  ("img_size", 224), ("seed", 0), ("attack_pc_n_patch", 1), ("basic_unit", 7),
+                  ("eot_sampler", "host"))
 
 
 def generate_saving_path(configs):

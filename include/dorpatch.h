@@ -275,6 +275,38 @@ int32_t dp_failed_set_update(dp_engine* e, int32_t B, int32_t S, const int32_t* 
                              void* stream);
 int32_t dp_failed_set_read(dp_engine* e, int32_t b, int32_t* idx_host_out, int32_t cap, int32_t* n_out, void* stream);
 
+/* ---- on-device EOT draw (DorPatch.generate(eot_sampler="device")) ------------------------------------------------
+ * The sampling of attack.py:193-218 on the device, from a counter-based generator instead of numpy's stream: a step's
+ * indices, the rectangles built from them and the failed-set update never leave the device.
+ * dp_eot_universe_upload: the universe's rectangle table [n_mask][k][4] int16 (k <= 4; k <= 2 for a dual draw),
+ *   copied into the engine.  A new upload invalidates the last draw.
+ * dp_eot_draw: for every image b with active_host[b] (the others are left untouched), at step (stage, iter): n_ff[b] =
+ *   iter >= 1000 ? min(|F_b|, S/2) : 0 distinct members of the image's failed set F_b (its bitmap's set bits below n_mask),
+ *   then S - n_ff[b] distinct universe indices drawn independently of them; with dual a second, independent draw of
+ *   the same form (rectangle slots 2-3).  Exact sampling without replacement in uniformly random order, every random
+ *   number Philox4x32-10 keyed by seeds_host[b] (uint64) at a counter of (stage, iter, draw, position): the result
+ *   depends on nothing else -- not on B, the other images, the rank or the launch.  The samples [rank * S/world,
+ *   (rank + 1) * S/world) of every image are gathered from the table into the rectangles dp_attack_grad_drawn reads
+ *   (masks.gather's layout).  idx_host_out [B*S], idx2_host_out [B*S] (dual only) and nff_host_out [B] receive host
+ *   copies when not NULL (then the call synchronises).  Refused: no universe, S > n_mask, a universe larger than the
+ *   failed-set bitmaps (dp_failed_set_reset), dual with k > 2, a rank outside the world or S not divisible by it.
+ * dp_eot_draw_rects: host copy of the last draw's rectangles [B * S/world][4][4] (n = B * S/world).
+ * dp_attack_grad_drawn: dp_attack_grad with the last draw's rectangles (a->rects_host must be NULL; S = the local
+ *   slice, S_total = the draw's S; xform_host is accepted).  Its step replays one CUDA graph per shape like
+ *   dp_attack_grad's.
+ * dp_failed_set_update_drawn: dp_failed_set_update with the last draw's idx / n_ff (S = the draw's S), on the device.
+ *   It uses the draw up: a draw serves one step, and dp_attack_grad_drawn or a second update without a new draw is
+ *   refused as stale (as is any use after a universe upload or dp_failed_set_reset).
+ * Added without changing any other entry point: the ABI stays 9. */
+int32_t dp_eot_universe_upload(dp_engine* e, const int16_t* table_host, int32_t n_mask, int32_t k, void* stream);
+int32_t dp_eot_draw(dp_engine* e, int32_t B, int32_t S, const uint64_t* seeds_host, int32_t stage, int32_t iter,
+                    const uint8_t* active_host, int32_t dual, int32_t rank, int32_t world, int32_t* idx_host_out,
+                    int32_t* idx2_host_out, int32_t* nff_host_out, void* stream);
+int32_t dp_eot_draw_rects(dp_engine* e, int16_t* rects_host_out, int32_t n, void* stream);
+int32_t dp_attack_grad_drawn(dp_engine* e, const dp_attack_args* a, void* stream);
+int32_t dp_failed_set_update_drawn(dp_engine* e, int32_t B, int32_t S, const uint8_t* active_host, const float* loss_host,
+                                   float thresh, int32_t* count_host, void* stream);
+
 /* Op-level hooks for the parity tests (tests/test_gpu_ops.py); not part of the reference-facing surface.
  * dp_debug_stem_bwd_reduce: the bf16 engine's fused stem-dgrad + masked EOT reduce (K1^T as the bench runs it) on a
  *   caller-supplied dY [B*S, H/2, H/2, 64] bf16 dev: G[B,3,H,W] = 2 * sum_s keep_s * conv7x7s2^T(dY_s, W_stem).
