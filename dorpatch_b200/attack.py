@@ -25,8 +25,15 @@ Semantics beyond the reference (see DESIGN.md):
   * ``eot_sampler="device"`` draws the EOT occlusions on the GPU (dp_eot_draw): the rule of attack.py:193-218 from a
     counter-based generator seeded per image, so the draws are reproducible but not numpy's; indices, rectangles and the
     failed-set update never leave the device.
+  * ``checkpoint=<path>`` saves everything the loop carries from one step to the next every ``checkpoint_every`` steps
+    and at each stage boundary; a later call with the same arguments continues from the file as the uninterrupted call
+    would have (the reference resumes only at the stage-0 cache and main.py's per-batch artefacts).
 """
+import hashlib
+import io
 import os
+import sys
+import tempfile
 
 import numpy as np
 import torch
@@ -155,6 +162,24 @@ class _ImageState(object):
             self.not_decay = 0
         return improved, bool(self.lr < np.float32(1e-3))
 
+    def state(self):
+        """Everything generate() carries from one step to the next for this image, as plain values (a checkpoint's)."""
+        failed = self.dev[0].failed_read(self.dev[1]) if self.dev is not None else self.failed
+        return dict(lr=float(self.lr), loss_best=float(self.loss_best), not_decay=int(self.not_decay),
+                    num_failure=float(self.num_failure) if np.isinf(self.num_failure) else int(self.num_failure),
+                    coeff_group_lasso=float(self.coeff_group_lasso), structured=float(self.structured), y=int(self.y),
+                    targeted=bool(self.targeted), crit_targeted=bool(self.crit_targeted),
+                    certifiable=bool(self.certifiable), active=bool(self.active), n_failed=int(self.n_failed),
+                    failed=torch.tensor(np.asarray(failed, np.int32).reshape(-1)))
+
+    def load_state(self, d):
+        """Inverse of state(): the failed set goes back to the device when it lives there."""
+        self.set_failed(d["failed"].tolist())
+        self.lr, self.loss_best = np.float32(d["lr"]), np.float32(d["loss_best"])
+        for k in ("not_decay", "num_failure", "coeff_group_lasso", "structured", "y", "targeted", "crit_targeted",
+                  "certifiable", "active", "n_failed"):
+            setattr(self, k, d[k])
+
 
 def _may_prefetch(states, i, max_iterations):
     """May step i+1's samples be drawn before step i's bookkeeping without changing the reference's RNG consumption?
@@ -187,7 +212,8 @@ def _dist():
     return None
 
 
-def _assert_same_on_all_ranks(dist, arr, device, what):
+def _assert_same_on_all_ranks(dist, arr, device, what,
+                              hint="seed every rank identically (utils.set_random_seed) before generate()"):
     """Cheap consistency check of host-side state that EOT sharding assumes identical on every rank."""
     a = np.ascontiguousarray(arr).astype(np.int64).ravel()
     chk = torch.tensor([int(a.sum()), int((a * (np.arange(a.size) % 8191 + 1)).sum())], dtype=torch.int64, device=device)
@@ -195,7 +221,7 @@ def _assert_same_on_all_ranks(dist, arr, device, what):
     dist.all_reduce(lo, op=dist.ReduceOp.MIN)
     dist.all_reduce(hi, op=dist.ReduceOp.MAX)
     if not torch.equal(lo, hi):
-        raise RuntimeError("ranks disagree on %s: seed every rank identically (utils.set_random_seed) before generate()" % what)
+        raise RuntimeError("ranks disagree on %s: %s" % (what, hint))
 
 
 def exchange_shards(dist, G, loss_adv, preds, defer=False):
@@ -315,6 +341,121 @@ def scan_failures(predict, all_rects, y, targeted, dist=None, device="cpu", inv=
     return np.nonzero(f)[0].tolist()
 
 
+# ----------------------------------------------------------------------------------------
+# step-level checkpoints of generate()
+CHECKPOINT_VERSION = 1
+
+
+def checkpoint_fingerprint(x, y, world, precision, **kw):
+    """What a checkpoint must have been written by: the image batch (shape and a content hash), the effective labels,
+    every keyword that changes the computation (`kw`, in a fixed order), the world size and the engine precision.
+    A list of (field, value) pairs of plain Python values, so the first differing field can be named."""
+    xb = x.detach().float().contiguous().cpu().numpy()
+    fp = [("x_shape", list(xb.shape)), ("x_sha256", hashlib.sha256(xb.tobytes()).hexdigest()),
+          ("y", [int(v) for v in y])]
+    for k in sorted(kw):
+        v = kw[k]
+        if isinstance(v, (list, tuple, np.ndarray)):
+            v = [int(s) for s in v]
+        elif isinstance(v, (bool, np.bool_)):
+            v = bool(v)
+        elif isinstance(v, (int, np.integer)):
+            v = int(v)
+        elif isinstance(v, (float, np.floating)):
+            v = float(v)
+        fp.append((k, v))
+    fp += [("world_size", int(world)), ("precision", str(precision))]
+    return fp
+
+
+def rng_state_out(rs):
+    """A numpy RandomState's (or the legacy global stream's) state as values torch.load(weights_only=True) reads back."""
+    name, keys, pos, has_gauss, cached = rs.get_state()
+    return [name, torch.from_numpy(keys.astype(np.int64)), int(pos), int(has_gauss), float(cached)]
+
+
+def rng_state_in(rs, state):
+    name, keys, pos, has_gauss, cached = state
+    rs.set_state((name, keys.numpy().astype(np.uint32), pos, has_gauss, cached))
+
+
+def save_checkpoint(path, ckpt):
+    """Replace `path` by `ckpt` atomically: write a temporary file in the same directory, flush and fsync it, then
+    os.replace it over the old one, so a process killed mid-write leaves the previous checkpoint intact."""
+    d = os.path.dirname(os.path.abspath(path))
+    fd, tmp = tempfile.mkstemp(prefix=os.path.basename(path) + ".", suffix=".tmp", dir=d)
+    try:
+        with os.fdopen(fd, "wb") as f:
+            torch.save(ckpt, f)
+            f.flush()
+            os.fsync(f.fileno())
+        os.replace(tmp, path)
+    except BaseException:
+        if os.path.exists(tmp):
+            os.unlink(tmp)
+        raise
+    dfd = os.open(d, os.O_RDONLY)                            # make the rename itself durable
+    try:
+        os.fsync(dfd)
+    finally:
+        os.close(dfd)
+
+
+def load_checkpoint(path, fingerprint):
+    """Read a checkpoint written by save_checkpoint and check that it belongs to the call whose fingerprint is given:
+    ValueError naming the format version or the first field that differs.  Returns (checkpoint, digest of the file's
+    bytes as uint16 words)."""
+    with open(path, "rb") as f:
+        raw = f.read()
+    ck = torch.load(io.BytesIO(raw), map_location="cpu", weights_only=True)
+    if not isinstance(ck, dict) or ck.get("version") != CHECKPOINT_VERSION:
+        raise ValueError("checkpoint %s: format version %r, this code reads version %d"
+                         % (path, ck.get("version") if isinstance(ck, dict) else None, CHECKPOINT_VERSION))
+    saved = dict((k, v) for k, v in ck["fingerprint"])
+    for k, v in fingerprint:
+        if k not in saved or saved[k] != v:
+            raise ValueError("checkpoint %s was written by a different call: %s differs (checkpoint: %r, this call: %r)"
+                             % (path, k, saved.get(k, "<missing>"), v))
+    if len(saved) != len(fingerprint):
+        extra = sorted(set(saved) - set(k for k, _ in fingerprint))
+        raise ValueError("checkpoint %s was written by a different call: %s differs" % (path, extra[0]))
+    return ck, np.frombuffer(hashlib.sha256(raw).digest(), np.uint16)
+
+
+_SHARED = "every rank must read the same checkpoint file: keep it in a directory all ranks share"
+
+
+def read_checkpoint(path, fingerprint, dist=None, device="cpu"):
+    """The validated checkpoint at `path`, or None if there is none.  Under torch.distributed every rank reads the file
+    and the ranks check that they agree on whether it exists and on its contents."""
+    exists = os.path.exists(path)
+    if dist:
+        _assert_same_on_all_ranks(dist, [int(exists)], device, "whether %s exists" % path, _SHARED)
+    if not exists:
+        return None
+    ck, digest = load_checkpoint(path, fingerprint)
+    if dist:
+        _assert_same_on_all_ranks(dist, digest, device, "the contents of %s" % path, _SHARED)
+    return ck
+
+
+def write_checkpoint(path, make, dist=None):
+    """save_checkpoint(path, make()) on rank 0 alone (every rank holds the same state); the other ranks wait at a barrier
+    until the file is in place."""
+    if dist is None or dist.get_rank() == 0:
+        save_checkpoint(path, make())
+    if dist:
+        dist.barrier()
+
+
+def remove_checkpoint(path, dist=None):
+    """Delete the checkpoint of a finished call (rank 0), so that a later call with the same path starts fresh."""
+    if (dist is None or dist.get_rank() == 0) and os.path.exists(path):
+        os.remove(path)
+    if dist:
+        dist.barrier()
+
+
 class DorPatch(object):
     def __init__(self):
         self.last_stats = {}
@@ -323,7 +464,8 @@ class DorPatch(object):
     def generate(self, model, x, patch_budget, n_classes, save_dir, batch_id, y=None, targeted=False,
                  lr=1e-2, confidence=1e-1, clip_min=0, clip_max=1, max_iterations=5000, basic_unit=7,
                  selection='topk', dropout=2, sampling_size=128, density=1e-3, structured=1e-3, eps=4., dual=False,
-                 eot_affine=0.0, eot_colour=0.0, eot_seed=0, pc_n_patch=1, eot_sampler="host", **kwargs):
+                 eot_affine=0.0, eot_colour=0.0, eot_seed=0, pc_n_patch=1, eot_sampler="host", checkpoint=None,
+                 checkpoint_every=100, **kwargs):
         """Reference signature (attack.py:51-53) plus three opt-in keywords for the affine / colour
         EOT extension (default 0 = off = the reference's behaviour).  `image_seeds=[s_0..s_{B-1}]` (keyword)
         makes row b of a B > 1 call replay the B == 1 run seeded with s_b (SURVEY section 0: parity of the
@@ -334,7 +476,16 @@ class DorPatch(object):
         `eot_sampler="device"` draws every step's EOT occlusions on the GPU (dp_eot_draw) instead of with numpy on the
         host (`"host"`, the default and the reference's stream): the indices, their rectangles and the failed-set update
         stay on the device, so a long run is paced by the GPU.  The draws are reproducible from per-image seeds --
-        `image_seeds[b]`, else B seeds drawn once from the global numpy stream -- but are not numpy's."""
+        `image_seeds[b]`, else B seeds drawn once from the global numpy stream -- but are not numpy's.
+        `checkpoint=<path>` makes the call resumable: if the file exists, the call continues from the step it records
+        (ValueError if it was written by a call with other inputs, keywords, world size or precision); while running it
+        rewrites the file atomically after every `checkpoint_every`-th step of a stage and at the stage boundary, and
+        deletes it on return.  The resumed call returns, prints from the resumed step on, and leaves the global numpy
+        and torch RNG states as the uninterrupted call would have (bit for bit with the fp32 engine, or with any
+        precision under DORPATCH_AUTOTUNE=0, without affine / colour EOT).  None (the default) reads and writes nothing."""
+        if checkpoint is not None and (isinstance(checkpoint_every, bool) or
+                                       not isinstance(checkpoint_every, (int, np.integer)) or checkpoint_every < 1):
+            raise ValueError("checkpoint_every=%r must be a positive integer" % (checkpoint_every,))
         if eot_sampler not in ("host", "device"):
             raise ValueError("eot_sampler=%r: 'host' or 'device'" % (eot_sampler,))
         on_device = eot_sampler == "device"
@@ -460,34 +611,85 @@ class DorPatch(object):
             sl = slice(rank * S_loc, (rank + 1) * S_loc)
             return idx, idx2, nff, _masks.gather(table, idx[:, sl], idx2[:, sl] if dual else None)
 
+        start_stage, start_i = 0, 0
+        adv_x_prev = None
+        if checkpoint is not None:
+            fingerprint = checkpoint_fingerprint(
+                x, y, world, eng.precision, patch_budget=patch_budget, targeted=targeted, lr=lr, confidence=confidence,
+                clip_min=clip_min, clip_max=clip_max, max_iterations=max_iterations, basic_unit=basic_unit,
+                selection=selection, dropout=dropout, sampling_size=sampling_size, density=density,
+                structured=structured, eps=eps, dual=dual, eot_affine=eot_affine, eot_colour=eot_colour,
+                eot_seed=eot_seed, pc_n_patch=pc_n_patch, eot_sampler=eot_sampler, image_seeds=image_seeds)
+            ck = read_checkpoint(checkpoint, fingerprint, dist, dev)
+            if ck is not None:
+                # the set-up above drew from the RNG streams as a fresh call does; the checkpoint's states replace them
+                cs = ck["state"]
+                start_stage, start_i = int(ck["stage"]), int(ck["i"])
+                for s, d in zip(st, cs["images"]):
+                    s.load_state(d)
+                adv_mask, adv_pattern = cs["adv_mask"].to(dev), cs["adv_pattern"].to(dev)
+                mask_best, pattern_best = cs["mask_best"].to(dev), cs["pattern_best"].to(dev)
+                have_stale = cs["have_stale"]
+                if have_stale:
+                    stale_gp = cs["stale_gp"].to(dev)
+                last_preds = None if cs["last_preds"] is None else cs["last_preds"].numpy()
+                adv_x_prev = None if cs["adv_x_prev"] is None else cs["adv_x_prev"].to(dev)
+                steps = cs["steps"]
+                scans[:] = cs["scans"]
+                if on_device:
+                    seeds[:] = cs["seeds"]
+                for r, rs in zip(rngs, cs["rngs"]):
+                    if rs is not None:
+                        rng_state_in(r, rs)
+                rng_state_in(eot_rng, cs["eot_rng"])
+                rng_state_in(np.random, cs["np_global"])
+                torch.set_rng_state(cs["torch_cpu"])
+                sys.stderr.write(">> resuming from %s at stage %d, iteration %d\n" % (checkpoint, start_stage, start_i))
+
+        def snapshot(next_stage, next_i):                        # the loop's state at a step boundary (stage, i) -> next
+            cpu = lambda t: None if t is None else t.detach().cpu()    # noqa: E731
+            state = dict(
+                images=[s.state() for s in st], adv_mask=cpu(adv_mask), adv_pattern=cpu(adv_pattern),
+                mask_best=cpu(mask_best), pattern_best=cpu(pattern_best), have_stale=bool(have_stale),
+                stale_gp=cpu(stale_gp) if have_stale else None, adv_x_prev=cpu(adv_x_prev),
+                last_preds=None if last_preds is None else torch.from_numpy(np.ascontiguousarray(last_preds)),
+                steps=int(steps), scans=[int(v) for v in scans], seeds=list(seeds) if on_device else None,
+                rngs=[None if r is None or r is np.random else rng_state_out(r) for r in rngs],
+                eot_rng=rng_state_out(eot_rng), np_global=rng_state_out(np.random), torch_cpu=torch.get_rng_state())
+            return dict(version=CHECKPOINT_VERSION, fingerprint=fingerprint, stage=int(next_stage), i=int(next_i),
+                        state=state)
+
         from concurrent.futures import ThreadPoolExecutor
         sampler = ThreadPoolExecutor(max_workers=1)
         prefetched = None
 
-        for stage in range(2):
-            print('============= Stage %d =============' % stage)
-            for s in st:
-                s.reset()
-            if stage == 0 and dir_0 and os.path.exists(os.path.join(dir_0, "adv_mask_%d.pt" % batch_id)):
-                mask_best = torch.load(os.path.join(dir_0, "adv_mask_%d.pt" % batch_id)).to(dev)
-                pattern_best = torch.load(os.path.join(dir_0, "adv_pattern_%d.pt" % batch_id)).to(dev)
-                continue
-            if stage == 1:                                       # attack.py:143-165
-                adv_x, _, _ = eng.paste(x, mask_best, pattern_best, eps)
-                if any(not s.targeted for s in st):
-                    p1 = eng.predict(adv_x)
-                    for b, s in enumerate(st):
-                        if not s.targeted:
-                            s.targeted = True
-                            s.y, sw = _pick_target(p1[b:b + 1], s.y)
-                            s.crit_targeted = s.crit_targeted or sw
-                pattern_best = adv_x.clone()
-                torch.nn.Conv2d(1, 1, basic_unit, stride=basic_unit, bias=False)   # attack.py:365 RNG draw
-                adv_mask = self.patch_selection(mask_best, patch_budget, basic_unit, selection)
-                mask_best = adv_mask.clone()
-                adv_pattern = pattern_best.clone()
-            adv_x = adv_x_prev = None
-            for i in range(max_iterations):
+        for stage in range(start_stage, 2):
+            first = start_i if stage == start_stage else 0       # > 0: resumed inside the stage, its start already ran
+            if first == 0:
+                print('============= Stage %d =============' % stage)
+                for s in st:
+                    s.reset()
+                if stage == 0 and dir_0 and os.path.exists(os.path.join(dir_0, "adv_mask_%d.pt" % batch_id)):
+                    mask_best = torch.load(os.path.join(dir_0, "adv_mask_%d.pt" % batch_id)).to(dev)
+                    pattern_best = torch.load(os.path.join(dir_0, "adv_pattern_%d.pt" % batch_id)).to(dev)
+                    continue
+                if stage == 1:                                   # attack.py:143-165
+                    adv_x, _, _ = eng.paste(x, mask_best, pattern_best, eps)
+                    if any(not s.targeted for s in st):
+                        p1 = eng.predict(adv_x)
+                        for b, s in enumerate(st):
+                            if not s.targeted:
+                                s.targeted = True
+                                s.y, sw = _pick_target(p1[b:b + 1], s.y)
+                                s.crit_targeted = s.crit_targeted or sw
+                    pattern_best = adv_x.clone()
+                    torch.nn.Conv2d(1, 1, basic_unit, stride=basic_unit, bias=False)   # attack.py:365 RNG draw
+                    adv_mask = self.patch_selection(mask_best, patch_budget, basic_unit, selection)
+                    mask_best = adv_mask.clone()
+                    adv_pattern = pattern_best.clone()
+                adv_x_prev = None
+            adv_x = None
+            for i in range(first, max_iterations):
                 if stage == 0 and i == 500:                      # attack.py:169-182
                     for b, s in enumerate(st):
                         if s.targeted or not s.active:
@@ -515,8 +717,10 @@ class DorPatch(object):
                 # Draw step i+1's samples on a helper thread while the GPU runs step i -- only where the reference's RNG
                 # consumption is provably unchanged: the draw depends on nothing this step can alter (i+1 < 1000: no
                 # failed-set samples), the stage does run an iteration i+1, and no image can stop at step i (a stop needs
-                # lr * 0.1 < 1e-3 together with a plateau, i.e. not_decay >= PATIENCE before the step).
-                if not on_device and _may_prefetch(st, i, max_iterations):
+                # lr * 0.1 < 1e-3 together with a plateau, i.e. not_decay >= PATIENCE before the step).  Not before a
+                # checkpoint either: the RNG states it saves must not hold step i+1's draw yet.
+                ckpt_after = checkpoint is not None and (i + 1) % checkpoint_every == 0 and i + 1 < max_iterations
+                if not on_device and not ckpt_after and _may_prefetch(st, i, max_iterations):
                     prefetched = ((stage, i + 1), sampler.submit(draw, i + 1))
                 if dist and i % 100 == 0:
                     # every rank must have drawn the same indices (same RNG streams): a diverged rank would evaluate a
@@ -594,6 +798,8 @@ class DorPatch(object):
                 bias = stale_gp if (stage == 1 and i == 0 and have_stale) else None
                 eng.attack_update(x, adv_mask, adv_pattern, G, lr_used, structured_used, coeff_used, density, stage,
                                   clip_min, clip_max, grad_pattern_bias=bias)   # attack.py:332-342
+                if ckpt_after:
+                    write_checkpoint(checkpoint, lambda: snapshot(stage, i + 1), dist)
             for b, s in enumerate(st):                           # attack.py:344-346
                 if s.active and np.isinf(s.loss_best):
                     mask_best[b].copy_(adv_mask[b])
@@ -607,7 +813,11 @@ class DorPatch(object):
                     if not s.targeted and last_preds is not None:
                         s.y, sw = _pick_target(last_preds[b], s.y)
                         s.crit_targeted = s.crit_targeted or sw
+                if checkpoint is not None:                       # after the end-of-stage work, which must not rerun
+                    write_checkpoint(checkpoint, lambda: snapshot(1, 0), dist)
         sampler.shutdown(wait=True)
+        if checkpoint is not None:
+            remove_checkpoint(checkpoint, dist)
         self.last_stats = dict(steps=steps, samples_per_step=B * S, final_labels=[s.y for s in st],
                                scans=scans[0], scan_forwards=scans[1])
         return mask_best, pattern_best

@@ -3,7 +3,7 @@
 
 Flags added here (all excluded from the result-directory name so layouts stay compatible):
 --synthetic N, --random_init, --max_iterations, --sampling_size, --num_batches, --precision,
---chunk, --img_size, --seed, --pc_n_patch, --attack_pc_n_patch, --basic_unit, --eot_sampler.
+--chunk, --img_size, --seed, --pc_n_patch, --attack_pc_n_patch, --basic_unit, --eot_sampler, --checkpoint_every.
 
 --pc_n_patch 2 evaluates against the two-patch PatchCleanser (MaskWindow(img, r, 2), reference
 defenses/PatchCleanser.py:34-37).  It does not change the generated patches, so a run on an existing
@@ -20,6 +20,12 @@ non-default unit is also appended to the first path component (`__basic_unit=N`)
 --eot_sampler device draws generate()'s EOT occlusions on the GPU (DorPatch.generate(eot_sampler="device")): seeded and
 reproducible, but not numpy's stream, so the patches differ from a host-sampler run.  It is appended to the first path
 component (`__eot_sampler=device`), so such a run has its own results and stage-0 cache.
+
+--checkpoint_every N (default 0: off) makes every batch's generate() resumable: batch i keeps its state in
+<result_dir>/adv_ckpt_<i>.pt every N steps (DorPatch.generate(checkpoint=..., checkpoint_every=N)).  A rerun with the same
+flags skips the finished batches, continues the interrupted one from its checkpoint and, since the checkpoint restores the
+RNG streams, computes what the uninterrupted run would have.  It changes nothing that is computed, so it stays out of the
+result path.
 
 Under torchrun the PatchCleanser evaluation is sharded too (PatchCleanser(..., shard=True)): each rank forwards a share of
 every robust_predict call and the labels are gathered, so every rank holds the single-process records and rank 0 writes them (DESIGN section 5).
@@ -79,6 +85,9 @@ parser.add_argument('--basic_unit', default=7, type=int,
 parser.add_argument('--eot_sampler', default='host', choices=['host', 'device'],
                     help="where generate() draws the EOT occlusions: 'host' (numpy, the reference's stream) or 'device' "
                          "(seeded counter-based draws on the GPU; non-host: path suffix)")
+parser.add_argument('--checkpoint_every', default=0, type=int,
+                    help='resumable generation: save each batch\'s attack state to <result_dir>/adv_ckpt_<i>.pt every N '
+                         'steps (0: off)')
 
 
 def _init_distributed():
@@ -166,7 +175,9 @@ def main(args):
                     y=target if args.targeted else None, lr=args.lr, num_patch=args.num_patch, dropout=args.dropout,
                     density=args.density, structured=args.structured, save_dir=result_dir, batch_id=i,
                     eps=args.epsilon, max_iterations=args.max_iterations, sampling_size=args.sampling_size,
-                    pc_n_patch=args.attack_pc_n_patch, basic_unit=args.basic_unit, eot_sampler=args.eot_sampler)
+                    pc_n_patch=args.attack_pc_n_patch, basic_unit=args.basic_unit, eot_sampler=args.eot_sampler,
+                    checkpoint=os.path.join(result_dir, "adv_ckpt_%d.pt" % i) if args.checkpoint_every > 0 else None,
+                    checkpoint_every=args.checkpoint_every)
                 if rank == 0:                     # every rank holds the identical result; one writer
                     torch.save(adv_mask, os.path.join(result_dir, "adv_mask_%d.pt" % i))
                     torch.save(adv_pattern, os.path.join(result_dir, "adv_pattern_%d.pt" % i))

@@ -32,7 +32,8 @@ def set_random_seed(seed=1234):
 # flags added by this implementation; excluded from the result path so that directory
 # layouts (and therefore resume) stay compatible with the reference's
 EXTRA_FLAGS = ("synthetic", "random_init", "max_iterations", "sampling_size", "num_batches",
-               "precision", "chunk", "img_size", "seed", "pc_n_patch", "attack_pc_n_patch", "basic_unit", "eot_sampler")
+               "precision", "chunk", "img_size", "seed", "pc_n_patch", "attack_pc_n_patch", "basic_unit", "eot_sampler",
+               "checkpoint_every")
 
 
 # extra flags that change WHAT is computed (and therefore the artefacts a later run would resume from), with the
